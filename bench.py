@@ -13,6 +13,7 @@ kNN search + graph assembly are outside the step (the reference rebuilds the gra
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched under torchrun)
   python bench.py --impl reference ...                     (CPU arm: oracle port on host cores)
+  python bench.py ... --dump-outputs DIR                   (also write the last timed step's outputs as DIR/<name>.npy)
 
 Prints ONE JSON line (see the repository README / DESIGN.md for the field definitions).
 """
@@ -44,7 +45,8 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_tflops_sustained=d.get("bf16_tflops_sustained"),
                     source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=None, source="H100 SXM data sheet")
 
 
 # ------------------------------------------------------------------------------------ synthetic data
@@ -267,6 +269,8 @@ def main():
                     help="collectives of the data path under N > 1: torch.distributed (NCCL) or the C-ABI's own NCCL communicator (b2_comm_*)")
     ap.add_argument("--no-checks", action="store_true", help="skip the fp64 spot checks and the 16-bit aggregate side measurement")
     ap.add_argument("--cuda-profiler", action="store_true", help="bracket the timed region with cudaProfilerStart/Stop (for ncu --profile-from-start off)")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="write what the last timed step computed as DIR/<name>.npy (rank 0; fixed seeded row sample of the embeddings)")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "b200":
         args.warmup = 3
@@ -351,10 +355,12 @@ def main():
         torch.index_select(z_all, 0, perm, out=z_perm)      # one 0.5 GB gather per step buys L2-resident gathers in 4 aggregates
         return z_perm
 
+    last = {}
+
     def step(x_src):
-        fae.train_epoch(x_src, BATCH, "LTMG", 0.9, None, z_all, None, n_steps=n_steps)
+        last["fae_loss"] = fae.train_epoch(x_src, BATCH, "LTMG", 0.9, None, z_all, None, n_steps=n_steps)
         eps.normal_(generator=gen)
-        gae.train_step(gae_input(), A, labels, norm, pos_weight, eps)
+        last["gae_z"], last["gae_mu"], last["gae_logvar"] = gae.train_step(gae_input(), A, labels, norm, pos_weight, eps)
 
     def timed(fn, k):
         comm.barrier()
@@ -389,6 +395,8 @@ def main():
         torch.cuda.profiler.stop()
     launches = ops.counters()["launches"] - launches_before
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(Path(args.dump_outputs), last, z_all, gae, inv if perm is not None else None)
     ms_per_step = total_ms / args.steps
     value = N / (ms_per_step / 1e3)
 
@@ -420,8 +428,7 @@ def main():
         b16 = A.nnz * 8 + (n_loc + 1) * 4 + N * 32 * 2 + n_loc * 32 * 4
         spmm16 = {"kernel": "spmm_stream_kernel<bf16, 64 B rows> (Â·support, F=32, bf16 operand, fp32 accumulate/output)", "bound": "hbm",
                   "achieved": b16 / (ms16 * 1e-3) / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                  "frac": b16 / (ms16 * 1e-3) / 1e9 / peaks["hbm_gbs"], "traffic": traffic_from_profiles("spmm_stream_kernel<bf16>"),
-                  "ms_per_launch": ms16, "algorithmic_bytes": b16, "l2_policy": "256 MB flush between launches", "peak_source": peaks["source"]}
+                  "frac": b16 / (ms16 * 1e-3) / 1e9 / peaks["hbm_gbs"], "ms_per_launch": ms16, "algorithmic_bytes": b16, "l2_policy": "256 MB flush between launches", "peak_source": peaks["source"]}
         del flush, S16, out
 
     # ---- e2e: the public handlers (numpy in / numpy out), host-resident pinned X, copies inside the timed region ---------------
@@ -529,7 +536,7 @@ def main():
     if spmm_ms:
         ach = spmm_bytes / (spmm_ms * 1e-3) / 1e9
         roof_spmm = {"kernel": "spmm_stream_kernel<f32, 128 B rows> (Â·support, F=32, fp32 operand; nnz-stream pipeline, cp.async-staged gathers)", "bound": "hbm", "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                     "frac": ach / peaks["hbm_gbs"], "traffic": traffic_from_profiles("spmm_stream_kernel<f32>"), "launches": spmm_n, "ms_per_launch": spmm_ms,
+                     "frac": ach / peaks["hbm_gbs"], "launches": spmm_n, "ms_per_launch": spmm_ms,
                      "algorithmic_bytes": spmm_bytes, "gather_bytes_through_l2": nnz_loc * F * 4, "peak_source": peaks["source"]}
     gemm_ms, gemm_n, gemm_total = kt("gemm_f32")
     fae_flops = 6.0 * n_loc * (G * 512 + 512 * 128 + 128 * 512 + 512 * G)       # fwd + dX + dW, 2 flops per MAC
@@ -537,12 +544,12 @@ def main():
     roof_gemm = None
     if gemm_ms:
         ach = (fae_flops + gcn_flops) / (gemm_total * 1e-3) / 1e12
-        roof_gemm = {"kernel": "gemm_tc_kernel (tcgen05 kind::tf32, %s)" % args.precision, "bound": "tensor", "achieved": ach,
+        roof_gemm = {"kernel": "gemm_tc_kernel (wgmma tf32, %s)" % args.precision, "bound": "tensor", "achieved": ach,
                      "peak": peaks["bf16_tflops_sustained"] or peaks["bf16_tflops"], "unit": "TFLOP/s",
-                     "frac": ach / (peaks["bf16_tflops_sustained"] or peaks["bf16_tflops"]), "traffic": traffic_from_profiles("gemm_tc_kernel"), "launches": gemm_n,
+                     "frac": ach / (peaks["bf16_tflops_sustained"] or peaks["bf16_tflops"]), "launches": gemm_n,
                      "ms_total": gemm_total, "algorithmic_flops": fae_flops + gcn_flops, "peak_source": peaks["source"],
                      "note": "achieved = fp32-equivalent algorithmic FLOPs; tf32x3 issues 3 tensor-core products per algorithmic product "
-                             "and kind::tf32 runs at half the bf16 rate, so the ceiling of this mode is peak/6"}
+                             "and tf32 runs at half the bf16 rate, so the ceiling of this mode is peak/6"}
     dec_ms, dec_n, dec_total = kt("gae_loss_grad_f32")
     phases = {k: {"ms": v["ms"], "launches": v["n"]} for k, v in sorted(ktimes.items(), key=lambda kv: -kv[1]["ms"])}
     dominant = max(ktimes.items(), key=lambda kv: kv[1]["ms"])[0] if ktimes else None
@@ -551,17 +558,15 @@ def main():
         # the exact N×N decoder is SFU/issue-bound; report it on the tensor roofline with its matmul flops (2·d per logit, S and G·Z)
         dec_flops = 2.0 * 2 * EMB * float(n_loc) * N
         ach = dec_flops / (dec_total * 1e-3) / 1e12 if dec_total else 0.0
-        roofline = {"kernel": "gae_sym_kernel (matrix-free symmetric z·zᵀ BCE decoder: tcgen05 kind::f16 hi/lo split, S / dZ in TMEM, each "
-                              "unordered 128×128 tile computed once and used for both gradient blocks)",
+        roofline = {"kernel": "gae_allpairs_tc_kernel (matrix-free z·zᵀ BCE decoder: wgmma tf32 hi/lo split, S and G in registers, "
+                              "row sweep over all 128×128 tiles)",
                     "bound": "tensor", "achieved": ach,
                     "peak": peaks["bf16_tflops_sustained"] or peaks["bf16_tflops"], "unit": "TFLOP/s",
-                    "frac": ach / (peaks["bf16_tflops_sustained"] or peaks["bf16_tflops"]), "traffic": traffic_from_profiles("gae_sym_kernel"),
-                    "launches": dec_n, "ms_total": dec_total, "peak_source": peaks["source"],
+                    "frac": ach / (peaks["bf16_tflops_sustained"] or peaks["bf16_tflops"]), "launches": dec_n, "ms_total": dec_total, "peak_source": peaks["source"],
                     "logits_per_s": float(n_loc) * N / (dec_total * 1e-3) if dec_total else None,
                     "note": "dominant kernel of the step; algorithmic flops = the two K=16 products per logit (S and G·Z) over ALL N² ordered "
-                            "pairs (the symmetric kernel evaluates each unordered pair once). Its real ceiling is the per-logit elementwise work "
-                            "(2 MUFU + ~11 ALU instructions per unordered logit), not the tensor pipe or HBM — see DESIGN.md §4.1 and "
-                            "profiles/r02_ncu_gae_sym.md; roofline_spmm / roofline_gemm are the HBM- and tensor-bound kernels"}
+                            "pairs. Its real ceiling is the per-logit elementwise work (2 MUFU + ~11 ALU instructions per logit), not the tensor "
+                            "pipe or HBM; roofline_spmm / roofline_gemm are the HBM- and tensor-bound kernels"}
 
     cpu_baseline, matched = None, None
     if not args.no_cpu_baseline and world == 1:
@@ -578,7 +583,7 @@ def main():
     line = {
         "metric": "cells/sec fwd+bwd scGNN", "value": value, "unit": "cells/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
-        "dtype": "f32 (tcgen05 3xTF32 split GEMMs, fp32 everything else)" if args.precision == "tf32x3" else args.precision,
+        "dtype": "f32 (wgmma 3xTF32 split GEMMs, fp32 everything else)" if args.precision == "tf32x3" else args.precision,
         "data": "synthetic",
         "config": workload_config(args),
         "implementation": {"decoder_loss": "exact-fused-blockwise (matrix-free, no N×N tensors)", "gemm_precision": args.precision,
@@ -593,20 +598,28 @@ def main():
     print(json.dumps(line), flush=True)
 
 
-def traffic_from_profiles(kernel_prefix):
-    """DRAM bytes per launch of a kernel from the committed `ncu --set full` capture summary (profiles/r02_traffic.json:
-    {kernel name prefix: dram__bytes_read.sum + dram__bytes_write.sum}); None when no capture has been committed for it."""
-    p = ROOT / "profiles" / "r02_traffic.json"
-    if not p.exists():
-        return None
-    try:
-        d = json.load(open(p))
-    except Exception:
-        return None
-    for k, v in d.items():
-        if k.startswith(kernel_prefix) or kernel_prefix.startswith(k):
-            return v
-    return None
+DUMP_ROWS = 65536
+
+
+def dump_outputs(out_dir, last, z_all, gae, inv):
+    """What a caller of the timed step receives after its last step, as float32 / float64 .npy files (≤ 64 MB in all): the two
+    losses, the Feature-AE embedding and the Graph-AE z / mu / logvar on a fixed seeded sample of DUMP_ROWS cells (rows in the
+    data's cell order, whatever order the Graph-AE ran in), and the Graph-AE weights after the step's Adam update."""
+    out_dir.mkdir(parents=True, exist_ok=True)
+    n = z_all.shape[0]
+    rows = np.sort(np.random.default_rng(1234).choice(n, size=min(n, DUMP_ROWS), replace=False))
+    rows_t = torch.from_numpy(rows).to(z_all.device)
+    gae_rows = inv[rows_t].long() if inv is not None else rows_t           # position of each sampled cell in the Graph-AE's order
+    arrays = {"cell_index": rows.astype(np.float64),
+              "feature_ae_loss": last["fae_loss"].double().cpu().numpy(),
+              "feature_ae_embedding": z_all[rows_t].float().cpu().numpy(),
+              "graph_ae_loss": gae.loss.double().cpu().numpy()}
+    for name in ("z", "mu", "logvar"):
+        arrays[f"graph_ae_{name}"] = last[f"gae_{name}"][gae_rows].float().cpu().numpy()
+    for name, w in gae.state_dict().items():
+        arrays[f"graph_ae_{name.replace('.', '_')}"] = w.float().cpu().numpy()
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", a)
 
 
 def gae_reference_rows(z, rowptr, colidx, norm, pw, rows, chunk=256):

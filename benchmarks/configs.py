@@ -113,7 +113,7 @@ def config5(args):
     model = SimpleGCDEC(50, 50, device=dev)
     init = torch.randint(0, 7, (n, ), generator=torch.Generator().manual_seed(0)).numpy()
     t0 = time.perf_counter()
-    model.bind(pcs, adj)                          # AX = adj · X once (tcgen05 GEMM); every epoch is then AX·W + b
+    model.bind(pcs, adj)                          # AX = adj · X once (tensor-core GEMM); every epoch is then AX·W + b
     torch.cuda.synchronize()
     bind_s = time.perf_counter() - t0
     model.fit(pcs, adj, lr=0.005, epochs=5, opt="admin", init_labels=init, tol=0)

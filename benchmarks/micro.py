@@ -13,7 +13,7 @@ import torch
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 from dance_b200 import ops  # noqa: E402
 
-PEAKS = {"hbm_gbs": 6566.1, "bf16_tflops": 1746.9}
+PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}   # NVIDIA H100 SXM data sheet (700 W); MEASURED_PEAKS.json overrides
 try:
     PEAKS.update(json.load(open(Path(__file__).resolve().parent.parent / "MEASURED_PEAKS.json")))
 except Exception:
@@ -51,6 +51,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, default=1_000_000)
     ap.add_argument("--only", type=str, default="")
+    ap.add_argument("--out", type=str, default=None, help="also write every result line as one JSON list to this file")
     args = ap.parse_args()
     dev = torch.device("cuda:0")
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
@@ -196,8 +197,9 @@ def main():
         med, best = timeit(lambda: ops.pca(X, k), iters=2, warmup=1)
         out.append(dict(kernel="pca (CellPCA: covariance GEMM + Jacobi eigensolver + projection)", n=nn, g=g, k=k, ms=med))
         print(json.dumps(out[-1]), flush=True)
-    Path("gpurun_out").mkdir(exist_ok=True)
-    json.dump(out, open("gpurun_out/micro.json", "w"), indent=1)
+    if args.out:
+        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
+        json.dump(out, open(args.out, "w"), indent=1)
 
 
 if __name__ == "__main__":

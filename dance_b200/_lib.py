@@ -151,11 +151,11 @@ def lib():
             fn.argtypes = args
         _lib = handle
         # A/B selector of the decoder kernel for a whole process (read once at load; tests switch paths with ops.set_path):
-        #   B2_FORCE_GAE_PATH = cuda | tf32 | f16 | sym
+        #   B2_FORCE_GAE_PATH = cuda | tc
         import os
         forced = os.environ.get("B2_FORCE_GAE_PATH")
         if forced:
-            modes = {"auto": 0, "cuda": 1, "tf32": 2, "f16": 3, "sym": 4}
+            modes = {"auto": 0, "cuda": 1, "tc": 2}
             if forced not in modes:
                 raise B2Error(f"B2_FORCE_GAE_PATH={forced!r}: expected one of {sorted(modes)}")
             handle.b2_set_path(0, modes[forced])

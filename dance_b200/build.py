@@ -1,8 +1,8 @@
-"""Build the C-ABI shared library ``dance_b200/lib/libdance_b200.so`` with nvcc for sm_100a.
+"""Build the C-ABI shared library ``dance_b200/lib/libdance_b200.so`` with nvcc for sm_90a.
 
-The library is built IN-TREE so that it travels with the repository snapshot to the
-GPU box (it is git-ignored, not gpurun-ignored).  ``python -m dance_b200.build`` or
-``__graft_entry__.build()`` run this; nothing is JIT-compiled at import time.
+The library is built IN-TREE (git-ignored) so that the package is importable from the
+repository tree.  ``python -m dance_b200.build`` or ``__graft_entry__.build()`` run this;
+nothing is JIT-compiled at import time.
 """
 from __future__ import annotations
 
@@ -21,7 +21,7 @@ OBJ_DIR = PKG / "lib" / "obj"
 LIB_PATH = LIB_DIR / "libdance_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "--expt-extended-lambda",
     "-Xcompiler", "-fPIC",
@@ -67,7 +67,7 @@ def _compile_one(src: Path, verbose: bool) -> Path:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every ``csrc/*.cu`` for sm_100a and link ``libdance_b200.so``; returns its path."""
+    """Compile every ``csrc/*.cu`` for sm_90a and link ``libdance_b200.so``; returns its path."""
     LIB_DIR.mkdir(exist_ok=True)
     OBJ_DIR.mkdir(exist_ok=True)
     if force:
@@ -81,7 +81,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     if LIB_PATH.exists() and stamp.exists() and stamp.read_text() == key and not force:
         return LIB_PATH
     cmd = [_nvcc(), "-shared", "-o", str(LIB_PATH), *map(str, objs),
-           "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
+           "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError(f"link failed:\n{res.stdout}\n{res.stderr}")

@@ -1,4 +1,4 @@
-// Shared helpers for the dance_b200 CUDA translation units (sm_100a only).
+// Shared helpers for the dance_b200 CUDA translation units (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,21 +1,21 @@
-// Tensor-core version of the matrix-free Graph-AE decoder loss (all-pairs part):
-//   Σ_{i,j} softplus(z_i·z_j)   and   dz_i = 2c·Σ_j σ(z_i·z_j) z_j
-// (reference: InnerProductDecoder + BCE-with-logits, scgnn2.py:423-426, 603-619).
+// Tensor-core version of the all-pairs part of the Graph-AE decoder loss (scgnn2.py:423-426, 603-619):
+//   loss += Σ_ij softplus(z_i · z_j),   dZ_i += 2·coef · Σ_j σ(z_i · z_j) · z_j
+// Flash-attention-shaped row sweep: a CTA owns 128 rows I (two consumer warpgroups of 64) and streams 128-row tiles J:
+//   S  = Z_I · Z_Jᵀ        wgmma m64n128k8 tf32, 3-product split (Z pre-split into hi = x & 0xFFFFE000 and lo = x − hi,
+//                          lo·hi + hi·lo + hi·hi), fp32 accumulators in registers
+//   G  = σ(S), loss       SFU math on the accumulator registers (e = 2^(−|x|·log2e), r = 1/(1+e), one lg2 per 32 logits)
+//   dZ_I += G · Z_J       wgmma m64nDk8 tf32 with A = G taken straight from the registers (hi / lo split of G and Z_J, three
+//                          products) and B = Z_Jᵀ from shared memory
+// A producer warp copies the pre-split J tiles into a two-stage ring with 1-D bulk copies (the tiles are laid out in global
+// memory exactly as wgmma reads them: K-major, 128-byte swizzle).
 //
-// Flash-attention-shaped, all on tcgen05:
-//   S  = Z_I · Z_Jᵀ            tcgen05.mma kind::tf32, 3-product split (Z pre-split into hi/lo), S in TMEM
-//   G  = σ(S), loss += softplus(S)   sixteen "elementwise" warps: tcgen05.ld S → SFU math → tcgen05.st G_hi/G_lo into TMEM
-//   dZ_I += G · Z_J             tcgen05.mma with the A operand read from TMEM (G), B = Z_Jᵀ tile from shared memory
-// The N×N logits never leave the SM.  One CTA owns a 128-row block I and streams 64-column tiles J through a
-// TMA ring; S and G are double-buffered in TMEM so the two MMAs of tile t overlap the SFU work of tile t±1.
-// Per logit: 2 SFU ops (ex2, rcp) — the log of softplus is taken once per 16 logits on a running product.
+// Register fragment trick: the accumulator of S gives a thread columns (2t, 2t+1) of each 8-column block, the tf32 A fragment
+// wants columns (t, t+4).  The sum over j does not care about order, so the 8 columns of each block are fed to the second
+// MMA in the order (0, 2, 4, 6, 1, 3, 5, 7) and Z_Jᵀ is stored with its columns permuted the same way.
 //
-// Operand layouts (embedding width d ≤ 16, zero-padded to 16):
-//   Z16  [n,16]  rows of 64 B  → K-major SWIZZLE_64B tiles: A (128 rows) and B (64 rows) of the S product, K = 16
-//   ZT   [16,n'] transposed    → K-major SWIZZLE_128B tiles [16 rows(d) × 32 j]: B of the dZ product (N = 16, K = j)
-// Round-1 measurements that shaped this: each CTA streams every row of Z, so the TMA ring is L2-bandwidth bound
-// unless the per-tile bytes are small (16 KB here), and a tcgen05.mma of this size costs ~60 cycles regardless of N,
-// so consecutive k-steps alternate between independent accumulators.
+// Work units: row blocks.  The row form covers [row_begin, row_begin + n_rows); the pair-sharded form (multi-GPU) takes
+// "super-blocks" s = {block s, block nb−1−s} (a lone middle block when nb is odd), so that super-block ranges split the work
+// evenly over ranks.  The J sweep of a unit can be cut into step ranges (grid.y), which then add into dz atomically.
 #include "tc_common.cuh"
 
 #include <stdlib.h>
@@ -26,318 +26,305 @@ namespace gtc {
 
 using namespace tc;
 
-constexpr int BI = 128;          // rows per CTA (UMMA M)
-constexpr int BJ = 64;           // columns per tile (UMMA N of the S product, K of the dZ product)
-constexpr int DW = 16;           // embedding width handled (d ≤ 16, zero-padded)
-constexpr int STAGES = 4;
-constexpr int EW_WARPS = 16;     // elementwise warps: 4 per TMEM lane quarter (= per SM sub-partition), 16 columns each
-constexpr int EW_THREADS = EW_WARPS * 32;
-constexpr int EW_COLS = BJ / (EW_WARPS / 4);
-constexpr int THREADS = 128 + EW_THREADS;   // warps: 0 TMA, 1 MMA, 2 TMEM alloc, 3 idle, 4.. elementwise
-constexpr int ZI_BYTES = BI * DW * 4;            // 8 KB  (hi or lo)
-constexpr int ZJ_BYTES = BJ * DW * 4;            // 4 KB  (hi or lo), K-major rows of 64 B
-constexpr int ZT_BYTES = DW * BJ * 4;            // 4 KB  (hi or lo): two boxes of [16 rows x 128 B]
-constexpr int STAGE_BYTES = 2 * ZJ_BYTES + 2 * ZT_BYTES;   // 16 KB
-constexpr uint32_t TM_S = 0, TM_GHI = 128, TM_GLO = 256, TM_D = 384, TM_COLS = 512;
-// dZ accumulators at TM_D + 16·{0: big A, 1: small A, 2: big B, 3: small B}
+constexpr int BT = 128;                 // rows per block / tile
+constexpr int CONSUMERS = 256;          // two warpgroups
+constexpr int THREADS = CONSUMERS + 32; // + producer warp
+constexpr int STAGES = 2;
+constexpr int MAX_D = 32;
+constexpr uint32_t ZS_BYTES = BT * 128; // one plane of a tile for S (K-major, 128-byte rows)
+constexpr int ZS_PLANES = 2;            // hi, lo
 
-struct Params {
-  CUtensorMap mI_hi, mI_lo;      // Z16 [n,16] box {16,128} SWIZZLE_64B   (A of the S product)
-  CUtensorMap mJ_hi, mJ_lo;      // Z16 [n,16] box {16,64}  SWIZZLE_64B   (B of the S product)
-  CUtensorMap mT_hi, mT_lo;      // ZT  [16,n'] box {32,16} SWIZZLE_128B  (B of the dZ product)
-  float* dz;                     // [n_rows, d]
-  double* loss_acc;
-  int n, d, row_begin, n_rows, j_chunk, j_splits;
-  float coef;
-};
+static int64_t padded_n(int32_t n) { return ((int64_t)n + BT - 1) / BT * BT; }
+template <int DP> constexpr uint32_t zt_bytes() { return (uint32_t)DP * 4 * 128; }   // one plane of Z_Jᵀ: 4 atoms of DP x 128 B
 
-// z [n,d] → hi/lo tf32 split, as Z16 (row-major, padded to 16) and ZT (transposed, row pitch npad)
+// position of column jj of a tile in the permuted order of the dZ MMA (see header)
+__host__ __device__ __forceinline__ int zt_pos(int jj) { const int q = jj & 7; return (jj & ~7) | ((q & 1) ? 4 + (q >> 1) : (q >> 1)); }
+
+__device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
+
+// z → hi / lo planes, tile by tile: ZS [tile][128 rows x 32 tf32, swizzled], ZT [tile][4 atoms][DP rows x 32 tf32, swizzled]
+template <int DP>
 __global__ void __launch_bounds__(256)
-split_kernel(const float* __restrict__ z, int64_t ldz, int32_t n, int32_t d, int64_t npad, float* __restrict__ z16h,
-             float* __restrict__ z16l, float* __restrict__ zth, float* __restrict__ ztl) {
-  const int64_t total = npad * DW;
+gae_split_kernel(const float* __restrict__ z, int64_t ldz, int32_t n, int32_t d, int64_t npad, uint8_t* __restrict__ zs_hi,
+                 uint8_t* __restrict__ zs_lo, uint8_t* __restrict__ zt_hi, uint8_t* __restrict__ zt_lo) {
+  const int64_t total = npad * DP;
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t i = t / DW;
-    const int c = (int)(t % DW);
-    const float v = (c < d && i < n) ? z[i * ldz + c] : 0.f;
-    const float h = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);   // exactly representable in tf32
-    if (i < n) { z16h[t] = h; z16l[t] = v - h; }
-    zth[(int64_t)c * npad + i] = h;
-    ztl[(int64_t)c * npad + i] = v - h;
+    const int64_t row = t / DP;
+    const int k = (int)(t % DP);
+    const float v = (row < n && k < d) ? z[row * ldz + k] : 0.f;
+    const float h = tf32_trunc(v);
+    const float l = v - h;
+    const int64_t tile = row / BT;
+    const int r = (int)(row % BT);
+    const size_t so = (size_t)tile * ZS_BYTES + sw128_offset32((uint32_t)r, (uint32_t)k);
+    *reinterpret_cast<float*>(zs_hi + so) = h;
+    *reinterpret_cast<float*>(zs_lo + so) = l;
+    const int p = zt_pos(r);
+    const size_t to = (size_t)tile * zt_bytes<DP>() + (size_t)(p >> 5) * (DP * 128) + sw128_offset32((uint32_t)k, (uint32_t)(p & 31));
+    *reinterpret_cast<float*>(zt_hi + to) = h;
+    *reinterpret_cast<float*>(zt_lo + to) = l;
   }
 }
 
-__device__ __forceinline__ float ex2a(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float lg2a(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float rcpa(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+struct Params {
+  const float* z;
+  int64_t ldz;
+  const uint8_t *zs_hi, *zs_lo, *zt_hi, *zt_lo;
+  float* dz;
+  double* loss_acc;
+  float coef;
+  int n, d;
+  int row_begin, row_end;      // row form: rows [row_begin, row_end), dz row i at dz[(i - row_begin) * d]
+  int sb_begin, nb, sym;       // pair-sharded form: grid.x = 2 x super-blocks from sb_begin, dz row i at dz[i * d]
+  int n_jt;                    // J tiles
+};
 
+template <int N>
+__device__ __forceinline__ void mma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+  if constexpr (N == 8) wgmma_tf32_rs_n8(d, a, b, scale_d);
+  else if constexpr (N == 16) wgmma_tf32_rs_n16(d, a, b, scale_d);
+  else wgmma_tf32_rs_n32(d, a, b, scale_d);
+}
+
+__device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+
+template <int DP>
 __global__ void __launch_bounds__(THREADS, 1)
 gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const uint32_t s_zi_hi = smem_u32(smem), s_zi_lo = s_zi_hi + ZI_BYTES;
-  const uint32_t s_ring = s_zi_lo + ZI_BYTES;
-  uint8_t* bar_area = smem + 2 * ZI_BYTES + STAGES * STAGE_BYTES;
-  const uint32_t bars = smem_u32(bar_area);
-  const uint32_t zi_bar = bars;                      // 1
-  const uint32_t full_bar = bars + 8;                // [STAGES] TMA → MMA
-  const uint32_t stage_free = full_bar + 8 * STAGES; // [STAGES] dZ-MMA commit → TMA
-  const uint32_t s_full = stage_free + 8 * STAGES;   // [2] S-MMA commit → elementwise
-  const uint32_t s_empty = s_full + 16;              // [2] elementwise → S-MMA
-  const uint32_t g_full = s_empty + 16;              // [2] elementwise → dZ-MMA
-  const uint32_t g_empty = g_full + 16;              // [2] dZ-MMA commit → elementwise
-  const uint32_t d_full = g_empty + 16;              // 1  last commit → epilogue
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(bar_area + 8 * (2 + 2 * STAGES + 8) + 8);
+  constexpr uint32_t ZT = zt_bytes<DP>();
+  constexpr uint32_t STAGE = ZS_PLANES * ZS_BYTES + 2 * ZT;
+  uint8_t* zi_hi = smem;
+  uint8_t* zi_lo = smem + ZS_BYTES;
+  uint8_t* ring = smem + ZS_PLANES * ZS_BYTES;
+  const uint32_t full_bar = smem_u32(ring + STAGES * STAGE), empty_bar = full_bar + 8 * STAGES;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int ib = blockIdx.x;                          // row block
-  const int j_begin = blockIdx.y * p.j_chunk;
-  const int j_end = min(p.n, j_begin + p.j_chunk);
-  const int n_tiles = (j_end - j_begin + BJ - 1) / BJ;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.mI_hi); tma_prefetch_desc(&p.mI_lo); tma_prefetch_desc(&p.mJ_hi);
-    tma_prefetch_desc(&p.mJ_lo); tma_prefetch_desc(&p.mT_hi); tma_prefetch_desc(&p.mT_lo);
+  // ---- work unit ----
+  int row0, row_end, dz_row0;
+  if (p.sym) {
+    const int sb = p.sb_begin + (int)(blockIdx.x >> 1);
+    const int blk = (blockIdx.x & 1) ? p.nb - 1 - sb : sb;
+    if ((blockIdx.x & 1) && blk == sb) return;           // lone middle block: one unit only
+    row0 = blk * BT; row_end = min(p.n, row0 + BT); dz_row0 = 0;
+  } else {
+    row0 = p.row_begin + (int)blockIdx.x * BT; row_end = min(p.row_end, row0 + BT); dz_row0 = p.row_begin;
   }
-  if (warp == 1 && lane == 0) {
-    mbar_init(zi_bar, 1);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(stage_free + 8 * s, 1); }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(s_full + 8 * b, 1);
-      mbar_init(s_empty + 8 * b, EW_WARPS);   // one arrival per elementwise warp (512 per-thread arrivals on one
-      mbar_init(g_full + 8 * b, EW_WARPS);    // mbarrier cost ~2000 cycles per tile — measured)
-      mbar_init(g_empty + 8 * b, 1);
-    }
-    mbar_init(d_full, 1);
+  const int per = (p.n_jt + (int)gridDim.y - 1) / (int)gridDim.y;
+  const int jt0 = (int)blockIdx.y * per, jt1 = min(p.n_jt, jt0 + per);
+  if (jt0 >= jt1) return;
+  const int nt = jt1 - jt0;
+
+  const int tid = threadIdx.x;
+  if (tid == 0) {
+    for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, CONSUMERS / 32); }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), TM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(zi_bar, 2 * ZI_BYTES);
-      tma_load_2d(s_zi_hi, &p.mI_hi, zi_bar, 0, p.row_begin + ib * BI);
-      tma_load_2d(s_zi_lo, &p.mI_lo, zi_bar, 0, p.row_begin + ib * BI);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = 0; t < n_tiles; ++t) {
-        mbar_wait(stage_free + 8 * stage, phase ^ 1);
-        const uint32_t fb = full_bar + 8 * stage, st = s_ring + stage * STAGE_BYTES;
-        const int j0 = j_begin + t * BJ;
-        mbar_expect_tx(fb, STAGE_BYTES);
-        tma_load_2d(st, &p.mJ_hi, fb, 0, j0);
-        tma_load_2d(st + ZJ_BYTES, &p.mJ_lo, fb, 0, j0);
-        tma_load_2d(st + 2 * ZJ_BYTES, &p.mT_hi, fb, j0, 0);
-        tma_load_2d(st + 2 * ZJ_BYTES + 2048, &p.mT_hi, fb, j0 + 32, 0);
-        tma_load_2d(st + 2 * ZJ_BYTES + ZT_BYTES, &p.mT_lo, fb, j0, 0);
-        tma_load_2d(st + 2 * ZJ_BYTES + ZT_BYTES + 2048, &p.mT_lo, fb, j0 + 32, 0);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  if (tid >= CONSUMERS) {
+    // ===================== producer warp =====================
+    if (tid == CONSUMERS) {
+      for (int i = 0; i < nt; ++i) {
+        const int s = i % STAGES;
+        if (i >= STAGES) mbar_wait(empty_bar + 8 * s, (uint32_t)((i / STAGES - 1) & 1));
+        const uint32_t fb = full_bar + 8 * s, dst = smem_u32(ring + s * STAGE);
+        const size_t t = (size_t)(jt0 + i);
+        mbar_expect_tx(fb, STAGE);
+        bulk_load(dst, p.zs_hi + t * ZS_BYTES, ZS_BYTES, fb);
+        bulk_load(dst + ZS_BYTES, p.zs_lo + t * ZS_BYTES, ZS_BYTES, fb);
+        bulk_load(dst + 2 * ZS_BYTES, p.zt_hi + t * ZT, ZT, fb);
+        bulk_load(dst + 2 * ZS_BYTES + ZT, p.zt_lo + t * ZT, ZT, fb);
       }
+    }
+    return;
+  }
+
+  // ===================== consumers =====================
+  // Z_I planes from z (rows past the range are zero: their logits are masked below)
+  for (int e = tid; e < BT * DP; e += CONSUMERS) {
+    const int r = e / DP, k = e % DP;
+    const int row = row0 + r;
+    const float v = (row < row_end && k < p.d) ? p.z[(int64_t)row * p.ldz + k] : 0.f;
+    const float h = tf32_trunc(v);
+    const uint32_t o = sw128_offset32((uint32_t)r, (uint32_t)k);
+    *reinterpret_cast<float*>(zi_hi + o) = h;
+    *reinterpret_cast<float*>(zi_lo + o) = v - h;
+  }
+  fence_proxy_async();
+  asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
+
+  const int wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+  const int ra = row0 + wg * 64 + warp * 16 + (lane >> 2);       // rows of this thread: ra, ra + 8
+  const bool live_a = ra < row_end, live_b = ra + 8 < row_end;
+  const uint32_t ai_hi = smem_u32(zi_hi) + wg * 64 * 128, ai_lo = smem_u32(zi_lo) + wg * 64 * 128;
+  constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
+
+  // The accumulation inside the tensor core truncates, and the hi·hi product carries almost all of dZ: over a whole J sweep one
+  // accumulator would drift by ~1e-5 relative (~6e-5 for |z| ~ 1e5).  So the hi·hi products of a tile go round-robin into NB
+  // accumulators (16 / NB adds each), the two cross terms into one more, and the tile's sum joins an fp32 total with
+  // round-to-nearest adds.
+  constexpr int NB = DP <= 16 ? 4 : 2;
+  float dzb[NB][DP / 2], dzs[DP / 2], dzt[DP / 2];
+#pragma unroll
+  for (int v = 0; v < DP / 2; ++v) dzt[v] = 0.f;
+  double loss = 0.0;
+
+  for (int i = 0; i < nt; ++i) {
+    const int s = i % STAGES;
+    mbar_wait(full_bar + 8 * s, (uint32_t)((i / STAGES) & 1));
+    const uint32_t st = smem_u32(ring + s * STAGE);
+    const uint32_t bs_hi = st, bs_lo = st + ZS_BYTES, bt_hi = st + 2 * ZS_BYTES, bt_lo = bt_hi + ZT;
+    float S[BT / 2];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < DP / 8; ++kk) {
+      const uint32_t o = kk * 32;
+      wgmma_tf32_ss_n128(S, wgmma_desc_sw128(ai_lo + o), wgmma_desc_sw128(bs_hi + o), kk > 0);
+      wgmma_tf32_ss_n128(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_lo + o), 1);
+      wgmma_tf32_ss_n128(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_hi + o), 1);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(S);
+
+    // ---- σ and softplus on the registers ----
+    const int jbase = (jt0 + i) * BT + 2 * (lane & 3);
+    float relu = 0.f, lg = 0.f, prod = 1.f;
+#pragma unroll
+    for (int v = 0; v < BT / 2; ++v) {
+      if ((v & 31) == 31) { lg += lg2_approx(prod); prod = 1.f; }
+      const int j = jbase + 8 * (v >> 2) + (v & 1);
+      const bool ok = j < p.n && (((v >> 1) & 1) ? live_b : live_a);
+      const float x = S[v];
+      const float e = ex2_approx(-fabsf(x) * LOG2E);
+      const float inv = rcp_approx(1.f + e);
+      const float sg = x >= 0.f ? inv : e * inv;
+      relu += ok ? fmaxf(x, 0.f) : 0.f;
+      prod *= ok ? 1.f + e : 1.f;
+      S[v] = ok ? sg : 0.f;
+    }
+    loss += (double)(relu + LN2 * (lg + lg2_approx(prod)));
+
+    // ---- dZ_I += G · Z_J ----
+    wgmma_fence();
+#pragma unroll
+    for (int kb = 0; kb < BT / 8; ++kb) {
+      const float g[4] = {S[4 * kb], S[4 * kb + 2], S[4 * kb + 1], S[4 * kb + 3]};   // (r, 2t) (r+8, 2t) (r, 2t+1) (r+8, 2t+1)
+      uint32_t ahi[4], alo[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        ahi[q] = __float_as_uint(g[q]) & 0xFFFFE000u;
+        alo[q] = __float_as_uint(g[q] - __uint_as_float(ahi[q]));
+      }
+      const uint32_t o = (uint32_t)(kb >> 2) * (DP * 128) + (uint32_t)(kb & 3) * 32;
+      mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
+      mma_rs<DP>(dzs, ahi, wgmma_desc_sw128(bt_lo + o), 1);
+      mma_rs<DP>(dzb[kb % NB], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NB);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int b = 0; b < NB; ++b) reg_fence(dzb[b]);
+    reg_fence(dzs);
+#pragma unroll
+    for (int v = 0; v < DP / 2; ++v) {
+      float t = dzs[v];
+#pragma unroll
+      for (int b = 0; b < NB; ++b) t += dzb[b][v];
+      dzt[v] += t;
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = umma_idesc(BI, BJ, 0, 0);   // S  = Z_I (K-major, K = 16) · Z_J (K-major)
-      const uint32_t idesc_d = umma_idesc(BI, DW, 0, 0);   // dZ = G (TMEM, K = j) · Z_Jᵀ tile (K-major, N = 16)
-      mbar_wait(zi_bar, 0);
-      tc_fence_after();
-      auto issue_s = [&](int t, int stage, uint32_t phase) {
-        const int b = t & 1;
-        mbar_wait(s_empty + 8 * b, ((t >> 1) & 1) ^ 1);
-        mbar_wait(full_bar + 8 * stage, phase);
-        tc_fence_after();
-        const uint32_t st = s_ring + stage * STAGE_BYTES;
-        const uint32_t d_s = tmem + TM_S + (uint32_t)(b * BJ);
-#pragma unroll
-        for (int k = 0; k < DW / 8; ++k) {
-          // SWIZZLE_64B K-major: 64-byte rows, 8-row groups 512 B apart
-          const uint64_t a_hi = umma_desc(s_zi_hi + k * 32, 16, 512, 4), a_lo = umma_desc(s_zi_lo + k * 32, 16, 512, 4);
-          const uint64_t b_hi = umma_desc(st + k * 32, 16, 512, 4), b_lo = umma_desc(st + ZJ_BYTES + k * 32, 16, 512, 4);
-          umma_tf32(d_s, a_lo, b_hi, idesc_s, k > 0);
-          umma_tf32(d_s, a_hi, b_lo, idesc_s, 1);
-          umma_tf32(d_s, a_hi, b_hi, idesc_s, 1);
-        }
-        umma_commit(s_full + 8 * b);
-      };
-      int stage_s = 0, stage_d = 0;
-      uint32_t phase_s = 0;
-      if (n_tiles > 0) { issue_s(0, 0, 0); if (++stage_s == STAGES) { stage_s = 0; phase_s ^= 1; } }
-      for (int t = 0; t < n_tiles; ++t) {
-        if (t + 1 < n_tiles) { issue_s(t + 1, stage_s, phase_s); if (++stage_s == STAGES) { stage_s = 0; phase_s ^= 1; } }
-        const int b = t & 1;
-        mbar_wait(g_full + 8 * b, (t >> 1) & 1);
-        tc_fence_after();
-        const uint32_t zt = s_ring + stage_d * STAGE_BYTES + 2 * ZJ_BYTES;
-        const uint32_t g_hi = tmem + TM_GHI + (uint32_t)(b * BJ), g_lo = tmem + TM_GLO + (uint32_t)(b * BJ);
-#pragma unroll
-        for (int k = 0; k < BJ / 8; ++k) {
-          // ZT tile: two boxes of [16 rows(d) x 128 B (32 j)], SWIZZLE_128B K-major; k-step = 8 j = 32 B
-          const uint32_t boff = (uint32_t)(k >> 2) * 2048u + (uint32_t)(k & 3) * 32u;
-          const uint64_t b_hi = umma_desc(zt + boff, 16, 1024, 2);
-          const uint64_t b_lo = umma_desc(zt + ZT_BYTES + boff, 16, 1024, 2);
-          // even / odd k-steps feed independent accumulator pairs (A / B) so consecutive MMAs never wait on each other
-          const uint32_t dbase = tmem + TM_D + (uint32_t)((k & 1) * 32);
-          const uint32_t acc = (t > 0 || k > 1) ? 1u : 0u;
-          umma_tf32_ts(dbase + 16, g_lo + k * 8, b_hi, idesc_d, acc);   // small: lo·hi
-          umma_tf32_ts(dbase, g_hi + k * 8, b_hi, idesc_d, acc);        // big:   hi·hi
-          umma_tf32_ts(dbase + 16, g_hi + k * 8, b_lo, idesc_d, 1);     // small: hi·lo
-        }
-        umma_commit(g_empty + 8 * b);
-        umma_commit(stage_free + 8 * stage_d);
-        if (++stage_d == STAGES) stage_d = 0;
-      }
-      umma_commit(d_full);
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    // ===================== elementwise warps =====================
-    const int sub = warp & 3;             // TMEM lane quarter
-    const int part = (warp - 4) >> 2;     // which EW_COLS-wide slice of the tile's 64 columns
-    const int row_local = ib * BI + sub * 32 + lane;
-    const bool live = row_local < p.n_rows;
-    const uint32_t lane_off = (uint32_t)(sub * 32) << 16;
-    constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
-    static_assert(EW_COLS == 16, "elementwise slice is written for 16 columns");
-    float relu_sum = 0.f, lg_sum = 0.f;
-    for (int t = 0; t < n_tiles; ++t) {
-      const int b = t & 1;
-      const uint32_t par = (t >> 1) & 1;
-      mbar_wait(s_full + 8 * b, par);
-      tc_fence_after();
-      uint32_t v[EW_COLS];
-      tmem_ld_32x32b_x16(tmem + lane_off + TM_S + (uint32_t)(b * BJ + part * EW_COLS), v);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_empty + 8 * b);       // S[b] has been copied to registers
-      const int col0 = j_begin + t * BJ + part * EW_COLS;
-      // staged so that the 16 independent SFU chains are issued back to back (ILP instead of one long dependent chain)
-      float e[EW_COLS], sg[EW_COLS];
-#pragma unroll
-      for (int c = 0; c < EW_COLS; ++c) e[c] = ex2a(-fabsf(__uint_as_float(v[c])) * LOG2E);
-#pragma unroll
-      for (int c = 0; c < EW_COLS; ++c) sg[c] = rcpa(1.f + e[c]);
-      float prod0 = 1.f, prod1 = 1.f;
-      uint32_t hi[EW_COLS], lo[EW_COLS];
-#pragma unroll
-      for (int c = 0; c < EW_COLS; ++c) {
-        const float x = __uint_as_float(v[c]);
-        float s = x >= 0.f ? sg[c] : e[c] * sg[c];               // sigmoid(x)
-        const bool valid = col0 + c < j_end;
-        relu_sum += valid ? fmaxf(x, 0.f) : 0.f;
-        const float f = valid ? 1.f + e[c] : 1.f;
-        if (c & 1) prod1 *= f; else prod0 *= f;
-        s = valid ? s : 0.f;
-        const uint32_t h = __float_as_uint(s) & 0xFFFFE000u;
-        hi[c] = h;
-        lo[c] = __float_as_uint(s - __uint_as_float(h));
-      }
-      lg_sum += lg2a(prod0 * prod1);                             // Σ log2(1+e) over this thread's logits of the tile
-      mbar_wait(g_empty + 8 * b, par ^ 1);                       // the dZ-MMA of tile t-2 has finished reading G[b]
-      tc_fence_after();
-      tmem_st_32x32b_x16(tmem + lane_off + TM_GHI + (uint32_t)(b * BJ + part * EW_COLS), hi);
-      tmem_st_32x32b_x16(tmem + lane_off + TM_GLO + (uint32_t)(b * BJ + part * EW_COLS), lo);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(g_full + 8 * b);
-    }
-    double loss = live ? (double)(relu_sum + LN2 * lg_sum) : 0.0;
-    loss = warp_sum(loss);
-    if (lane == 0 && loss != 0.0) atomicAdd(p.loss_acc, loss * (double)p.coef);
-    if (part == 0) {
-      mbar_wait(d_full, 0);
-      tc_fence_after();
-      uint32_t a0[16], a1[16], a2[16], a3[16];
-      tmem_ld_32x32b_x16(tmem + lane_off + TM_D, a0);
-      tmem_ld_32x32b_x16(tmem + lane_off + TM_D + 16, a1);
-      tmem_ld_32x32b_x16(tmem + lane_off + TM_D + 32, a2);
-      tmem_ld_32x32b_x16(tmem + lane_off + TM_D + 48, a3);
-      if (live && n_tiles > 0) {
-        const float c2 = 2.f * p.coef;
-        float* dst = p.dz + (size_t)row_local * p.d;
-#pragma unroll
-        for (int c = 0; c < 16; ++c) {
-          if (c < p.d) {
-            const float big = __uint_as_float(a0[c]) + __uint_as_float(a2[c]);
-            const float small = __uint_as_float(a1[c]) + __uint_as_float(a3[c]);
-            const float g = c2 * (big + small);
-            if (p.j_splits == 1) dst[c] += g; else atomicAdd(dst + c, g);
-          }
-        }
-      }
-    }
+    if (lane == 0) mbar_arrive(empty_bar + 8 * s);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem, TM_COLS);
+
+  // ---- epilogue ----
+  const float c2 = 2.f * p.coef;
+  const bool atomic = gridDim.y > 1;
+#pragma unroll
+  for (int v = 0; v < DP / 2; ++v) {
+    const int row = ra + 8 * ((v >> 1) & 1);
+    const int col = 8 * (v >> 2) + 2 * (lane & 3) + (v & 1);
+    if (row >= row_end || col >= p.d) continue;
+    float* dst = p.dz + (int64_t)(row - dz_row0) * p.d + col;
+    const float val = c2 * dzt[v];
+    if (atomic) atomicAdd(dst, val);
+    else *dst += val;
   }
+  loss = warp_sum(loss);
+  if (lane == 0) atomicAdd(p.loss_acc, loss * (double)p.coef);
 }
 
-static int64_t padded_n(int32_t n) { return ((int64_t)n + 63) / 64 * 64; }
+size_t workspace_bytes(int32_t n) { return (size_t)padded_n(n) / BT * (ZS_PLANES * ZS_BYTES + 2 * zt_bytes<MAX_D>()); }
 
-size_t workspace_bytes(int32_t n) {
-  return 2 * align_up((size_t)n * DW * sizeof(float), 256) + 2 * align_up((size_t)padded_n(n) * DW * sizeof(float), 256);
-}
+int super_blocks(int32_t n) { return (int)((padded_n(n) / BT + 1) / 2); }
 
 bool eligible(int32_t n, int32_t d, int32_t n_rows) {
-  const int mode = path_mode(B2_PATH_GAE_DECODER);           // 0 auto · 2 this kernel
-  if (mode != 0 && mode != 2) return false;
-  return d >= 1 && d <= DW && (int64_t)n * n_rows >= (1ll << 22);
+  const int mode = path_mode(B2_PATH_GAE_DECODER);           // 0 auto · 1 CUDA cores · 2 this kernel
+  if (d < 1 || d > MAX_D || mode == 1) return false;
+  return mode == 2 || (int64_t)n * n_rows >= (1ll << 22);
 }
 
-// all-pairs part on the tensor cores; returns B2_ERR_UNSUPPORTED if tensor maps cannot be built
-int launch(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t row_begin, int32_t n_rows, float coef, float* dz,
-           double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st) {
-  if (ws_bytes < workspace_bytes(n)) return B2_ERR_UNSUPPORTED;
+template <int DP>
+static int launch_dp(const float* z, int64_t ldz, int32_t n, int32_t d, Params p, int units, float* dz, double* loss_acc, void* ws,
+                     cudaStream_t st) {
   const int64_t npad = padded_n(n);
-  char* w = reinterpret_cast<char*>(ws);
-  const size_t a16 = align_up((size_t)n * DW * sizeof(float), 256), at = align_up((size_t)npad * DW * sizeof(float), 256);
-  float* z16h = reinterpret_cast<float*>(w);
-  float* z16l = reinterpret_cast<float*>(w + a16);
-  float* zth = reinterpret_cast<float*>(w + 2 * a16);
-  float* ztl = reinterpret_cast<float*>(w + 2 * a16 + at);
-  {
-    int64_t blocks = ceil_div<int64_t>(npad * DW, 256 * 4);
-    const int64_t cap = (int64_t)sm_count() * 16;
-    if (blocks > cap) blocks = cap;
-    split_kernel<<<(unsigned)blocks, 256, 0, st>>>(z, ldz, n, d, npad, z16h, z16l, zth, ztl);
-    B2_CHECK_LAUNCH("split_kernel");
-  }
-  Params p;
-  memset(&p, 0, sizeof(p));
-  const int SW64 = (int)CU_TENSOR_MAP_SWIZZLE_64B, SW128 = (int)CU_TENSOR_MAP_SWIZZLE_128B;
-  bool ok = make_tensor_map_f32_ex(&p.mI_hi, z16h, DW, (uint64_t)n, DW, DW, BI, SW64) &&
-            make_tensor_map_f32_ex(&p.mI_lo, z16l, DW, (uint64_t)n, DW, DW, BI, SW64) &&
-            make_tensor_map_f32_ex(&p.mJ_hi, z16h, DW, (uint64_t)n, DW, DW, BJ, SW64) &&
-            make_tensor_map_f32_ex(&p.mJ_lo, z16l, DW, (uint64_t)n, DW, DW, BJ, SW64) &&
-            make_tensor_map_f32_ex(&p.mT_hi, zth, (uint64_t)npad, DW, (uint64_t)npad, 32, DW, SW128) &&
-            make_tensor_map_f32_ex(&p.mT_lo, ztl, (uint64_t)npad, DW, (uint64_t)npad, 32, DW, SW128);
-  if (!ok) return B2_ERR_UNSUPPORTED;
-  const int row_blocks = ceil_div(n_rows, BI);
-  int j_splits = 1;
-  const int target = sm_count();
-  if (row_blocks < target) j_splits = min(ceil_div(target, row_blocks), ceil_div(n, 8 * BJ));
-  if (j_splits < 1) j_splits = 1;
-  int j_chunk = ceil_div(ceil_div(n, j_splits), BJ) * BJ;
-  j_splits = ceil_div(n, j_chunk);
-  p.dz = dz; p.loss_acc = loss_acc; p.n = n; p.d = d; p.row_begin = row_begin; p.n_rows = n_rows;
-  p.j_chunk = j_chunk; p.j_splits = j_splits; p.coef = coef;
-  const size_t smem = 2 * ZI_BYTES + STAGES * STAGE_BYTES + 1024 + 256;
+  const int nb = (int)(npad / BT);
+  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
+  uint8_t* zs_hi = w;
+  uint8_t* zs_lo = zs_hi + (size_t)nb * ZS_BYTES;
+  uint8_t* zt_hi = zs_lo + (size_t)nb * ZS_BYTES;
+  uint8_t* zt_lo = zt_hi + (size_t)nb * zt_bytes<DP>();
+  int64_t blocks = ceil_div<int64_t>(npad * DP, 256);
+  const int64_t cap = (int64_t)sm_count() * 16;
+  if (blocks > cap) blocks = cap;
+  gae_split_kernel<DP><<<(unsigned)blocks, 256, 0, st>>>(z, ldz, n, d, npad, zs_hi, zs_lo, zt_hi, zt_lo);
+  B2_CHECK_LAUNCH("gae_split_kernel");
+  if (units <= 0) return B2_OK;
+  p.z = z; p.ldz = ldz; p.zs_hi = zs_hi; p.zs_lo = zs_lo; p.zt_hi = zt_hi; p.zt_lo = zt_lo;
+  p.dz = dz; p.loss_acc = loss_acc; p.n = n; p.d = d; p.nb = nb; p.n_jt = nb;
+  // J step ranges: b2_set_tuning(B2_TUNE_GAE_SPLITS) when set, else enough to fill one wave of SMs
+  int splits = tuning(B2_TUNE_GAE_SPLITS);
+  if (splits <= 0) splits = ceil_div(sm_count(), units);
+  if (splits > nb) splits = nb;
+  if (splits < 1) splits = 1;
+  const size_t smem = ZS_PLANES * ZS_BYTES + STAGES * (ZS_PLANES * ZS_BYTES + 2 * zt_bytes<DP>()) + 16 * STAGES + 1024;
   static bool attr_set = false;
   if (!attr_set) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(gae_allpairs_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    B2_CHECK_CUDA(cudaFuncSetAttribute(gae_allpairs_tc_kernel<DP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
-  dim3 grid(row_blocks, j_splits);
-  gae_allpairs_tc_kernel<<<grid, THREADS, smem, st>>>(p);
+  gae_allpairs_tc_kernel<DP><<<dim3((unsigned)units, (unsigned)splits), THREADS, smem, st>>>(p);
   B2_CHECK_LAUNCH("gae_allpairs_tc_kernel");
   return B2_OK;
+}
+
+static int launch_any(const float* z, int64_t ldz, int32_t n, int32_t d, const Params& p, int units, float* dz, double* loss_acc,
+                      void* ws, size_t ws_bytes, cudaStream_t st) {
+  if (ws_bytes < workspace_bytes(n)) return B2_ERR_UNSUPPORTED;
+  if (d <= 8) return launch_dp<8>(z, ldz, n, d, p, units, dz, loss_acc, ws, st);
+  if (d <= 16) return launch_dp<16>(z, ldz, n, d, p, units, dz, loss_acc, ws, st);
+  return launch_dp<32>(z, ldz, n, d, p, units, dz, loss_acc, ws, st);
+}
+
+// rows [row_begin, row_begin + n_rows) against all n columns; adds into dz[n_rows, d] and loss_acc
+int launch(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t row_begin, int32_t n_rows, float coef, float* dz,
+           double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st) {
+  Params p;
+  memset(&p, 0, sizeof(p));
+  p.coef = coef; p.row_begin = row_begin; p.row_end = row_begin + n_rows; p.sym = 0;
+  return launch_any(z, ldz, n, d, p, ceil_div(n_rows, BT), dz, loss_acc, ws, ws_bytes, st);
+}
+
+// super-blocks [sb_begin, sb_end) against all n columns; adds into dz[n, d] (the rows of those blocks) and loss_acc
+int launch_super_blocks(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t sb_begin, int32_t sb_end, float coef, float* dz,
+                        double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st) {
+  Params p;
+  memset(&p, 0, sizeof(p));
+  p.coef = coef; p.sym = 1; p.sb_begin = sb_begin;
+  return launch_any(z, ldz, n, d, p, 2 * (sb_end - sb_begin), dz, loss_acc, ws, ws_bytes, st);
 }
 
 }  // namespace gtc

@@ -91,7 +91,7 @@ gat_aggregate_fwd_kernel(const int32_t* __restrict__ rowptr, const int32_t* __re
   if ((F & 31) == 0) {
     // Wide heads (F a multiple of 32, e.g. STAGATE's 1×512): every lane of a t-slot belongs to the same head, so the edge
     // coefficient is computed ONCE per (edge, head) instead of once per (edge, 32-column slot) — the exponentials, not the
-    // gather, dominated the first version of this kernel (20.9 → see profiles/r01_micro.json).
+    // gather, dominated the first version of this kernel.
     const int tper = F >> 5;
     for (int64_t v = warp; v < n; v += nwarps) {
       const int32_t s = rowptr[v], e = rowptr[v + 1];

@@ -1,4 +1,4 @@
-// b2_gemm_f32 dispatcher: tcgen05 (TF32 / 3xTF32) kernel when the shape qualifies,
+// b2_gemm_f32 dispatcher: tensor-core wgmma (TF32 / 3xTF32) kernel when the shape qualifies,
 // CUDA-core fp32 kernel otherwise (or when B2_PREC_FP32_SIMT is requested).
 #include "common.cuh"
 

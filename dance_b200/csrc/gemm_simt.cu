@@ -1,5 +1,5 @@
 // CUDA-core fp32 GEMM with fused epilogue — the exact-fp32 path and the
-// fallback for shapes the tcgen05 kernel does not take (tiny / unaligned).
+// fallback for shapes the tensor-core kernel does not take (tiny / unaligned).
 //   C = act(op(A)·op(B) + bias) ⊙ [mask > 0]  (+ beta·C)
 // Replaces torch.mm / nn.Linear on the reference hot path
 // (scgnn2.py:352-370,499; spagcn.py:358; gnn.py:57).

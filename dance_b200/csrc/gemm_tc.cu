@@ -1,18 +1,17 @@
-// tcgen05 GEMM for the dense feature projections (fp32 in / fp32 out):
+// Tensor-core GEMM for the dense feature projections (fp32 in / fp32 out):
 //   C[M,N] = epilogue( op(A)[M,K] · op(B)[K,N] )
-// Blackwell-native structure: persistent CTAs (one per SM), TMA (cp.async.bulk.tensor)
-// stages the fp32 operand tiles into 128B-swizzled shared memory, one elected thread
-// issues tcgen05.mma.kind::tf32 with the accumulator in TMEM (double-buffered), four
-// epilogue warps read the accumulator back with tcgen05.ld and apply bias / activation /
-// ReLU-mask / accumulate before storing.  All operand layouts (row-major A or Aᵀ, B or Bᵀ)
-// are handled by choosing K-major or MN-major UMMA descriptors — nothing is transposed
-// in memory.
+// Hopper structure: one CTA per 128 x BN output tile (and K split), two consumer warpgroups of 64 rows each.  TMA
+// (cp.async.bulk.tensor) stages the raw fp32 operand tiles of each 32-wide k-block into a ring; all 256 threads then rewrite the
+// stage as K-major, 128B-swizzled tf32 planes (wgmma reads tf32 operands only K-major, so this one pass also serves the
+// transposed layouts: nothing is transposed in global memory) and issue wgmma.mma_async m64nBNk8 with fp32 accumulators in
+// registers.  The rewrite of k-block i+1 overlaps the asynchronous MMAs of k-block i (two plane buffers); the epilogue applies
+// bias / activation / ReLU-mask / accumulate straight from the accumulator registers.
 //
 // Precision modes
-//   TF32   : one tcgen05.mma per k-step (inputs truncated to 10-bit mantissa by the MMA)
-//   TF32X3 : fp32-accurate. Four "splitter" warps rewrite each staged tile in shared memory
-//            as hi = x & 0xFFFFE000 (exactly representable in tf32) and lo = x - hi, and the
-//            issuing thread accumulates lo·hi + hi·lo + hi·hi  (error ~2^-21 relative).
+//   TF32   : one wgmma per k-step (tf32 operands: 10-bit mantissa)
+//   TF32X3 : fp32-accurate. The rewrite also splits each value into hi = x & 0xFFFFE000 (exactly representable in tf32) and
+//            lo = x - hi, and the MMAs accumulate lo·hi + hi·lo into one accumulator and hi·hi into another, summed in the
+//            epilogue (error ~2^-21 relative).
 //
 // Replaces torch.mm / nn.Linear on the reference path (scgnn2.py:352-370, 499).
 #include "tc_common.cuh"
@@ -23,13 +22,12 @@
 namespace b2 {
 namespace tc {
 
-constexpr int BM = 128;            // UMMA M (cta_group::1)
+constexpr int BM = 128;            // two warpgroups x 64 rows
 constexpr int BK = 32;             // k-block: 32 tf32 = 128 B = one swizzle span
-constexpr int UK = 8;              // UMMA K for kind::tf32 (32 bytes)
-constexpr int THREADS = 384;       // 12 warps: TMA, MMA, TMEM-alloc, idle, 4 epilogue, 4 splitter
-constexpr int A_TILE_BYTES = BM * BK * 4;
-constexpr int MAX_STAGES = 8;
-constexpr int ATOM_BYTES = BK * 128;  // one MN-major atom: BK k-rows x 128 B
+constexpr int UK = 8;              // wgmma K for tf32
+constexpr int THREADS = 256;
+constexpr int MAX_STAGES = 4;
+constexpr int SMEM_LIMIT = 227 * 1024;
 
 struct Params {
   CUtensorMap tmA;
@@ -40,290 +38,168 @@ struct Params {
   float* partial;          // split-K partial tiles [splits][M][N] (dense) or nullptr
   long long ldc, ldmask;
   int M, N, K;
-  int BN;                  // 32 | 64 | 128
-  int a_mn, b_mn;          // operand major-ness: 0 = K-major, 1 = MN-major
+  int a_mn, b_mn;          // raw tile layout: 0 = K contiguous, 1 = M / N contiguous
   int x3;                  // 3xTF32 split
   int act;
   float beta;
   int tiles_m, tiles_n, splits, kb_per_split, kb_total, stages;
-  unsigned mn_lbo, mn_sbo, mn_layout;   // MN-major descriptor fields (bring-up overridable, see gemm_tc())
 };
 
-struct StageLayout {
-  uint32_t a_hi, a_lo, b_hi, b_lo;  // byte offsets inside one stage
-  uint32_t stage_bytes, b_bytes;
+// shared memory: [2 plane buffers: A hi | A lo | B hi | B lo] [ring: stages x (A raw | B raw)] [barriers]
+struct SmemLayout {
+  uint32_t a_plane, b_plane, plane_buf, raw_a, raw_stage, ring, bars, total;
 };
-__host__ __device__ inline StageLayout stage_layout(int BN, int x3) {
-  StageLayout L;
-  L.b_bytes = (uint32_t)BN * BK * 4;
-  L.a_hi = 0;
-  L.a_lo = A_TILE_BYTES;
-  L.b_hi = x3 ? 2 * A_TILE_BYTES : A_TILE_BYTES;
-  L.b_lo = L.b_hi + L.b_bytes;
-  L.stage_bytes = (x3 ? 2u : 1u) * (A_TILE_BYTES + L.b_bytes);
+__host__ __device__ inline SmemLayout smem_layout(int BN, int x3, int stages) {
+  SmemLayout L;
+  L.a_plane = BM * BK * 4;
+  L.b_plane = (uint32_t)BN * BK * 4;
+  L.plane_buf = (x3 ? 2u : 1u) * (L.a_plane + L.b_plane);
+  L.raw_a = BM * BK * 4;
+  L.raw_stage = L.raw_a + L.b_plane;
+  L.ring = 2 * L.plane_buf;
+  L.bars = L.ring + (uint32_t)stages * L.raw_stage;
+  L.total = L.bars + 8 * MAX_STAGES;
   return L;
 }
 
-__device__ __forceinline__ void split_tile(uint32_t hi_addr, uint32_t lo_addr, uint32_t bytes, int tid) {
-  // elementwise, so the 128B swizzle pattern written by TMA is preserved in both copies.  The "hi" operand is the staged fp32 tile
-  // itself: kind::tf32 reads the top 19 bits of each 32-bit container and ignores the low 13 mantissa bits — the truncation the
-  // residual below is computed against — so only the lo plane is written (one third less shared-memory traffic for the splitters).
-  for (uint32_t off = (uint32_t)tid * 16; off < bytes; off += 128 * 16) {
-    uint32_t x0, x1, x2, x3;
-    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(x0), "=r"(x1), "=r"(x2), "=r"(x3) : "r"(hi_addr + off));
-    const uint32_t h0 = x0 & 0xFFFFE000u, h1 = x1 & 0xFFFFE000u, h2 = x2 & 0xFFFFE000u, h3 = x3 & 0xFFFFE000u;
-    const float l0 = __uint_as_float(x0) - __uint_as_float(h0);
-    const float l1 = __uint_as_float(x1) - __uint_as_float(h1);
-    const float l2 = __uint_as_float(x2) - __uint_as_float(h2);
-    const float l3 = __uint_as_float(x3) - __uint_as_float(h3);
-    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(lo_addr + off), "f"(l0), "f"(l1), "f"(l2), "f"(l3) : "memory");
+// raw tile (rows x 32 k, K-contiguous [row][k] or row-contiguous [k][row]) → K-major swizzled tf32 plane(s)
+__device__ __forceinline__ void convert_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int rows, int mn, int x3, int tid) {
+  for (int c = tid; c < rows * (BK / 4); c += THREADS) {
+    int r, kc;
+    float4 v;
+    if (!mn) {
+      r = c >> 3; kc = c & 7;
+      v = *reinterpret_cast<const float4*>(raw + r * 128 + kc * 16);
+    } else {
+      r = c % rows; kc = c / rows;
+      const float* col = reinterpret_cast<const float*>(raw) + r;
+      v = make_float4(col[(kc * 4 + 0) * rows], col[(kc * 4 + 1) * rows], col[(kc * 4 + 2) * rows], col[(kc * 4 + 3) * rows]);
+    }
+    const uint32_t off = sw128_offset32((uint32_t)r, (uint32_t)kc * 4);
+    if (x3) {
+      const float4 h = make_float4(__uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u), __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u),
+                                   __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u), __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u));
+      *reinterpret_cast<float4*>(hi + off) = h;
+      *reinterpret_cast<float4*>(lo + off) = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
+    } else {
+      *reinterpret_cast<float4*>(hi + off) = v;
+    }
   }
 }
 
+template <int BN>
+__device__ __forceinline__ void mma_ss(float (&d)[BN / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
+  if constexpr (BN == 32) wgmma_tf32_ss_n32(d, a, b, scale_d);
+  else if constexpr (BN == 64) wgmma_tf32_ss_n64(d, a, b, scale_d);
+  else wgmma_tf32_ss_n128(d, a, b, scale_d);
+}
+
+template <int BN, bool X3>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment is required by the 128B swizzle atoms
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const StageLayout L = stage_layout(p.BN, p.x3);
-  const uint32_t smem_base = smem_u32(smem);
-  uint8_t* bar_area = smem + (size_t)p.stages * L.stage_bytes;
-  const uint32_t bars = smem_u32(bar_area);
-  // barrier slots (8 bytes each)
-  const uint32_t full_bar = bars;                               // [stages]
-  const uint32_t split_bar = bars + 8 * MAX_STAGES;             // [stages]
-  const uint32_t empty_bar = bars + 16 * MAX_STAGES;            // [stages]
-  const uint32_t tfull_bar = bars + 24 * MAX_STAGES;            // [2]
-  const uint32_t tempty_bar = tfull_bar + 16;                   // [2]
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(bar_area + 24 * MAX_STAGES + 32);
+  const SmemLayout L = smem_layout(BN, p.x3, p.stages);
+  const uint32_t full_bar = smem_u32(smem + L.bars);
+  const int tid = threadIdx.x, wg = tid >> 7, lt = tid & 127;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  // accumulator ring: 2 stages; in 3xTF32 mode each stage holds TWO accumulators (big = hi·hi, small = lo·hi + hi·lo)
-  const uint32_t acc_stride = (uint32_t)(p.x3 ? 2 * p.BN : p.BN);
-  const uint32_t need_cols = 2 * acc_stride;
-  const uint32_t tmem_cols = need_cols <= 32 ? 32 : (need_cols <= 64 ? 64 : (need_cols <= 128 ? 128 : (need_cols <= 256 ? 256 : 512)));
+  const int u = blockIdx.x;
+  const int ks = u % p.splits;
+  const int t = u / p.splits;
+  const int tn = t % p.tiles_n, tm = t / p.tiles_n;
+  const int kb0 = ks * p.kb_per_split;
+  const int nk = max(0, min(p.kb_total, kb0 + p.kb_per_split) - kb0);
 
-  if (warp == 0 && lane == 0) {
+  if (tid == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmB);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < p.stages; ++s) {
-      mbar_init(full_bar + 8 * s, 1);
-      mbar_init(split_bar + 8 * s, 4);     // one arrival per splitter warp
-      mbar_init(empty_bar + 8 * s, 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar + 8 * a, 1);
-      mbar_init(tempty_bar + 8 * a, 4);    // one arrival per epilogue warp
-    }
+    for (int s = 0; s < p.stages; ++s) mbar_init(full_bar + 8 * s, 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  auto issue = [&](int i) {
+    const int s = i % p.stages, kb = kb0 + i;
+    const uint32_t fb = full_bar + 8 * s;
+    const uint32_t ra = smem_u32(smem + L.ring + s * L.raw_stage), rb = ra + L.raw_a;
+    mbar_expect_tx(fb, L.raw_stage);
+    if (!p.a_mn) tma_load_2d(ra, &p.tmA, fb, kb * BK, tm * BM);
+    else tma_load_2d(ra, &p.tmA, fb, tm * BM, kb * BK);
+    if (!p.b_mn) tma_load_2d(rb, &p.tmB, fb, kb * BK, tn * BN);
+    else tma_load_2d(rb, &p.tmB, fb, tn * BN, kb * BK);
+  };
+  if (tid == 0)
+    for (int i = 0; i < min(nk, p.stages); ++i) issue(i);
 
-  const int units = p.tiles_m * p.tiles_n * p.splits;
+  float acc[BN / 2], acc_s[BN / 2];     // hi·hi and the two cross terms (3xTF32)
+#pragma unroll
+  for (int j = 0; j < BN / 2; ++j) { acc[j] = 0.f; acc_s[j] = 0.f; }
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t tx_bytes = A_TILE_BYTES + L.b_bytes;
-      for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        const int ks = u % p.splits;
-        const int t = u / p.splits;
-        const int tn = t % p.tiles_n, tm = t / p.tiles_n;
-        const int kb0 = ks * p.kb_per_split;
-        const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(empty_bar + 8 * stage, phase ^ 1);
-          const uint32_t fb = full_bar + 8 * stage;
-          mbar_expect_tx(fb, tx_bytes);
-          const uint32_t sa = smem_base + stage * L.stage_bytes + L.a_hi;
-          const uint32_t sb = smem_base + stage * L.stage_bytes + L.b_hi;
-          if (!p.a_mn) {
-            tma_load_2d(sa, &p.tmA, fb, kb * BK, tm * BM);
-          } else {
+  for (int i = 0; i < nk; ++i) {
+    const int s = i % p.stages;
+    uint8_t* planes = smem + (i & 1) * L.plane_buf;
+    uint8_t* a_hi = planes;
+    uint8_t* a_lo = planes + L.a_plane;
+    uint8_t* b_hi = planes + (p.x3 ? 2 : 1) * L.a_plane;
+    uint8_t* b_lo = b_hi + L.b_plane;
+    mbar_wait(full_bar + 8 * s, (uint32_t)((i / p.stages) & 1));
+    const uint8_t* raw = smem + L.ring + s * L.raw_stage;
+    convert_tile(raw, a_hi, a_lo, BM, p.a_mn, p.x3, tid);
+    convert_tile(raw + L.raw_a, b_hi, b_lo, BN, p.b_mn, p.x3, tid);
+    fence_proxy_async();                       // generic-proxy plane writes → visible to the tensor core (async proxy)
+    __syncthreads();                           // planes complete; the raw stage is free again
+    if (tid == 0 && i + p.stages < nk) issue(i + p.stages);
+    wgmma_fence();
+    const uint32_t ah = smem_u32(a_hi) + wg * 64 * 128, al = smem_u32(a_lo) + wg * 64 * 128;
+    const uint32_t bh = smem_u32(b_hi), bl = smem_u32(b_lo);
 #pragma unroll
-            for (int at = 0; at < BM / 32; ++at) tma_load_2d(sa + at * ATOM_BYTES, &p.tmA, fb, tm * BM + at * 32, kb * BK);
-          }
-          if (!p.b_mn) {
-            tma_load_2d(sb, &p.tmB, fb, kb * BK, tn * p.BN);
-          } else {
-            for (int at = 0; at < p.BN / 32; ++at) tma_load_2d(sb + at * ATOM_BYTES, &p.tmB, fb, tn * p.BN + at * 32, kb * BK);
-          }
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
+    for (int k = 0; k < BK / UK; ++k) {
+      const uint32_t ko = k * UK * 4;
+      if (X3) {
+        mma_ss<BN>(acc_s, wgmma_desc_sw128(al + ko), wgmma_desc_sw128(bh + ko), 1);
+        mma_ss<BN>(acc_s, wgmma_desc_sw128(ah + ko), wgmma_desc_sw128(bl + ko), 1);
       }
+      mma_ss<BN>(acc, wgmma_desc_sw128(ah + ko), wgmma_desc_sw128(bh + ko), 1);
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // the whole warp runs the role; each k-block's MMAs and commits are one single-thread issue region (tc_common.cuh: issued from a
-    // divergent `lane == 0` branch each MMA costs an ELECT / BRA.U.ANY loop plus per-instruction descriptor arithmetic)
-    {
-      const uint32_t idesc = umma_idesc(BM, p.BN, p.a_mn, p.b_mn);
-      const uint32_t a_lbo = p.a_mn ? p.mn_lbo : 16, b_lbo = p.b_mn ? p.mn_lbo : 16;
-      const uint32_t a_kstep = p.a_mn ? 1024u : (uint32_t)(UK * 4), b_kstep = p.b_mn ? 1024u : (uint32_t)(UK * 4);
-      const uint32_t a_sbo = p.a_mn ? p.mn_sbo : 1024u, b_sbo = p.b_mn ? p.mn_sbo : 1024u;
-      const uint32_t a_lay = p.a_mn ? p.mn_layout : 2u, b_lay = p.b_mn ? p.mn_layout : 2u;
-      const uint32_t a_hiw = umma_desc_hi(a_sbo, a_lay), b_hiw = umma_desc_hi(b_sbo, b_lay);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0;
-      for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        const int ks = u % p.splits;
-        const int kb0 = ks * p.kb_per_split;
-        const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-        mbar_wait(tempty_bar + 8 * acc, acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)acc * acc_stride;
-        const uint32_t d_small = d_tmem + (uint32_t)p.BN;
-        uint32_t accumulate = 0;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait((p.x3 ? split_bar : full_bar) + 8 * stage, phase);
-          tc_fence_after();
-          const uint32_t st = smem_base + stage * L.stage_bytes;
-          if (elect_one_pred()) {
-            // single-thread issue region (tc_common.cuh): 32-bit descriptor words; the start-address field counts 16-byte units in
-            // the low 14 bits (shared memory < 256 KB), so a k-step advances the low word by kstep / 16
-            const uint32_t a_hi0 = umma_desc_lo(st + L.a_hi, a_lbo), b_hi0 = umma_desc_lo(st + L.b_hi, b_lbo);
-            const uint32_t a_lo0 = umma_desc_lo(st + L.a_lo, a_lbo), b_lo0 = umma_desc_lo(st + L.b_lo, b_lbo);
-            uint32_t accf = accumulate;
-#pragma unroll
-            for (int k = 0; k < BK / UK; ++k) {
-              const uint32_t ak = (k * a_kstep) >> 4, bk = (k * b_kstep) >> 4;
-              if (p.x3) {
-                // The TMEM accumulate truncates (measured: error grows linearly with the number of accumulations),
-                // so the two small cross terms go to their own accumulator: the big one sees 1/3 of the additions
-                // and the small one's truncation is ~2^-11 smaller in absolute terms.  Summed (RN) in the epilogue.
-                umma_tf32_lo(d_small, a_lo0 + ak, a_hiw, b_hi0 + bk, b_hiw, idesc, accf);
-                umma_tf32_lo(d_small, a_hi0 + ak, a_hiw, b_lo0 + bk, b_hiw, idesc, 1);
-                umma_tf32_lo(d_tmem, a_hi0 + ak, a_hiw, b_hi0 + bk, b_hiw, idesc, accf);
-              } else {
-                umma_tf32_lo(d_tmem, a_hi0 + ak, a_hiw, b_hi0 + bk, b_hiw, idesc, accf);
-              }
-              accf = 1;
-            }
-            umma_commit(empty_bar + 8 * stage);                        // frees the smem stage once these MMAs have read it
-            if (kb == kb1 - 1) umma_commit(tfull_bar + 8 * acc);       // accumulator complete → epilogue
-          }
-          __syncwarp();
-          accumulate = 1;
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
-        if (kb1 <= kb0) {                                // empty K range: nothing was issued, the epilogue still expects the hand-over
-          if (elect_one_pred()) umma_commit(tfull_bar + 8 * acc);
-          __syncwarp();
-        }
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-    __syncwarp();
-  } else if (warp >= 8) {
-    // ===================== splitter warps (3xTF32) =====================
-    if (p.x3) {
-      const int tid = threadIdx.x - 8 * 32;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int u = blockIdx.x; u < units; u += gridDim.x) {
-        const int ks = u % p.splits;
-        const int kb0 = ks * p.kb_per_split;
-        const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar + 8 * stage, phase);
-          const uint32_t st = smem_base + stage * L.stage_bytes;
-          split_tile(st + L.a_hi, st + L.a_lo, A_TILE_BYTES, tid);
-          split_tile(st + L.b_hi, st + L.b_lo, L.b_bytes, tid);
-          fence_proxy_async();                   // generic-proxy writes → visible to the tensor core (async proxy)
-          __syncwarp();
-          if (lane == 0) mbar_arrive(split_bar + 8 * stage);
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue warps =====================
-    const int sub = warp & 3;                    // TMEM sub-partition this warp may read
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    const bool vec_ok = ((p.ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
-    for (int u = blockIdx.x; u < units; u += gridDim.x) {
-      const int ks = u % p.splits;
-      const int t = u / p.splits;
-      const int tn = t % p.tiles_n, tm = t / p.tiles_n;
-      mbar_wait(tfull_bar + 8 * acc, acc_phase);
-      tc_fence_after();
-      const int row = tm * BM + sub * 32 + lane;
-      for (int c0 = 0; c0 < p.BN; c0 += 32) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem_base + ((uint32_t)(sub * 32) << 16) + (uint32_t)acc * acc_stride + (uint32_t)c0;
-        tmem_ld_32x32b_x32(taddr, v);
-        if (p.x3) {
-          uint32_t w[32];
-          tmem_ld_32x32b_x32(taddr + (uint32_t)p.BN, w);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(w[j]));
-        }
-        const int col0 = tn * p.BN + c0;
-        if (row < p.M && col0 < p.N) {
-          if (p.partial) {
-            float* dst = p.partial + ((size_t)ks * p.M + row) * p.N + col0;
-            const bool pv = ((p.N & 3) == 0);
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              if (pv && col0 + j + 3 < p.N) {
-                *reinterpret_cast<float4*>(dst + j) = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                                                  __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-              } else {
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) if (col0 + j + jj < p.N) dst[j + jj] = __uint_as_float(v[j + jj]);
-              }
-            }
-          } else {
-            float* dst = p.C + (size_t)row * p.ldc + col0;
-            const float* mrow = p.mask ? p.mask + (size_t)row * p.ldmask + col0 : nullptr;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              float o[4];
-#pragma unroll
-              for (int jj = 0; jj < 4; ++jj) {
-                const int col = col0 + j + jj;
-                float x = __uint_as_float(v[j + jj]);
-                if (col < p.N) {
-                  if (p.bias) x += __ldg(p.bias + col);
-                  x = apply_act(x, p.act);
-                  if (mrow && !(__ldg(mrow + j + jj) > 0.f)) x = 0.f;
-                  if (p.beta != 0.f) x = fmaf(p.beta, dst[j + jj], x);
-                }
-                o[jj] = x;
-              }
-              if (vec_ok && col0 + j + 3 < p.N) {
-                *reinterpret_cast<float4*>(dst + j) = make_float4(o[0], o[1], o[2], o[3]);
-              } else {
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) if (col0 + j + jj < p.N) dst[j + jj] = o[jj];
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar + 8 * acc);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
+    wgmma_commit();
+    wgmma_wait<1>();                           // the MMAs of k-block i-1 are done: their plane buffer may be rewritten
+    __syncthreads();                           // ... by every warpgroup
   }
+  wgmma_wait<0>();
+  reg_fence(acc);
+  reg_fence(acc_s);
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
+  // ===================== epilogue: straight from the accumulator registers =====================
+  const int warp = lt >> 5, lane = lt & 31;
+  const int row_base = tm * BM + wg * 64 + warp * 16 + (lane >> 2);
+  const bool vec_ok = ((p.ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
+#pragma unroll
+  for (int v = 0; v < BN / 2; v += 2) {
+    const int row = row_base + 8 * ((v >> 1) & 1);
+    const int col = tn * BN + 8 * (v >> 2) + 2 * (lane & 3);
+    if (row >= p.M || col >= p.N) continue;
+    float o[2] = {acc[v] + acc_s[v], acc[v + 1] + acc_s[v + 1]};
+    const bool two = col + 1 < p.N;
+    if (p.partial) {
+      float* dst = p.partial + ((size_t)ks * p.M + row) * p.N + col;
+      dst[0] = o[0];
+      if (two) dst[1] = o[1];
+      continue;
+    }
+    float* dst = p.C + (size_t)row * p.ldc + col;
+    const float* mrow = p.mask ? p.mask + (size_t)row * p.ldmask + col : nullptr;
+#pragma unroll
+    for (int jj = 0; jj < 2; ++jj) {
+      if (jj == 1 && !two) break;
+      float x = o[jj];
+      if (p.bias) x += __ldg(p.bias + col + jj);
+      x = apply_act(x, p.act);
+      if (mrow && !(__ldg(mrow + jj) > 0.f)) x = 0.f;
+      if (p.beta != 0.f) x = fmaf(p.beta, dst[jj], x);
+      o[jj] = x;
+    }
+    if (two && vec_ok) *reinterpret_cast<float2*>(dst) = make_float2(o[0], o[1]);
+    else { dst[0] = o[0]; if (two) dst[1] = o[1]; }
   }
 }
 
@@ -365,7 +241,6 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-// 2-D fp32 tensor map: `inner` contiguous elements, `outer` rows `ld` elements apart; box = {32, box_outer}
 // general 2-D fp32 tensor map: box = {box_inner, box_outer}; swizzle: 0 none, 1 32B, 2 64B, 3 128B, 4 128B_ATOM_32B
 bool make_tensor_map_f32_ex(CUtensorMap* map, const float* ptr, uint64_t inner, uint64_t outer, uint64_t ld, uint32_t box_inner,
                             uint32_t box_outer, int swizzle) {
@@ -393,12 +268,6 @@ bool make_tensor_map_f16_ex(CUtensorMap* map, const void* ptr, uint64_t inner, u
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-bool make_tensor_map_f32(CUtensorMap* map, const float* ptr, uint64_t inner, uint64_t outer, uint64_t ld, uint32_t box_outer,
-                         bool mn_major) {
-  const int mn_swz = (int)CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B;
-  return make_tensor_map_f32_ex(map, ptr, inner, outer, ld, 32, box_outer, mn_major ? mn_swz : (int)CU_TENSOR_MAP_SWIZZLE_128B);
-}
-
 struct Plan {
   int BN, stages, tiles_m, tiles_n, splits, kb_per_split, kb_total;
   size_t smem;
@@ -407,13 +276,11 @@ struct Plan {
 static Plan make_plan(int M, int N, int K, int x3) {
   Plan pl;
   pl.BN = N <= 32 ? 32 : (N <= 64 ? 64 : 128);
-  const StageLayout L = stage_layout(pl.BN, x3);
-  const size_t budget = 200 * 1024;
-  int stages = (int)(budget / L.stage_bytes);
+  const SmemLayout L0 = smem_layout(pl.BN, x3, 0);
+  int stages = (int)((SMEM_LIMIT - 1024 - L0.total) / L0.raw_stage);
   if (stages > MAX_STAGES) stages = MAX_STAGES;
-  if (stages < 2) stages = 2;
-  pl.stages = stages;
-  pl.smem = (size_t)stages * L.stage_bytes + 1024 /*align slack*/ + 24 * MAX_STAGES + 64;
+  pl.stages = stages;               // ≥ 2 for every BN (128 KB of planes + 2 x 32 KB raw stages at BN = 128, 3xTF32)
+  pl.smem = (size_t)smem_layout(pl.BN, x3, stages).total + 1024 /*align slack*/;
   pl.tiles_m = ceil_div(M, BM);
   pl.tiles_n = ceil_div(N, pl.BN);
   pl.kb_total = ceil_div(K, BK);
@@ -429,6 +296,18 @@ static Plan make_plan(int M, int N, int K, int x3) {
   pl.kb_per_split = ceil_div(pl.kb_total, splits);
   pl.splits = ceil_div(pl.kb_total, pl.kb_per_split);
   return pl;
+}
+
+template <int BN, bool X3>
+static int launch_gemm(const Params& p, const Plan& pl, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    B2_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    attr_set = true;
+  }
+  gemm_tc_kernel<BN, X3><<<pl.tiles_m * pl.tiles_n * pl.splits, THREADS, pl.smem, st>>>(p);
+  B2_CHECK_LAUNCH("gemm_tc_kernel");
+  return B2_OK;
 }
 
 }  // namespace tc
@@ -453,21 +332,20 @@ int gemm_tc(const float* A, int64_t lda, int transA, const float* B, int64_t ldb
   const Plan pl = make_plan(M, N, K, x3);
   Params p;
   memset(&p, 0, sizeof(p));
-  // A operand: K-major when A is [M,K] row-major, MN-major when stored [K,M]
-  const bool okA = transA ? make_tensor_map_f32(&p.tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, BK, true)
-                          : make_tensor_map_f32(&p.tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BM, false);
-  // B operand (UMMA B is N x K): K-major when B is stored [N,K] (transB), MN-major when [K,N]
-  const bool okB = transB ? make_tensor_map_f32(&p.tmB, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, (uint32_t)pl.BN, false)
-                          : make_tensor_map_f32(&p.tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, BK, true);
+  // raw tiles, unswizzled: A is [M,K] row-major (box 32 k x 128 rows) or stored [K,M] (box 128 rows x 32 k); B likewise
+  const int NONE = (int)CU_TENSOR_MAP_SWIZZLE_NONE;
+  const bool okA = transA ? make_tensor_map_f32_ex(&p.tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, BM, BK, NONE)
+                          : make_tensor_map_f32_ex(&p.tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda, BK, BM, NONE);
+  const bool okB = transB ? make_tensor_map_f32_ex(&p.tmB, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb, BK, (uint32_t)pl.BN, NONE)
+                          : make_tensor_map_f32_ex(&p.tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, (uint32_t)pl.BN, BK, NONE);
   if (!okA || !okB) return B2_ERR_UNSUPPORTED;
   p.C = C; p.bias = bias; p.mask = mask; p.ldc = ldc; p.ldmask = ldmask;
-  p.M = M; p.N = N; p.K = K; p.BN = pl.BN;
+  p.M = M; p.N = N; p.K = K;
   p.a_mn = transA ? 1 : 0;
   p.b_mn = transB ? 0 : 1;
   p.x3 = x3; p.act = act; p.beta = beta;
   p.tiles_m = pl.tiles_m; p.tiles_n = pl.tiles_n; p.splits = pl.splits; p.kb_per_split = pl.kb_per_split;
   p.kb_total = pl.kb_total; p.stages = pl.stages;
-  p.mn_lbo = ATOM_BYTES; p.mn_sbo = 512; p.mn_layout = 1;
   p.partial = nullptr;
   if (pl.splits > 1) {
     const size_t need = (size_t)pl.splits * M * N * sizeof(float);
@@ -477,15 +355,9 @@ int gemm_tc(const float* A, int64_t lda, int transA, const float* B, int64_t ldb
     }
     p.partial = reinterpret_cast<float*>(workspace);
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  const int units = pl.tiles_m * pl.tiles_n * pl.splits;
-  const int grid = units < sm_count() ? units : sm_count();
-  gemm_tc_kernel<<<grid, THREADS, pl.smem, st>>>(p);
-  B2_CHECK_LAUNCH("gemm_tc_kernel");
+  const int rc = x3 ? (pl.BN == 32 ? launch_gemm<32, true>(p, pl, st) : (pl.BN == 64 ? launch_gemm<64, true>(p, pl, st) : launch_gemm<128, true>(p, pl, st)))
+                    : (pl.BN == 32 ? launch_gemm<32, false>(p, pl, st) : (pl.BN == 64 ? launch_gemm<64, false>(p, pl, st) : launch_gemm<128, false>(p, pl, st)));
+  if (rc != B2_OK) return rc;
   if (pl.splits > 1) {
     size_t total = (size_t)M * N;
     int blocks = (int)((total + 255) / 256);

@@ -280,7 +280,7 @@ static size_t cand_smem_bytes(int M) {
 // `need` = number of sorted ranks that must be recovered (k, +1 when rank 0 is dropped); 8 spare candidates
 static int choose_M(int need) { return (need + 8 <= 32) ? 32 : 64; }
 
-namespace ktc {   // knn_tc.cu: tcgen05 candidate filter
+namespace ktc {   // knn_tc.cu: tensor-core candidate filter
 size_t workspace_bytes(int32_t n, int32_t d, int32_t n_q);
 bool eligible(int32_t n, int32_t d, int32_t n_q, int M);
 float tc_err_rel(int32_t d);

@@ -1,19 +1,19 @@
 // Tensor-core candidate filter for the exact kNN search (phase 1 of knn.cu: the N²·d part).
 //
-// One CTA owns 128 queries and streams every 128-reference tile through a TMA ring:
-//   S = Q · Rᵀ            tcgen05.mma kind::f16 on fp16 (hi, lo) pairs of 2^e·x (22 significant bits; hi·hi + hi·lo + lo·hi),
-//                         fp32 accumulation in TMEM, K = padded feature width (16 per instruction)
-//   d̂² = |q|² + |r|² − 2·S/4^e   four selection warps (TMEM lane = query row) read the 128 estimates of their query straight
-//                         from TMEM and keep the M smallest in an UNSORTED per-query list held in registers (replace-the-maximum:
-//                         32 predicated moves + a 32-entry rescan per insertion; insertions are warp-divergent and some lane
-//                         hits in ≈ 95 % of the 32-estimate chunks, so their cost — not their count, ≈ M·ln(n/M) per query —
-//                         is what matters; the refine pass ranks the candidates anyway)
+// One CTA (one warpgroup) owns 64 queries and streams every 64-reference tile through a TMA ring:
+//   S = Q · Rᵀ            wgmma.mma_async m64n64k16 on fp16 (hi, lo) pairs of 2^e·x (22 significant bits; hi·hi + hi·lo + lo·hi),
+//                         fp32 accumulation in registers, K = padded feature width (16 per instruction); the accumulators are
+//                         written to shared memory so that a thread can read a query's row
+//   d̂² = |q|² + |r|² − 2·S/4^e   two threads per query (one per half of the tile's columns) keep the M smallest estimates they
+//                         see in an UNSORTED list held in registers (replace-the-maximum: 32 predicated moves + a 32-entry
+//                         rescan per insertion); at the end the second half's list is inserted into the first's, which then
+//                         holds the M smallest estimates of the query over all references
 // The estimates only FILTER: phase 2 (knn_refine_kernel) re-ranks the candidates in fp64 exactly like the reference and
 // proves with an error bound that no non-candidate can enter the top-k; unproven queries fall back to fp64 brute force.
-// The bound for this filter is documented at `tc_err_rel` below.  Replaces the 26 TFLOP/s SIMT filter (10 s at 1 M × 128).
+// The bound for this filter is documented at `tc_err_rel` below.
 //
 // Operand layout: Xh / Xl [n, dp] halves (dp = d rounded up to 64 = one 128-byte swizzle atom per 64 features), K-major
-// SWIZZLE_128B boxes {64 halves, 128 rows}; an operand tile is dp/64 atoms of 16 KB.
+// SWIZZLE_128B boxes {64 halves, 64 rows}; an operand tile is dp/64 atoms of 8 KB.
 #include "tc_common.cuh"
 
 #include <cuda_fp16.h>
@@ -26,23 +26,23 @@ namespace ktc {
 
 using namespace tc;
 
-constexpr int BQ = 128;          // queries per CTA (UMMA M)
-constexpr int BR = 128;          // references per tile (UMMA N)
+constexpr int BQ = 64;           // queries per CTA (wgmma M)
+constexpr int BR = 64;           // references per tile (wgmma N)
 constexpr int MC = 32;           // candidates kept per query
 constexpr int MAX_ATOMS = 2;     // dp <= 128
-constexpr int ATOM_BYTES = 128 * 128;   // 128 rows x 128 B
-constexpr int THREADS = 256;     // warps: 0 TMA, 1 MMA, 2 TMEM alloc, 3 idle, 4..7 selection
-constexpr uint32_t TM_COLS = 256;  // two D buffers of 128 fp32 columns
+constexpr int ATOM_BYTES = 64 * 128;   // 64 rows x 128 B
+constexpr int THREADS = 128;
+constexpr int STAGES = 2;
+constexpr int S_PITCH = BR + 4;  // floats per row of the estimate tile (16-byte rows, conflict-free float4 reads)
 
 struct Params {
-  CUtensorMap m_hi, m_lo;        // [n, dp] halves, box {64, 128}, SWIZZLE_128B
+  CUtensorMap m_hi, m_lo;        // [n, dp] halves, box {64, 64}, SWIZZLE_128B
   const float* sqn;              // |x|² (fp32, unscaled)
   const float* scale;            // scale[1] = 4^-e
   int32_t* cand_idx;             // [n_q, MC]
   float* cand_thr;               // [n_q]
-  int n, n_q, q_begin, atoms, stages;
+  int n, n_q, q_begin, atoms;
 };
-
 // max |x| → 2^e with max·2^e ∈ [256, 512);  scale[0] = 2^e, scale[1] = 4^-e
 __global__ void __launch_bounds__(256)
 absmax_kernel(const float* __restrict__ X, int64_t ldx, int32_t n, int32_t d, uint32_t* __restrict__ maxbits) {
@@ -78,177 +78,156 @@ split_kernel(const float* __restrict__ X, int64_t ldx, int32_t n, int32_t d, int
   }
 }
 
-__global__ void __launch_bounds__(THREADS, 1)
+struct CandList {
+  float key[MC];
+  int32_t kid[MC];
+  int maxslot;                     // slot currently holding the largest kept estimate (= thr)
+  float thr;
+  __device__ __forceinline__ void init() {
+    maxslot = 0;
+    thr = CUDART_INF_F;
+#pragma unroll
+    for (int s = 0; s < MC; ++s) { key[s] = CUDART_INF_F; kid[s] = -1; }
+  }
+  __device__ __forceinline__ void insert(float e, int32_t id) {
+#pragma unroll
+    for (int s = 0; s < MC; ++s)
+      if (s == maxslot) { key[s] = e; kid[s] = id; }
+    float mx = key[0];
+    maxslot = 0;
+#pragma unroll
+    for (int s = 1; s < MC; ++s)
+      if (key[s] > mx) { mx = key[s]; maxslot = s; }
+    thr = mx;
+  }
+};
+
+__global__ void __launch_bounds__(THREADS)
 knn_candidates_tc_kernel(const __grid_constant__ Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int op_bytes = p.atoms * ATOM_BYTES;                 // one operand part (hi or lo) of one tile
   const uint32_t s_q_hi = smem_u32(smem), s_q_lo = s_q_hi + op_bytes;
-  const uint32_t s_ring = s_q_lo + op_bytes;                 // [stages][hi | lo]
-  uint8_t* bar_area = smem + 2 * op_bytes + p.stages * 2 * op_bytes;
-  const uint32_t bars = smem_u32(bar_area);
-  const uint32_t q_bar = bars;                      // 1
-  const uint32_t full_bar = bars + 8;               // [4] TMA → MMA
-  const uint32_t stage_free = full_bar + 32;        // [4] MMA commit → TMA
-  const uint32_t d_full = stage_free + 32;          // [2] MMA commit → selection
-  const uint32_t d_empty = d_full + 16;             // [2] selection → MMA
-  volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(bar_area + 128);
+  const uint32_t s_ring = s_q_lo + op_bytes;                 // [STAGES][hi | lo]
+  float* S = reinterpret_cast<float*>(smem + (2 + 2 * STAGES) * op_bytes);   // [BQ][S_PITCH] estimates of the current tile
+  const uint32_t q_bar = smem_u32(S + BQ * S_PITCH);
+  const uint32_t full_bar = q_bar + 8;              // [STAGES]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int q0 = blockIdx.x * BQ;                   // local query offset
   const int n_tiles = (p.n + BR - 1) / BR;
 
-  if (warp == 0 && lane == 0) { tma_prefetch_desc(&p.m_hi); tma_prefetch_desc(&p.m_lo); }
-  if (warp == 1 && lane == 0) {
+  if (tid == 0) {
+    tma_prefetch_desc(&p.m_hi);
+    tma_prefetch_desc(&p.m_lo);
     mbar_init(q_bar, 1);
-    for (int s = 0; s < 4; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(stage_free + 8 * s, 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(d_full + 8 * b, 1); mbar_init(d_empty + 8 * b, 4); }
+    for (int s = 0; s < STAGES; ++s) mbar_init(full_bar + 8 * s, 1);
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(smem_u32(const_cast<uint32_t*>(tmem_slot)), TM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
+  auto issue = [&](int t) {
+    const int s = t % STAGES;
+    const uint32_t fb = full_bar + 8 * s, st = s_ring + s * 2 * op_bytes;
+    mbar_expect_tx(fb, 2 * op_bytes);
+    for (int a = 0; a < p.atoms; ++a) {
+      tma_load_2d(st + a * ATOM_BYTES, &p.m_hi, fb, a * 64, t * BR);
+      tma_load_2d(st + op_bytes + a * ATOM_BYTES, &p.m_lo, fb, a * 64, t * BR);
+    }
+  };
+  if (tid == 0) {
+    mbar_expect_tx(q_bar, 2 * op_bytes);
+    for (int a = 0; a < p.atoms; ++a) {
+      tma_load_2d(s_q_hi + a * ATOM_BYTES, &p.m_hi, q_bar, a * 64, p.q_begin + q0);
+      tma_load_2d(s_q_lo + a * ATOM_BYTES, &p.m_lo, q_bar, a * 64, p.q_begin + q0);
+    }
+    for (int t = 0; t < min(n_tiles, STAGES); ++t) issue(t);
+  }
 
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(q_bar, 2 * op_bytes);
-      for (int a = 0; a < p.atoms; ++a) {
-        tma_load_2d(s_q_hi + a * ATOM_BYTES, &p.m_hi, q_bar, a * 64, p.q_begin + q0);
-        tma_load_2d(s_q_lo + a * ATOM_BYTES, &p.m_lo, q_bar, a * 64, p.q_begin + q0);
-      }
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = 0; t < n_tiles; ++t) {
-        mbar_wait(stage_free + 8 * stage, phase ^ 1);
-        const uint32_t fb = full_bar + 8 * stage, st = s_ring + stage * 2 * op_bytes;
-        mbar_expect_tx(fb, 2 * op_bytes);
-        for (int a = 0; a < p.atoms; ++a) {
-          tma_load_2d(st + a * ATOM_BYTES, &p.m_hi, fb, a * 64, t * BR);
-          tma_load_2d(st + op_bytes + a * ATOM_BYTES, &p.m_lo, fb, a * 64, t * BR);
-        }
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_f16(BQ, BR, 0, 0);
-      mbar_wait(q_bar, 0);
-      tc_fence_after();
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = 0; t < n_tiles; ++t) {
-        const int b = t & 1;
-        mbar_wait(d_empty + 8 * b, ((t >> 1) & 1) ^ 1);
-        mbar_wait(full_bar + 8 * stage, phase);
-        tc_fence_after();
-        const uint32_t st = s_ring + stage * 2 * op_bytes;
-        const uint32_t d_t = tmem + (uint32_t)(b * BR);
-        uint32_t acc = 0;
-        for (int a = 0; a < p.atoms; ++a) {
+  // selection role: query ql, columns [half·32, half·32 + 32) of every tile (warps 0-1: first half, warps 2-3: second half)
+  const int ql = tid & (BQ - 1), half = tid >> 6;
+  const int q = q0 + ql;
+  const float inv_s2 = p.scale[1];
+  const bool live = q < p.n_q;
+  const float qn = live ? p.sqn[p.q_begin + q] : 0.f;
+  const float m2 = -2.f * inv_s2;
+  CandList cl;
+  cl.init();
+  mbar_wait(q_bar, 0);
+
+  for (int t = 0; t < n_tiles; ++t) {
+    const int s = t % STAGES;
+    mbar_wait(full_bar + 8 * s, (uint32_t)((t / STAGES) & 1));
+    const uint32_t st = s_ring + s * 2 * op_bytes;
+    float acc[BR / 2];
+    wgmma_fence();
+    for (int a = 0; a < p.atoms; ++a) {
 #pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {             // 64 halves per atom = 4 k-steps of 16
-            const uint32_t off = (uint32_t)(a * ATOM_BYTES + kk * 32);
-            const uint64_t a_hi = umma_desc(s_q_hi + off, 16, 1024, 2), a_lo = umma_desc(s_q_lo + off, 16, 1024, 2);
-            const uint64_t b_hi = umma_desc(st + off, 16, 1024, 2), b_lo = umma_desc(st + op_bytes + off, 16, 1024, 2);
-            umma_f16(d_t, a_lo, b_hi, idesc, acc);
-            umma_f16(d_t, a_hi, b_lo, idesc, 1);
-            umma_f16(d_t, a_hi, b_hi, idesc, 1);
-            acc = 1;
-          }
-        }
-        umma_commit(d_full + 8 * b);
-        umma_commit(stage_free + 8 * stage);
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
+      for (int kk = 0; kk < 4; ++kk) {             // 64 halves per atom = 4 k-steps of 16
+        const uint32_t off = (uint32_t)(a * ATOM_BYTES + kk * 32);
+        wgmma_f16_ss_n64(acc, wgmma_desc_sw128(s_q_lo + off), wgmma_desc_sw128(st + off), (a | kk) != 0);
+        wgmma_f16_ss_n64(acc, wgmma_desc_sw128(s_q_hi + off), wgmma_desc_sw128(st + op_bytes + off), 1);
+        wgmma_f16_ss_n64(acc, wgmma_desc_sw128(s_q_hi + off), wgmma_desc_sw128(st + off), 1);
       }
     }
-    __syncwarp();
-  } else if (warp >= 4) {
-    // ===================== selection warps: thread = query row =====================
-    const int sub = warp & 3;
-    const int ql = sub * 32 + lane;                  // local query
-    const int q = q0 + ql;
-    const uint32_t lane_off = (uint32_t)(sub * 32) << 16;
-    const float inv_s2 = p.scale[1];
-    const bool live = q < p.n_q;
-    const float qn = live ? p.sqn[p.q_begin + q] : 0.f;
-    // the M kept candidates live in REGISTERS (static indexing only): replacing the maximum is 32 predicated moves and the
-    // rescan 32 compares — no memory traffic, one copy of the code (the hit loop below is not unrolled)
-    float key[MC];
-    int32_t kid[MC];
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(acc);
+    __syncthreads();                               // every thread has finished the previous tile's selection and this tile's MMAs
+    if (tid == 0 && t + STAGES < n_tiles) issue(t + STAGES);
+    {
+      const int r = warp * 16 + (lane >> 2);
 #pragma unroll
-    for (int s2 = 0; s2 < MC; ++s2) { key[s2] = CUDART_INF_F; kid[s2] = -1; }
-    int maxslot = 0;                                  // slot currently holding the largest kept estimate (= thr)
-    float thr = CUDART_INF_F;
-    const float m2 = -2.f * inv_s2;
-    for (int t = 0; t < n_tiles; ++t) {
-      const int b = t & 1;
-      mbar_wait(d_full + 8 * b, (t >> 1) & 1);
-      tc_fence_after();
-      const int r0 = t * BR;
-      // |r|² of the tile: four coalesced loads per lane issued up front, then broadcast by shuffle (a per-element load of the
-      // warp-uniform address serialised ~300 cycles of L2 latency per estimate in the first version of this loop)
-      float rn_l[BR / 32];
-#pragma unroll
-      for (int u = 0; u < BR / 32; ++u) {
-        const int r = r0 + u * 32 + lane;
-        rn_l[u] = r < p.n ? __ldg(p.sqn + r) : CUDART_INF_F;
+      for (int v = 0; v < BR / 2; v += 2) {
+        const int c = 8 * (v >> 2) + 2 * (lane & 3);
+        const int rr = r + 8 * ((v >> 1) & 1);
+        *reinterpret_cast<float2*>(S + rr * S_PITCH + c) = make_float2(acc[v], acc[v + 1]);
       }
-#pragma unroll
-      for (int chunk = 0; chunk < BR / 32; ++chunk) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem + lane_off + (uint32_t)(b * BR + chunk * 32), v);
-        float est[32];
-        float mn = CUDART_INF_F;
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          const float rn = __shfl_sync(0xffffffffu, rn_l[chunk], c);
-          est[c] = fmaf(m2, __uint_as_float(v[c]), qn + rn);
-          mn = fminf(mn, est[c]);
-        }
-        uint32_t mask = 0;
-#pragma unroll
-        for (int c = 0; c < 32; ++c) mask |= (est[c] < thr ? 1u : 0u) << c;
-        if (live && mask) {
-          // Per lane ≈ 9 % of the chunks contain a hit, per WARP ≈ 95 % do: the path must be short and exist once.
-          float es[32];                               // dynamic indexing below → local memory, touched only on this path
-#pragma unroll
-          for (int c = 0; c < 32; ++c) es[c] = est[c];
-          while (mask) {
-            const int c = __ffs(mask) - 1;
-            mask &= mask - 1;
-            const float e = es[c];
-            if (e < thr) {                            // thr may have dropped since the mask was built
-              const int32_t rid = r0 + chunk * 32 + c;
-#pragma unroll
-              for (int s2 = 0; s2 < MC; ++s2)
-                if (s2 == maxslot) { key[s2] = e; kid[s2] = rid; }
-              float mx = key[0];
-              maxslot = 0;
-#pragma unroll
-              for (int s2 = 1; s2 < MC; ++s2)
-                if (key[s2] > mx) { mx = key[s2]; maxslot = s2; }
-              thr = mx;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      if (lane == 0) mbar_arrive(d_empty + 8 * b);
     }
-    if (live) {
+    __syncthreads();
+    const int r0 = t * BR + half * 32;
+    // |r|² of the 32 columns: one coalesced load per lane, broadcast by shuffle
+    const float rn_l = r0 + lane < p.n ? __ldg(p.sqn + r0 + lane) : CUDART_INF_F;
+    float est[32];
 #pragma unroll
-      for (int c = 0; c < MC; ++c) p.cand_idx[(int64_t)q * MC + c] = kid[c];
-      p.cand_thr[q] = thr;
+    for (int c = 0; c < 32; c += 4) {
+      const float4 v = *reinterpret_cast<const float4*>(S + ql * S_PITCH + half * 32 + c);
+      est[c] = fmaf(m2, v.x, qn + __shfl_sync(0xffffffffu, rn_l, c));
+      est[c + 1] = fmaf(m2, v.y, qn + __shfl_sync(0xffffffffu, rn_l, c + 1));
+      est[c + 2] = fmaf(m2, v.z, qn + __shfl_sync(0xffffffffu, rn_l, c + 2));
+      est[c + 3] = fmaf(m2, v.w, qn + __shfl_sync(0xffffffffu, rn_l, c + 3));
+    }
+    uint32_t mask = 0;
+#pragma unroll
+    for (int c = 0; c < 32; ++c) mask |= (est[c] < cl.thr ? 1u : 0u) << c;
+    if (live && mask) {
+      float es[32];                                // dynamic indexing below → local memory, touched only on this path
+#pragma unroll
+      for (int c = 0; c < 32; ++c) es[c] = est[c];
+      while (mask) {
+        const int c = __ffs(mask) - 1;
+        mask &= mask - 1;
+        const float e = es[c];
+        if (e < cl.thr) cl.insert(e, r0 + c);      // thr may have dropped since the mask was built
+      }
     }
   }
-  tc_fence_before();
+  // merge: the second half's list goes through shared memory into the first half's
   __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem, TM_COLS);
+  float* mkey = S;
+  int32_t* mid = reinterpret_cast<int32_t*>(S + BQ * MC);
+  if (half == 1) {
+#pragma unroll
+    for (int c = 0; c < MC; ++c) { mkey[ql * MC + c] = cl.key[c]; mid[ql * MC + c] = cl.kid[c]; }
+  }
+  __syncthreads();
+  if (half == 0 && live) {
+    for (int c = 0; c < MC; ++c) {
+      const float e = mkey[ql * MC + c];
+      if (e < cl.thr) cl.insert(e, mid[ql * MC + c]);
+    }
+#pragma unroll
+    for (int c = 0; c < MC; ++c) p.cand_idx[(int64_t)q * MC + c] = cl.kid[c];
+    p.cand_thr[q] = cl.thr;
   }
 }
 
@@ -266,7 +245,7 @@ bool eligible(int32_t n, int32_t d, int32_t n_q, int M) {
 
 // Relative error bound of the filter estimate d̂² w.r.t. (|q| + |r|)²:
 //   operands carry 22 bits (hi + lo, each rounded to nearest)            → |Δ(q·r)| ≤ 2^-21 |q||r| (+ dropped lo·lo 2^-22)
-//   dp/16 · 3 products accumulated in fp32 with TRUNCATING adds in TMEM  → ≤ 3·dp/16 · 2^-23 · |q||r|  (≤ 24 adds → 2^-18.4)
+//   dp/16 · 3 products accumulated in fp32 (bounded as if every add truncated) → ≤ 3·dp/16 · 2^-23 · |q||r|  (≤ 24 adds → 2^-18.4)
 //   norms and the final fma in fp32                                       → (d + 8) · 2^-23 (|q|² + |r|²)
 // 2·|Δ(q·r)| ≤ 2^-17 |q||r| covers the first two lines with margin.
 float tc_err_rel(int32_t d) { return 7.62939453125e-06f + 1.1920928955078125e-07f * (float)(d + 8); }
@@ -304,12 +283,7 @@ int launch(const float* X, int64_t ldx, const float* sqn, int32_t n, int32_t d, 
   p.sqn = sqn; p.scale = scale; p.cand_idx = cand_idx; p.cand_thr = cand_thr;
   p.n = n; p.n_q = n_q; p.q_begin = q_begin; p.atoms = dp / 64;
   const int op_bytes = p.atoms * ATOM_BYTES;
-  const size_t fixed = 2 * (size_t)op_bytes + 256 + 1024;
-  int stages = (int)((232448 - fixed) / (2 * (size_t)op_bytes));
-  if (stages > 4) stages = 4;
-  if (stages < 2) return B2_ERR_UNSUPPORTED;
-  p.stages = stages;
-  const size_t smem = fixed + (size_t)stages * 2 * op_bytes;
+  const size_t smem = (size_t)(2 + 2 * STAGES) * op_bytes + (size_t)BQ * S_PITCH * 4 + 8 * (1 + STAGES) + 1024;
   static size_t attr_smem = 0;
   if (smem > attr_smem) {
     B2_CHECK_CUDA(cudaFuncSetAttribute(knn_candidates_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

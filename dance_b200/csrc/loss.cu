@@ -64,17 +64,8 @@ constexpr int GL_JT = 128;                 // j-tile staged in shared memory
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-// packed fp32 FMA (Blackwell FFMA2): two independent fused multiply-adds per issue slot
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra, rb, rc, rd;
-  asm("mov.b64 %0, {%1,%2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1,%2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mov.b64 %0, {%1,%2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  float2 d;
-  asm("mov.b64 {%0,%1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
-}
+// two independent fused multiply-adds on a feature pair (round-to-nearest, like one packed f32x2 FMA)
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 // All-pairs part: thread t owns rows i0+t and i0+t+GL_THREADS, loops over every column j (tiles in smem,
 // broadcast reads).  Per logit: 2·D FMA (dot + gradient accumulate) and three SFU ops
@@ -82,14 +73,10 @@ __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
 template <int D>
 __global__ void __launch_bounds__(GL_THREADS)
 gae_allpairs_kernel(const float* __restrict__ z, int64_t ldz, int32_t n, int32_t row_begin, int32_t n_rows,
-                    int32_t j_chunk, float coef, float* __restrict__ dz, double* __restrict__ loss_acc,
-                    const float* __restrict__ only_if) {
-  // device-side predicate: the fp16-operand tensor-core kernel of gae_tch.cu steps aside (and raises this flag) when the embedding
-  // is too large for its operand format; this fp32 kernel then does the work, otherwise it returns at once
-  if (only_if && only_if[0] == 0.f) return;
+                    int32_t j_chunk, float coef, float* __restrict__ dz, double* __restrict__ loss_acc) {
   constexpr int GL_RPT = GaeCfg<D>::RPT, GL_ROWS = GaeCfg<D>::ROWS;
   __shared__ __align__(16) float zj[GL_JT][D];
-  float2 zi[GL_RPT][D / 2], acc[GL_RPT][D / 2];   // feature pairs (d, d+1) packed for FFMA2
+  float2 zi[GL_RPT][D / 2], acc[GL_RPT][D / 2];   // feature pairs (d, d+1), two FMA chains each
   bool live[GL_RPT];
 #pragma unroll
   for (int r = 0; r < GL_RPT; ++r) {
@@ -250,27 +237,15 @@ gae_kld_kernel(const float* __restrict__ mu, const float* __restrict__ logvar, i
 
 __global__ void gae_finish_kernel(const double* acc, float* loss_out) { loss_out[0] = (float)acc[0]; }
 
-namespace gtc {   // gae_tc.cu: tcgen05 version of the all-pairs part
-size_t workspace_bytes(int32_t n);
-bool eligible(int32_t n, int32_t d, int32_t n_rows);
-int launch(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t row_begin, int32_t n_rows, float coef, float* dz,
-           double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st);
-}  // namespace gtc
-namespace gtch {   // gae_tch.cu: fp16-split tcgen05 version (half the MMA count of gae_tc.cu)
-size_t workspace_bytes(int32_t n);
-bool eligible(int32_t n, int32_t d, int32_t n_rows);
-int launch(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t row_begin, int32_t n_rows, float coef, float* dz,
-           double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st);
-const float* overflow_flag(const void* ws);    // device flag: 1 when the embedding is too large for fp16 operands (kernel stepped aside)
-}  // namespace gtch
-
-namespace gsym {   // gae_sym.cu: symmetric (unordered block pairs) tcgen05 version — half the elementwise work of gae_tch.cu
+namespace gtc {   // gae_tc.cu: wgmma version of the all-pairs part
 size_t workspace_bytes(int32_t n);
 int super_blocks(int32_t n);
-bool eligible(int32_t n, int32_t d);
-int launch(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t sb_begin, int32_t sb_end, float coef, float* dz,
+bool eligible(int32_t n, int32_t d, int32_t n_rows);
+int launch(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t row_begin, int32_t n_rows, float coef, float* dz,
            double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st);
-}  // namespace gsym
+int launch_super_blocks(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t sb_begin, int32_t sb_end, float coef, float* dz,
+                        double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st);
+}  // namespace gtc
 
 template <int D>
 static int launch_gae_edges(const float* z, int64_t ldz, const int32_t* rp, const int32_t* ci, int32_t row_begin, int32_t n_rows,
@@ -287,8 +262,8 @@ static int launch_gae_edges(const float* z, int64_t ldz, const int32_t* rp, cons
 template <int D>
 static int launch_gae(const float* z, int64_t ldz, const int32_t* rp, const int32_t* ci, int32_t n, int32_t row_begin,
                       int32_t n_rows, float coef, float pw, int use_pw, float* dz, double* acc, bool skip_allpairs,
-                      cudaStream_t st, const float* only_if = nullptr) {
-  if (skip_allpairs && !only_if) return launch_gae_edges<D>(z, ldz, rp, ci, row_begin, n_rows, coef, pw, use_pw, dz, acc, st);
+                      cudaStream_t st) {
+  if (skip_allpairs) return launch_gae_edges<D>(z, ldz, rp, ci, row_begin, n_rows, coef, pw, use_pw, dz, acc, st);
   const int row_blocks = ceil_div(n_rows, GaeCfg<D>::ROWS);
   // split the j range so that small graphs still fill the machine
   int j_splits = 1;
@@ -299,7 +274,7 @@ static int launch_gae(const float* z, int64_t ldz, const int32_t* rp, const int3
   int j_chunk = ceil_div(ceil_div(n, j_splits), GL_JT) * GL_JT;
   j_splits = ceil_div(n, j_chunk);
   dim3 grid(row_blocks, j_splits);
-  gae_allpairs_kernel<D><<<grid, GL_THREADS, 0, st>>>(z, ldz, n, row_begin, n_rows, j_chunk, coef, dz, acc, only_if);
+  gae_allpairs_kernel<D><<<grid, GL_THREADS, 0, st>>>(z, ldz, n, row_begin, n_rows, j_chunk, coef, dz, acc);
   B2_CHECK_LAUNCH("gae_allpairs_kernel");
   return launch_gae_edges<D>(z, ldz, rp, ci, row_begin, n_rows, coef, pw, use_pw, dz, acc, st);
 }
@@ -325,10 +300,8 @@ extern "C" int b2_mse_sum_loss_grad_f32(const float* recon, const float* target,
 }
 
 extern "C" size_t b2_gae_loss_workspace_bytes(int32_t n, int32_t d) {
-  // 256 B of accumulators + the hi/lo tf32 split of z (padded to 32 columns) for the tensor-core path
-  const size_t a = gtc::workspace_bytes(n), b = gtch::workspace_bytes(n), c = gsym::workspace_bytes(n);
-  const size_t m = a > b ? (a > c ? a : c) : (b > c ? b : c);
-  return 256 + (d <= 32 ? m : 0);
+  // 256 B of accumulators + the hi/lo tf32 planes of z for the tensor-core path
+  return 256 + (d <= 32 ? gtc::workspace_bytes(n) : 0);
 }
 
 extern "C" int b2_gae_loss_grad_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
@@ -348,31 +321,18 @@ extern "C" int b2_gae_loss_grad_f32(const float* z, int64_t ldz, const float* mu
   B2_CHECK_CUDA(cudaMemsetAsync(dz, 0, sizeof(float) * (size_t)n_rows * d, st));
   const float coef = (use_pos_weight ? norm : 1.f) / ((float)n * (float)n);
   int rc;
-  // large problems: the all-pairs part runs on tcgen05 (gae_tc.cu); the CUDA-core kernel serves small graphs
+  // large problems: the all-pairs part runs on the tensor cores (gae_tc.cu); the CUDA-core kernel serves small graphs
   bool tc_done = false;
-  const float* fallback_flag = nullptr;          // set when the chosen tensor-core kernel may step aside on the device
-  // full row range: the symmetric kernel evaluates every unordered block pair once (gae_sym.cu); a row shard of a multi-GPU run
-  // goes through b2_gae_loss_grad_sym_f32 instead (super-block ranges + all-reduce of dz), or falls through to the row-sweep kernel
-  if (row_begin == 0 && n_rows == n && gsym::eligible(n, d) && workspace_bytes >= 256 + gsym::workspace_bytes(n)) {
-    rc = gsym::launch(z, ldz, n, d, 0, gsym::super_blocks(n), coef, dz, acc, reinterpret_cast<char*>(workspace) + 256, workspace_bytes - 256, st);
-    if (rc == B2_OK) tc_done = true;
-    else if (rc != B2_ERR_UNSUPPORTED) return rc;
-  }
-  if (!tc_done && gtch::eligible(n, d, n_rows) && workspace_bytes >= 256 + gtch::workspace_bytes(n)) {
-    rc = gtch::launch(z, ldz, n, d, row_begin, n_rows, coef, dz, acc, reinterpret_cast<char*>(workspace) + 256, workspace_bytes - 256, st);
-    if (rc == B2_OK) { tc_done = true; fallback_flag = gtch::overflow_flag(reinterpret_cast<char*>(workspace) + 256); }
-    else if (rc != B2_ERR_UNSUPPORTED) return rc;
-  }
-  if (!tc_done && gtc::eligible(n, d, n_rows) && workspace_bytes >= 256 + gtc::workspace_bytes(n)) {
+  if (gtc::eligible(n, d, n_rows) && workspace_bytes >= 256 + gtc::workspace_bytes(n)) {
     rc = gtc::launch(z, ldz, n, d, row_begin, n_rows, coef, dz, acc, reinterpret_cast<char*>(workspace) + 256, workspace_bytes - 256, st);
     if (rc == B2_OK) tc_done = true;
     else if (rc != B2_ERR_UNSUPPORTED) return rc;
   }
   switch (d) {
-    case 8: rc = launch_gae<8>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st, fallback_flag); break;
-    case 16: rc = launch_gae<16>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st, fallback_flag); break;
-    case 32: rc = launch_gae<32>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st, fallback_flag); break;
-    case 64: rc = launch_gae<64>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st, fallback_flag); break;
+    case 8: rc = launch_gae<8>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st); break;
+    case 16: rc = launch_gae<16>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st); break;
+    case 32: rc = launch_gae<32>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st); break;
+    case 64: rc = launch_gae<64>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st); break;
     default:
       set_error("b2_gae_loss_grad_f32: embedding size %d unsupported (8, 16, 32, 64)", d);
       return B2_ERR_UNSUPPORTED;
@@ -392,14 +352,13 @@ extern "C" int b2_gae_loss_grad_f32(const float* z, int64_t ldz, const float* mu
 }
 
 
-// Pair-sharded form of b2_gae_loss_grad_f32 for multi-GPU runs (the symmetric decoder cannot be row-sharded: a tile feeds the
-// gradient of BOTH its row block and its column block).  Rank r evaluates the super-blocks [sb_begin, sb_end) of the cyclic
-// block-pair schedule (b2_gae_sym_super_blocks(n) in total, equal work each) plus the label / KLD terms of its own rows
-// [row_begin, row_begin + n_rows):
-//   dz_full [n, d]  : zero-filled here, receives this rank's all-pairs contributions to ALL rows and the label terms of its own
-//                     rows — the caller sums dz_full over ranks (all-reduce) and keeps its rows;
+// Pair-sharded form of b2_gae_loss_grad_f32 for multi-GPU runs.  Rank r evaluates the all-pairs part of the super-blocks
+// [sb_begin, sb_end) (b2_gae_sym_super_blocks(n) in total, equal work each: super-block s = the 128-row blocks s and nb−1−s)
+// plus the label / KLD terms of its own rows [row_begin, row_begin + n_rows):
+//   dz_full [n, d]  : zero-filled here, receives this rank's all-pairs contributions (the rows of its super-blocks) and the label
+//                     terms of its own rows — the caller sums dz_full over ranks (all-reduce) and keeps its rows;
 //   loss_out        : this rank's share of the loss (sum over ranks = the loss).
-extern "C" int b2_gae_sym_super_blocks(int32_t n) { return b2::gsym::super_blocks(n); }
+extern "C" int b2_gae_sym_super_blocks(int32_t n) { return b2::gtc::super_blocks(n); }
 
 extern "C" int b2_gae_loss_grad_sym_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
                                         const int32_t* lab_rowptr, const int32_t* lab_colidx, int32_t n, int32_t d,
@@ -409,8 +368,8 @@ extern "C" int b2_gae_loss_grad_sym_f32(const float* z, int64_t ldz, const float
   B2_REQUIRE(z && lab_rowptr && lab_colidx && dz_full && loss_out, "b2_gae_loss_grad_sym_f32: null pointer");
   B2_REQUIRE(n > 0 && d > 0 && d <= 16 && ldz >= d, "b2_gae_loss_grad_sym_f32: bad shape (d <= 16)");
   B2_REQUIRE(row_begin >= 0 && n_rows >= 0 && row_begin + n_rows <= n, "b2_gae_loss_grad_sym_f32: bad row range");
-  B2_REQUIRE(sb_begin >= 0 && sb_begin <= sb_end && sb_end <= gsym::super_blocks(n), "b2_gae_loss_grad_sym_f32: bad super-block range");
-  B2_REQUIRE(workspace && workspace_bytes >= 256 + gsym::workspace_bytes(n), "b2_gae_loss_grad_sym_f32: workspace too small");
+  B2_REQUIRE(sb_begin >= 0 && sb_begin <= sb_end && sb_end <= gtc::super_blocks(n), "b2_gae_loss_grad_sym_f32: bad super-block range");
+  B2_REQUIRE(workspace && workspace_bytes >= 256 + gtc::workspace_bytes(n), "b2_gae_loss_grad_sym_f32: workspace too small");
   B2_REQUIRE((mu == nullptr) == (logvar == nullptr), "b2_gae_loss_grad_sym_f32: mu/logvar must both be given or both NULL");
   if (mu) B2_REQUIRE(dmu && dlogvar && ldm >= d && ldd >= d, "b2_gae_loss_grad_sym_f32: dmu/dlogvar required with mu/logvar");
   cudaStream_t st = as_stream(stream);
@@ -418,9 +377,10 @@ extern "C" int b2_gae_loss_grad_sym_f32(const float* z, int64_t ldz, const float
   B2_CHECK_CUDA(cudaMemsetAsync(acc, 0, sizeof(double), st));
   B2_CHECK_CUDA(cudaMemsetAsync(dz_full, 0, sizeof(float) * (size_t)n * d, st));
   const float coef = (use_pos_weight ? norm : 1.f) / ((float)n * (float)n);
-  int rc = gsym::launch(z, ldz, n, d, sb_begin, sb_end, coef, dz_full, acc, reinterpret_cast<char*>(workspace) + 256, workspace_bytes - 256, st);
+  int rc = gtc::launch_super_blocks(z, ldz, n, d, sb_begin, sb_end, coef, dz_full, acc, reinterpret_cast<char*>(workspace) + 256,
+                                    workspace_bytes - 256, st);
   if (rc != B2_OK) {
-    if (rc == B2_ERR_UNSUPPORTED) set_error("b2_gae_loss_grad_sym_f32: tensor maps could not be built");
+    if (rc == B2_ERR_UNSUPPORTED) set_error("b2_gae_loss_grad_sym_f32: workspace too small");
     return rc;
   }
   float* dz_rows = dz_full + (size_t)row_begin * d;

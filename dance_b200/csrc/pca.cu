@@ -1,7 +1,7 @@
 // Symmetric eigensolver + centring helpers for the PCA transforms.
 //
 // Replaces sklearn.decomposition.PCA inside WeightedFeaturePCA / CellPCA (reference transforms/cell_feature.py:49-75,
-// 168-194): PCA = eigen-decomposition of the (small) Gram / covariance matrix, which is built by the tcgen05 GEMM.
+// 168-194): PCA = eigen-decomposition of the (small) Gram / covariance matrix, which is built by the tensor-core GEMM.
 // The eigensolver is a parallel one-sided Jacobi (Hestenes) iteration on the rows of W = C:
 //   every round rotates g/2 disjoint row pairs (p,q) so that <w_p, w_q> = 0, the same rotations are accumulated in V.
 //   After convergence the rows of W are orthogonal, ||w_i|| = |λ_i| and row i of V is the eigenvector.

@@ -2,9 +2,9 @@
 //
 // Same contract as b2_spmm_csr_f32 (spmm.cu) — torch.spmm(adj, support) scgnn2.py:500, DGL update_all(u_mul_e, sum|mean)
 // gnn.py:90 / graphsci.py:112-115 — for the reduced-precision configurations (BASELINE config 3 "GraphSCI … bf16", SURVEY
-// §8(b)4 `b2_spmm_csr_f32/bf16`).  The aggregate is bound by the gather stream nnz·F·sizeof(x) through L2 (ncu, profiles/):
-// halving the element size halves the bytes every non-zero pulls, and at 1 M cells × 32 features the operand (64 MB) fits
-// the 126 MB L2 outright, so the gathers stop spilling to HBM.
+// §8(b)4 `b2_spmm_csr_f32/bf16`).  The aggregate is bound by the gather stream nnz·F·sizeof(x) through L2:
+// halving the element size halves the bytes every non-zero pulls, and at 1 M cells × 32 features the operand (64 MB instead
+// of 128 MB) comes closer to fitting the 50 MB L2, so fewer gathers spill to HBM.
 //
 // Layout: a sub-warp group of G lanes owns one output row, lane gl owns features [8·gl, 8·gl+8) (one 16-byte gather per
 // non-zero).  The group prefetches up to 32 (col, val) pairs with coalesced loads, then issues the gathers in batches of 8

@@ -2,9 +2,8 @@
 // (fp32 F = 8 / 16 / 32, bf16 / fp16 F = 16 / 32 / 64) — the scGNN aggregate Â·support (scgnn2.py:500) and its backward.
 //
 // Why a second kernel.  The row-per-lane-group kernels (spmm.cu, spmm16.cu) chain rowptr → (col, val) → gathers → FMA per row and
-// per 8-entry chunk; measured on the 1 M-cell kNN graph (profiles/r02_ncu_spmm.md) they issue ~65 SASS instructions per four
-// non-zeros, keep 42 % (fp32) / 22 % (bf16) of the warps resident and leave DRAM at 9 % and L2 at 13 % of their throughput: latency-
-// and issue-bound, not bandwidth-bound.  Here every warp owns a contiguous range of rows — hence a contiguous stream of non-zeros —
+// per 8-entry chunk; partial-mask shuffles in loops of per-row trip count cost them ~65 SASS instructions per four non-zeros and
+// low occupancy: latency- and issue-bound, not bandwidth-bound.  Here every warp owns a contiguous range of rows — hence a contiguous stream of non-zeros —
 // and runs a software pipeline over 32-entry blocks of that stream:
 //
 //   block b+NG : its (col, val) pairs are copied to a shared-memory ring with cp.async (4 B per lane)
@@ -19,11 +18,8 @@
 // evict-last hint, the one-pass streams evict-first.  Accumulation order inside a row = CSR order up to the NPI-way lane split
 // (deterministic, independent of the launch geometry).
 //
-// Measured (B200, 1 M cells, nnz 28.1 M, F = 32, cold L2; scripts/lab/gather_lab.cu is the harness the design was selected with):
-// fp32 operand 0.49 ms vs 1.21 ms for spmm_csr_kernel<8,1>; bf16 operand 0.49 ms vs 0.96 ms (lab versions without the C-ABI's
-// options: 0.46 / 0.44 ms).  TMA tile::gather4 and per-row cp.async.bulk staging of the same pipeline were slower (0.64–1.05 ms):
-// the copies are too small for the TMA unit to pay off.  ncu: issue slots 76 % busy (14 instructions per non-zero) — the kernel is
-// issue-bound, which is why the bf16 operand is no faster (profiles/r02_ncu_spmm.md).
+// TMA row copies (tile::gather4, per-row cp.async.bulk) are a poor fit for this pipeline: 64–128-byte rows are too small for the
+// TMA unit to pay off.
 #include "common.cuh"
 
 #include <cuda_bf16.h>

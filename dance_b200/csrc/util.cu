@@ -40,7 +40,7 @@ static int g_path[B2_PATH_COUNT] = {0, 0, 0};
 int path_mode(int which) { return (which >= 0 && which < B2_PATH_COUNT) ? g_path[which] : 0; }
 
 // scheduling knobs of the tensor-core decoder (b2_set_tuning): they move work in time, never change a result
-static int g_tune[B2_TUNE_COUNT] = {1500, 1, 0};
+static int g_tune[B2_TUNE_COUNT] = {0};
 int tuning(int which) { return (which >= 0 && which < B2_TUNE_COUNT) ? g_tune[which] : 0; }
 
 }  // namespace b2
@@ -55,7 +55,7 @@ int64_t b2_launch_count(void) { return (int64_t)b2::g_launch_count; }
 
 int b2_set_path(int which, int mode) {
   B2_REQUIRE(which >= 0 && which < B2_PATH_COUNT, "b2_set_path: unknown selector %d", which);
-  B2_REQUIRE(mode >= 0 && mode <= (which == B2_PATH_GAE_DECODER ? 4 : 1), "b2_set_path: mode %d out of range for selector %d", mode, which);
+  B2_REQUIRE(mode >= 0 && mode <= (which == B2_PATH_GAE_DECODER ? 2 : 1), "b2_set_path: mode %d out of range for selector %d", mode, which);
   b2::g_path[which] = mode;
   return B2_OK;
 }

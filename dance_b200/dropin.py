@@ -1,7 +1,7 @@
 """Make the unmodified reference example scripts importable against this package.
 
 ``install()`` puts ``dance_b200/shims`` on ``sys.path`` — a ``dance`` package with the reference's module tree whose leaves
-re-export the B200-native classes, and a minimal ``scanpy`` exposing the ``pp`` functions the examples pass to
+re-export the H100-native classes, and a minimal ``scanpy`` exposing the ``pp`` functions the examples pass to
 ``AnnDataTransform`` — unless real ``dance`` / ``scanpy`` installations are importable.  ``run_example(path, argv)`` then
 executes a script such as ``examples/single_modality/imputation/scgnn2.py`` as ``__main__``.
 

@@ -311,9 +311,9 @@ class GraphAEEngine:
         z_all = self._gather(z, "z")
         n_all = z_all.shape[0]
         path = ops.get_path("gae")
-        if sharded and e <= 16 and (path == "sym" or (path == "auto" and n_all * n_all >= (1 << 24))):
-            # the symmetric decoder is partitioned by block PAIR (each logit tile feeds two row blocks): this rank takes its share of
-            # the equal-work super-blocks, writes partial gradients for ALL rows and the ranks sum them (one 64 MB all-reduce at 1 M)
+        if sharded and e <= 16 and (path == "tc" or (path == "auto" and n_all * n_all >= (1 << 24))):
+            # the tensor-core decoder is partitioned by super-block (row blocks s and nb−1−s, equal work each): this rank takes its
+            # share, writes partial gradients into a full-size buffer and the ranks sum them (one 64 MB all-reduce at 1 M)
             from .parallel import shard_bounds
             sb0, sb1 = shard_bounds(ops.gae_sym_super_blocks(n_all), comm.world)[comm.rank]
             dzf = self._bufs.setdefault(("dz_full", n_all), torch.empty(n_all, e, dtype=torch.float32, device=self.device))

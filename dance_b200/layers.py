@@ -111,7 +111,7 @@ class AdjLinearLayer:
     * STdGCN ``conGraphConvolutionlayer``      modules/spatial/cell_type_deconvo/stdgcn.py:63-90    (U(±1/√out) W and b)
     * scGNN / SpaGCN ``GraphConvolution``      scgnn2.py:479-502, spagcn.py:337-363
 
-    One tcgen05 GEMM + one SpMM (bias and activation fused into the aggregate); backward = SpMM over Âᵀ + two GEMMs."""
+    One tensor-core GEMM + one SpMM (bias and activation fused into the aggregate); backward = SpMM over Âᵀ + two GEMMs."""
 
     def __init__(self, in_features: int, out_features: int, *, bias: bool = False, activation: Optional[str] = None, init: str = "xavier",
                  device="cuda", precision: Optional[str] = None, seed: Optional[int] = None):

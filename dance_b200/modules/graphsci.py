@@ -1,4 +1,4 @@
-"""GraphSCI on the B200-native kernels — host-side mirror of ``dance/modules/single_modality/imputation/graphsci.py``
+"""GraphSCI on the H100-native kernels — host-side mirror of ``dance/modules/single_modality/imputation/graphsci.py``
 (buildNetwork :37-45, activations :48-63, MultiplyLayer :66-87, AEModel :90-112, GNNModel :115-131, GraphSCI :134-560).
 
 Model (one full-batch step = train forward → loss → eval forward for the validation loss → backward → Adam, :333-365):
@@ -183,6 +183,8 @@ class GraphSCI:
             m2b, S2b, ls = m2a, S2a, mu
         if eps is None:
             eps = torch.randn(mu.shape, device=self.device, generator=self.gen)
+        else:
+            eps = _t(eps, self.device)
         z = ops.adj_sample(mu, ls, eps)
         return z, ls, mu, dict(f_d=f_d, m0=m0, h1=h1, m1=m1, S1=S1, h2=h2, m2a=m2a, m2b=m2b, S2a=S2a, S2b=S2b, eps=eps, shared=(ls is mu))
 

@@ -1,4 +1,4 @@
-"""scDeepSort on the B200-native kernels — host-side mirror of
+"""scDeepSort on the H100-native kernels — host-side mirror of
 ``dance/modules/single_modality/cell_type_annotation/scdeepsort.py`` (GNN :26-88, ScDeepSort :91-349) and of
 ``dance/models/nn/gnn.py`` (AdaptiveSAGE :8-96).
 

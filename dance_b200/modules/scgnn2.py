@@ -1,4 +1,4 @@
-"""scGNN 2.0 on the B200-native engines — host-side mirror of the reference module
+"""scGNN 2.0 on the H100-native engines — host-side mirror of the reference module
 ``dance/modules/single_modality/imputation/scgnn2.py`` for the stages on the hot path.
 
 Same names, argument meaning and return types as the reference:

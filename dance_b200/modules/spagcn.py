@@ -1,9 +1,9 @@
-"""SpaGCN on the B200-native kernels — host-side mirror of ``dance/modules/spatial/spatial_domain/spagcn.py``
+"""SpaGCN on the H100-native kernels — host-side mirror of ``dance/modules/spatial/spatial_domain/spagcn.py``
 (GraphConvolution :337-366, SimpleGCDEC :369-584, calculate_p / search_l :249-287, SpaGCN :700-892).
 
 The layer is ``z = adj_exp · (X · W) + b`` with a DENSE ``adj_exp = exp(-D² / 2l²)`` (N×N, ``torch.spmm`` on a dense
 matrix at spagcn.py:359).  ``X`` and ``adj_exp`` never change during training, so this implementation builds
-``AX = adj_exp · X`` ONCE with the tcgen05 GEMM and trains on ``z = AX · W + b`` — the N²·h product leaves the epoch
+``AX = adj_exp · X`` ONCE with the tensor-core GEMM and trains on ``z = AX · W + b`` — the N²·h product leaves the epoch
 loop, and the backward pass needs only ``dW = AXᵀ · dz`` (re-association of the same fp32 sums, parity ≤1e-4 pinned by
 tests/test_gpu_spagcn.py against the reference's own ``fit``).
 

@@ -1,4 +1,4 @@
-"""STAGATE on the B200-native kernels — host-side mirror of ``dance/modules/spatial/spatial_domain/stagate.py``
+"""STAGATE on the H100-native kernels — host-side mirror of ``dance/modules/spatial/spatial_domain/stagate.py``
 (GATConv :31-128, Stagate :131-284).
 
 Forward (stagate.py:175-200), one attention head, no bias, no self-loop insertion::

@@ -125,12 +125,12 @@ def _workspace(nbytes: int, device) -> torch.Tensor:
     return buf
 
 
-_PATHS = {"gae": (0, {"auto": 0, "cuda": 1, "tf32": 2, "f16": 3, "sym": 4}), "knn": (1, {"auto": 0, "simt": 1}),
+_PATHS = {"gae": (0, {"auto": 0, "cuda": 1, "tc": 2}), "knn": (1, {"auto": 0, "simt": 1}),
           "spmm": (2, {"auto": 0, "rowgroup": 1})}
 
 
 def set_path(which: str, mode: str = "auto") -> None:
-    """Select the kernel path of the decoder ("gae": auto | cuda | tf32 | f16 | sym), of the kNN candidate filter
+    """Select the kernel path of the decoder ("gae": auto | cuda | tc), of the kNN candidate filter
     ("knn": auto | simt) or of the aggregate ("spmm": auto | rowgroup).  All paths return the same result; the switch exists
     for A/B tests and timing."""
     sel, modes = _PATHS[which]
@@ -138,8 +138,9 @@ def set_path(which: str, mode: str = "auto") -> None:
 
 
 def set_tuning(knob: str, value: int) -> None:
-    """Scheduling knobs of the symmetric decoder ("gae_stagger" cycles, "gae_late_gempty" 0/1, "gae_splits" CTAs per super-block, 0 = automatic): timing experiments only."""
-    check(lib().b2_set_tuning({"gae_stagger": 0, "gae_late_gempty": 1, "gae_splits": 2}[knob], int(value)), "b2_set_tuning")
+    """Scheduling knob of the tensor-core decoder ("gae_splits": step ranges per 128-row block of the J sweep, 0 = automatic):
+    timing experiments only."""
+    check(lib().b2_set_tuning({"gae_splits": 0}[knob], int(value)), "b2_set_tuning")
 
 
 def get_path(which: str) -> str:
@@ -363,7 +364,7 @@ def gae_loss_grad(z, labels: CSR, norm: float, pos_weight: float, mu=None, logva
 
 
 def gae_sym_super_blocks(n: int) -> int:
-    """Equal-work units of the symmetric decoder's block-pair schedule (see gae_loss_grad_sym)."""
+    """Equal-work units of the pair-sharded decoder (super-block s = 128-row blocks s and nb−1−s; see gae_loss_grad_sym)."""
     return int(lib().b2_gae_sym_super_blocks(n))
 
 
@@ -884,6 +885,10 @@ def zinb_loss_grad(a_pi, b_disp, c_mean, Y, size_factors, mask=None, le: float =
 
 
 def adj_sample(mu, log_std, eps):
+    for t, name in ((mu, "mu"), (log_std, "log_std"), (eps, "eps")):
+        _chk(t, torch.float32, f"adj_sample: {name}")
+        if t.numel() != mu.numel() or not t.is_contiguous():
+            raise B2Error(f"adj_sample: {name} must be a contiguous tensor of {mu.numel()} elements")
     z = torch.empty_like(mu)
     check(lib().b2_adj_sample_f32(_p(mu), _p(log_std), _p(eps), mu.numel(), _p(z), _stream()), "b2_adj_sample_f32")
     return z

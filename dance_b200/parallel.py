@@ -48,50 +48,30 @@ def batch_schedule(n_local: int, batch_size: int, n_steps: Optional[int] = None)
     return sched
 
 
-def sym_schedule(n_blocks: int, super_block: int) -> List[Tuple[int, int]]:
-    """Logit tiles (I, J) of 128-row blocks that super-block ``super_block`` of the symmetric decoder evaluates — the host-side
-    statement of ``gsym::Sweep`` (csrc/gae_sym.cu), used to shard the decoder over ranks and to test the schedule.
+def _sym_blocks(n_blocks: int, super_block: int) -> List[int]:
+    return sorted({super_block, n_blocks - 1 - super_block})
 
-    Block I owns the unordered pairs {I, (I+o) mod nb}, o = 0..h with h = nb // 2; for even nb the antipodal pair (o = h) belongs
-    to the smaller index.  A super-block is the two adjacent blocks (2·sb, 2·sb+1); together the super-blocks cover every
-    unordered pair exactly once with (almost) equal work."""
-    nb, h = n_blocks, n_blocks // 2
-    even = nb % 2 == 0
-    out = []
-    for I in (2 * super_block, 2 * super_block + 1):
-        if I >= nb:
-            continue
-        for o in range(h + 1):
-            if o == h and o > 0 and even and I + h >= nb:
-                continue
-            out.append((I, (I + o) % nb))
-    return out
+
+def sym_schedule(n_blocks: int, super_block: int) -> List[Tuple[int, int]]:
+    """Logit tiles (I, J) of 128-row blocks that super-block ``super_block`` of the pair-sharded decoder evaluates — the host-side
+    statement of the work units of ``gae_allpairs_tc_kernel`` (csrc/gae_tc.cu), used to shard the decoder over ranks and to test it.
+
+    A super-block is the row blocks sb and nb−1−sb (one block when they coincide); each row block sweeps every J.  Together the
+    super-blocks cover every ordered pair of blocks exactly once, two row blocks of work each (one for a lone middle block)."""
+    return [(I, J) for I in _sym_blocks(n_blocks, super_block) for J in range(n_blocks)]
 
 
 def sym_steps(n_blocks: int, super_block: int) -> List[List[Tuple[int, int]]]:
-    """The same tiles grouped by J-step: step s of super-block sb stages Z_J for J = (2·sb + s) mod nb and evaluates the tiles of its
-    one or two owned blocks against it (block 2·sb at offset o = s, block 2·sb+1 at o = s − 1).  Trailing empty steps are dropped,
-    as in ``gsym::Sweep::n_steps``."""
-    nb, h = n_blocks, n_blocks // 2
-    even = nb % 2 == 0
-    steps = []
-    for s in range(h + 2):
-        tiles = []
-        for g, I in enumerate((2 * super_block, 2 * super_block + 1)):
-            o = s - g
-            if I >= nb or o < 0 or o > h or (o == h and o > 0 and even and I + h >= nb):
-                continue
-            tiles.append((I, (I + o) % nb))
-        steps.append(tiles)
-    while steps and not steps[-1]:
-        steps.pop()
-    return steps
+    """The same tiles grouped by J-step: step s stages Z_J for J = s and evaluates it against the super-block's row blocks (in the
+    kernel each row block is its own CTA; both walk the same steps)."""
+    return [[(I, J) for I in _sym_blocks(n_blocks, super_block)] for J in range(n_blocks)]
 
 
 def sym_step_range(n_steps: int, part: int, splits: int) -> Tuple[int, int]:
-    """Steps [s0, s1) of a super-block's sweep that CTA ``part`` of ``splits`` runs (``gsym::Sweep::s0 / s1``): the decoder cuts
-    sweeps into step ranges so that a rank's grid fills whole waves of SMs."""
-    return n_steps * part // splits, n_steps * (part + 1) // splits
+    """Steps [s0, s1) of a J sweep that CTA ``part`` of ``splits`` runs (``gae_allpairs_tc_kernel``: ⌈n_steps / splits⌉ steps per
+    part, trailing parts may be empty): the decoder cuts sweeps into step ranges so that a grid fills a wave of SMs."""
+    per = -(-n_steps // splits)
+    return min(n_steps, part * per), min(n_steps, (part + 1) * per)
 
 
 def spmm_stream_partition(rowptr, n_warps: int) -> List[Tuple[int, int]]:

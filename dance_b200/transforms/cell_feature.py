@@ -1,4 +1,4 @@
-"""PCA feature transforms on the GPU (``ops.pca``: tcgen05 GEMM for the Gram / covariance matrix + Jacobi
+"""PCA feature transforms on the GPU (``ops.pca``: tensor-core GEMM for the Gram / covariance matrix + Jacobi
 eigensolver).  Same constructors, output channels and ``repr`` as the reference
 (dance/transforms/cell_feature.py: ``WeightedFeaturePCA`` :19-75, ``CellPCA`` :146-194; reprs pinned by the
 reference's tests/transforms/test_basics.py:5-22).

@@ -209,7 +209,7 @@ class FeatureFeatureGraph(BaseTransform):
     ``spearman`` (Pearson of the tie-averaged ranks, scipy.stats.spearmanr) or ``rbf`` (Gaussian kernel of the euclidean
     distance, utils/matrix.py:70-97) — entries with |score| below ``threshold`` dropped, edges in row-major order, unit weights
     optionally normalised like ``dgl.nn.EdgeWeightNorm("both")``.  Result: ``uns[out]`` = graph with ``ndata["feat"] = Xᵀ`` and
-    ``edata["weight"]``.  The correlations run through the fp64 Gram kernel; the rbf Gram through the tcgen05 GEMM (the
+    ``edata["weight"]``.  The correlations run through the fp64 Gram kernel; the rbf Gram through the tensor-core GEMM (the
     reference uses an fp32 BLAS product there, so entries within round-off of the threshold may differ)."""
 
     _DISPLAY_ATTRS = ("threshold", "positive_only", "normalize_edges", "score_func", "score_func_kwargs")

@@ -1,5 +1,5 @@
 /*
- * dance_b200 — C-ABI of the B200-native GNN message-passing hot path.
+ * dance_b200 — C-ABI of the H100-native (sm_90a) GNN message-passing hot path.
  *
  * This header is the drop-in boundary (SURVEY.md §8b.4).  The reference
  * (OmicsML/dance) has no FFI of its own: its hot path bottoms out in calls
@@ -42,22 +42,20 @@ extern "C" {
 
 /* GEMM precision modes */
 #define B2_PREC_FP32_SIMT 0 /* CUDA-core FFMA, exact fp32 accumulate            */
-#define B2_PREC_TF32X3 1    /* tcgen05 kind::tf32, 3-product split, ~fp32 accuracy */
-#define B2_PREC_TF32 2      /* tcgen05 kind::tf32, single product                */
+#define B2_PREC_TF32X3 1    /* wgmma tf32, 3-product split, ~fp32 accuracy      */
+#define B2_PREC_TF32 2      /* wgmma tf32, single product                        */
 
 /* Kernel-path selectors for A/B tests: every selectable path returns the same result (bit-exact for the kNN filter, to
  * rounding for the decoder); mode 0 = automatic choice by problem size. */
-#define B2_PATH_GAE_DECODER 0 /* 1 CUDA cores · 2 tcgen05 tf32 split · 3 tcgen05 fp16 row sweep · 4 tcgen05 fp16 symmetric */
+#define B2_PATH_GAE_DECODER 0 /* 1 CUDA cores · 2 tensor cores (wgmma tf32, 3-product split) */
 #define B2_PATH_KNN_FILTER 1  /* 1 SIMT candidate filter */
 #define B2_PATH_SPMM 2        /* 1 row-per-lane-group kernels for every shape (default: the nnz-stream kernel where it applies) */
 #define B2_PATH_COUNT 3
 int b2_set_path(int which, int mode);
 int b2_get_path(int which);
-/* Scheduling knobs of the symmetric decoder (timing experiments; results do not depend on them). */
-#define B2_TUNE_GAE_STAGGER 0     /* initial delay (cycles) of the second elementwise group, default 1500 */
-#define B2_TUNE_GAE_LATE_GEMPTY 1 /* 1 (default): the elementwise group waits for its G buffer after the first half's math; 0: before loading S */
-#define B2_TUNE_GAE_SPLITS 2      /* CTAs per super-block of the symmetric decoder (0 = automatic: fill whole waves of SMs) */
-#define B2_TUNE_COUNT 3
+/* Scheduling knob of the tensor-core decoder (timing experiments; results do not depend on it beyond summation order). */
+#define B2_TUNE_GAE_SPLITS 0      /* step ranges (CTAs) per 128-row block of the decoder's J sweep (0 = automatic: fill a wave of SMs) */
+#define B2_TUNE_COUNT 1
 int b2_set_tuning(int which, int value);
 
 const char* b2_last_error(void);
@@ -466,11 +464,10 @@ int b2_adj_reparam_bwd_f32(const float* dz, const float* mu, const float* log_st
                            float coef_kl, float* dmu, float* dlog_std, void* stream);
 
 /* Pair-sharded form of b2_gae_loss_grad_f32 for multi-GPU runs (InnerProductDecoder + gae_loss_function, scgnn2.py:423-426,
- * 603-619).  The all-pairs part is evaluated over UNORDERED 128-row block pairs (each logit tile feeds the gradient of its row
- * block and of its column block), so it is partitioned by pair, not by row: rank r takes super-blocks [sb_begin, sb_end) of the
- * b2_gae_sym_super_blocks(n) equal-work units, plus the label / KLD terms of its own rows [row_begin, row_begin + n_rows).
- * dz_full [n, d] is zero-filled here and receives contributions to ALL rows: sum it over ranks (all-reduce); loss_out holds
- * this rank's share of the loss.  d <= 16.  Workspace: b2_gae_loss_workspace_bytes(n, d). */
+ * 603-619).  The all-pairs part is partitioned into b2_gae_sym_super_blocks(n) equal-work units (super-block s = the 128-row
+ * blocks s and nb-1-s): rank r takes super-blocks [sb_begin, sb_end), plus the label / KLD terms of its own rows
+ * [row_begin, row_begin + n_rows).  dz_full [n, d] is zero-filled here and receives this rank's contributions: sum it over
+ * ranks (all-reduce); loss_out holds this rank's share of the loss.  d <= 16.  Workspace: b2_gae_loss_workspace_bytes(n, d). */
 int b2_gae_sym_super_blocks(int32_t n);
 int b2_gae_loss_grad_sym_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
                              const int32_t* lab_rowptr, const int32_t* lab_colidx, int32_t n, int32_t d,

@@ -499,6 +499,27 @@ def _graphsc_conv_fixture():
     np.savez_compressed(OUT / "graphsc_conv.npz", **out)
 
 
+def _feature2adj_fixture(ref):
+    """The reference's feature2adj / preprocess_graph on two seeded embeddings: integer k (3, 15) and a fractional
+    neighbourhood (0.05 of N, scgnn2.py:651-654)."""
+    out = {}
+    X = port.synthetic_embedding(257, d=24, n_clusters=5, seed=3)
+    for k in (3, 15):
+        _, adj_train, edges = ref.feature2adj(X, k, False)
+        a = sp.csr_matrix(adj_train)
+        a.sort_indices()
+        out[f"k{k}.edges_dst"] = np.array([e[1] for e in edges], dtype=np.int64)
+        out[f"k{k}.adj_indptr"], out[f"k{k}.adj_indices"], out[f"k{k}.adj_data"] = a.indptr.astype(np.int64), a.indices.astype(np.int64), a.data
+        an = ref.preprocess_graph(adj_train).coalesce()
+        out[f"k{k}.norm_values"], out[f"k{k}.norm_indices"] = an.values().numpy(), an.indices().numpy()
+    X2 = port.synthetic_embedding(120, d=8, n_clusters=3, seed=9)
+    _, adj_train, _ = ref.feature2adj(X2, 0.05, False)
+    a = sp.csr_matrix(adj_train)
+    a.sort_indices()
+    out["frac.adj_indptr"], out["frac.adj_indices"], out["frac.adj_data"] = a.indptr.astype(np.int64), a.indices.astype(np.int64), a.data
+    np.savez_compressed(OUT / "scgnn_feature2adj.npz", **out)
+
+
 def main():
     import sys
     OUT.mkdir(parents=True, exist_ok=True)
@@ -513,6 +534,7 @@ def main():
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
         X, adj_train, an, pw, norm = _knn_graph_fixture(ref)
+        _feature2adj_fixture(ref)
         _graph_ae_fixture(ref, X, adj_train, an, pw, norm)
         _gat_fixture(ref, X, _KNN_IDX, adj_train)
         _feature_ae_fixture(ref)

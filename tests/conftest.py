@@ -12,7 +12,7 @@ GOLDEN = Path(__file__).resolve().parent / "golden"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (select with `-m gpu`)")
 
 
 @pytest.fixture(scope="session")

@@ -22,7 +22,7 @@ def test_header_declares_something():
 def test_library_exports_every_declared_symbol():
     from dance_b200 import _lib
     from dance_b200.build import build
-    build()  # nvcc cross-compiles for sm_100a without a GPU
+    build()  # nvcc cross-compiles for sm_90a without a GPU
     handle = ctypes.CDLL(str(_lib.lib_path()))
     missing = [n for n in _declared() if not hasattr(handle, n)]
     assert not missing, f"symbols declared in dance_b200.h but not exported: {missing}"
@@ -51,21 +51,21 @@ def test_ops_refuse_cpu_tensors():
         ops.gemm(torch.zeros(4, 4), torch.zeros(4, 4))
 
 
-def test_sass_is_sm100a():
-    """The shipped library carries sm_100a SASS (and nothing else)."""
+def test_sass_is_sm90a():
+    """The shipped library carries sm_90a SASS (and nothing else)."""
     import shutil
     import subprocess
     from dance_b200 import _lib
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     out = subprocess.run([cuobjdump, "-lelf", str(_lib.lib_path())], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
-def test_library_contains_blackwell_tensor_core_and_tma_code():
-    """The shipped .so is sm_100a code that really uses the 5th-gen tensor cores, tensor memory and TMA: the SASS of the
-    GEMM, decoder and kNN-filter kernels must contain UTCHMMA (tcgen05.mma), LDTM/STTM (tcgen05.ld/st) and UTMALDG
-    (cp.async.bulk.tensor).  Needs cuobjdump (CUDA toolkit); skipped where it is not installed."""
+def test_library_contains_hopper_tensor_core_and_tma_code():
+    """The shipped .so is sm_90a code that really uses the warpgroup tensor-core MMA and TMA: the SASS of the GEMM, decoder
+    and kNN-filter kernels must contain HGMMA (wgmma.mma_async), UTMALDG (cp.async.bulk.tensor) and UBLKCP (cp.async.bulk).
+    Needs cuobjdump (CUDA toolkit); skipped where it is not installed."""
     import shutil
     import subprocess
     from dance_b200 import _lib
@@ -74,11 +74,11 @@ def test_library_contains_blackwell_tensor_core_and_tma_code():
         pytest.skip("cuobjdump not available")
     lib_path = Path(_lib.__file__).resolve().parent / "lib" / "libdance_b200.so"
     elf = subprocess.run([cuobjdump, "-lelf", str(lib_path)], capture_output=True, text=True, timeout=120).stdout
-    assert "sm_100a" in elf
+    assert "sm_90a" in elf
     sass = subprocess.run([cuobjdump, "-sass", str(lib_path)], capture_output=True, text=True, timeout=300).stdout
-    for mnemonic in ("UTCHMMA", "LDTM", "STTM", "UTMALDG"):
+    for mnemonic in ("HGMMA", "UTMALDG", "UBLKCP"):
         assert mnemonic in sass, mnemonic
-    for kernel in ("gemm_tc_kernel", "gae_allpairs_tch_kernel", "knn_candidates_tc_kernel"):
+    for kernel in ("gemm_tc_kernel", "gae_allpairs_tc_kernel", "knn_candidates_tc_kernel"):
         assert kernel in sass, kernel
 
 
@@ -107,14 +107,15 @@ def test_selector_tables_match_the_header():
     from dance_b200 import _lib, ops
     hdr = (Path(__file__).resolve().parent.parent / "include" / "dance_b200.h").read_text()
     consts = {m.group(1): int(m.group(2)) for m in re.finditer(r"#define\s+(B2_(?:PATH|TUNE)_[A-Z_]+)\s+(\d+)", hdr)}
-    assert consts["B2_PATH_COUNT"] == 3 and consts["B2_TUNE_COUNT"] == 3
+    assert consts["B2_PATH_COUNT"] == 3 and consts["B2_TUNE_COUNT"] == 1
     assert {k: v[0] for k, v in ops._PATHS.items()} == {"gae": consts["B2_PATH_GAE_DECODER"], "knn": consts["B2_PATH_KNN_FILTER"],
                                                          "spmm": consts["B2_PATH_SPMM"]}
     lib = _lib.lib()
     assert lib.b2_set_path(consts["B2_PATH_COUNT"], 0) != 0 and lib.b2_set_tuning(consts["B2_TUNE_COUNT"], 0) != 0
     assert lib.b2_set_path(consts["B2_PATH_SPMM"], 1) == 0 and lib.b2_get_path(consts["B2_PATH_SPMM"]) == 1
     assert lib.b2_set_path(consts["B2_PATH_SPMM"], 0) == 0
-    for knob, idx in (("gae_stagger", consts["B2_TUNE_GAE_STAGGER"]), ("gae_late_gempty", consts["B2_TUNE_GAE_LATE_GEMPTY"]),
-                      ("gae_splits", consts["B2_TUNE_GAE_SPLITS"])):
+    assert lib.b2_set_path(consts["B2_PATH_GAE_DECODER"], 2) == 0 and lib.b2_set_path(consts["B2_PATH_GAE_DECODER"], 3) != 0
+    assert lib.b2_set_path(consts["B2_PATH_GAE_DECODER"], 0) == 0
+    for knob, idx in (("gae_splits", consts["B2_TUNE_GAE_SPLITS"]),):
         assert lib.b2_set_tuning(idx, 1) == 0
-    ops.set_tuning("gae_stagger", 1500), ops.set_tuning("gae_late_gempty", 1), ops.set_tuning("gae_splits", 0)   # the defaults
+    ops.set_tuning("gae_splits", 0)   # the default

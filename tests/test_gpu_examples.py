@@ -1,8 +1,6 @@
-"""The reference's example scripts, UNMODIFIED, against the drop-in namespace (dance_b200/dropin.py + dance_b200/shims): the
-scripts are read from the reference checkout when it exists (build container) — on the GPU box, where /root/reference is absent,
-from the verbatim command-line surface restated in `_EXAMPLE_FLOWS` below (same imports, same calls, taken line by line from
+"""The reference's example flows against the drop-in namespace (dance_b200/dropin.py + dance_b200/shims): the command-line
+surface of the reference's example scripts restated in `_EXAMPLE_FLOWS` below (same imports, same calls, taken line by line from
 examples/single_modality/imputation/scgnn2.py:178-237 and examples/single_modality/cell_type_annotation/scdeepsort.py:40-77)."""
-import os
 import sys
 from pathlib import Path
 
@@ -10,7 +8,6 @@ import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
-REF_EXAMPLES = Path(os.environ.get("DANCE_REFERENCE_ROOT", "/root/reference")) / "examples"
 
 
 @pytest.fixture
@@ -25,12 +22,9 @@ def synth_env(tmp_path, monkeypatch):
         del sys.modules[k]
 
 
-def _script(rel: str, fallback: str, tmp_path: Path) -> Path:
-    p = REF_EXAMPLES / rel
-    if p.exists():
-        return p
+def _script(rel: str, flow: str, tmp_path: Path) -> Path:
     q = tmp_path / Path(rel).name
-    q.write_text(fallback)
+    q.write_text(flow)
     return q
 
 

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (TMA + TMEM, kind::tf32) against an fp64 reference: every operand layout,
+"""Tensor-core GEMM (TMA + wgmma tf32) against an fp64 reference: every operand layout,
 ragged shapes, split-K, all tile widths, fused epilogue; 3xTF32 must be fp32-accurate."""
 import numpy as np
 import pytest
@@ -8,8 +8,8 @@ from conftest import rel_err
 
 pytestmark = pytest.mark.gpu
 
-# tf32x3: operands are exact (hi/lo split) but the TMEM accumulate truncates, ~2e-8 relative per accumulation
-# (measured, see scripts/tc_race.py) → a few 1e-6 at K≈2000-3000; plain tf32 truncates the operands (~8e-4).
+# tf32x3: operands are exact (hi/lo split); the tensor-core accumulate is not fp32-exact, which over K≈2000-3000 leaves a few
+# 1e-6; plain tf32 truncates the operands (~8e-4).
 TOL = {"tf32x3": 1e-5, "tf32": 2e-3}
 
 SHAPES = [
@@ -76,7 +76,7 @@ def test_gemm_tc_splitk_epilogue_and_padded_ld(cuda):
 
 
 def test_gemm_tc_many_tiles_persistent(cuda):
-    """More tiles than SMs: exercises the persistent loop, the smem ring wrap-around and both TMEM buffers."""
+    """More tiles than SMs (several waves of CTAs) with a long K loop: exercises the TMA ring wrap-around and both plane buffers."""
     from dance_b200 import ops
     A = torch.randn(12800, 512, device=cuda)
     B = torch.randn(2000, 512, device=cuda)

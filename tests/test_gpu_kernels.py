@@ -248,7 +248,7 @@ def test_knn_bit_exact_vs_oracle(cuda, n, d, k):
 
 @pytest.mark.parametrize("n,d,k", [(6000, 128, 15), (5000, 50, 15), (4500, 16, 10)])
 def test_knn_tensor_core_filter_bit_exact(cuda, n, d, k):
-    """n·n_q ≥ 2^24 routes the candidate filter through tcgen05 (fp16 hi/lo split); the fp64 refine + proof keep the result
+    """n·n_q ≥ 2^24 routes the candidate filter through wgmma (fp16 hi/lo split); the fp64 refine + proof keep the result
     bit-exact with the reference ranking; duplicates, a query range, and the SIMT filter (ops.set_path("knn", "simt")) agree."""
     import os
     from dance_b200 import ops
@@ -415,8 +415,8 @@ def gae_reference_rows(z, rowptr, colidx, norm, pw, rows, chunk=512):
 
 
 def test_gae_loss_tensor_core_single_column_range(cuda):
-    """The branch bench.py times: n_rows ≥ 148·128 ⇒ j_splits == 1, every CTA sweeps ALL columns and the epilogue adds into dz without
-    atomics (gae_tch.cu).  Checked against the fp64 closed form evaluated in row chunks, full and row-sharded."""
+    """The tensor-core decoder at 150 row blocks (more than one wave of SMs: each CTA sweeps ALL columns and the epilogue adds into
+    dz without atomics).  Checked against the fp64 closed form evaluated in row chunks, full and row-sharded."""
     from dance_b200 import ops
     n, d, k = 19_200, 16, 7
     gen = torch.Generator(device=cuda).manual_seed(11)
@@ -429,7 +429,7 @@ def test_gae_loss_tensor_core_single_column_range(cuda):
     loss, dz, _, _ = ops.gae_loss_grad(z, L, norm, pw)
     assert abs(loss.item() - ref_loss) < 2e-6 * abs(ref_loss), (loss.item(), ref_loss)
     assert rel_err(dz, ref_dz) < 2e-5
-    # one shard with ≥ 148·128 rows (still j_splits == 1) + a short one (j_splits > 1)
+    # one shard with more row blocks than SMs (no J split) + a short one (J sweep split over CTAs)
     h = 148 * 128 + 3
     rp = A.rowptr.long()
     top = ops.CSR(A.rowptr[:h + 1].contiguous(), A.colidx[:rp[h]].contiguous(), None, (h, n))
@@ -442,8 +442,8 @@ def test_gae_loss_tensor_core_single_column_range(cuda):
 
 @pytest.mark.parametrize("n,d", [(128, 16), (100, 16), (256, 16), (300, 16), (384, 8), (1000, 16), (1537, 16), (1664, 8), (2048, 16), (2049, 16)])
 def test_gae_symmetric_decoder_small_graphs(cuda, n, d):
-    """gae_sym.cu forced onto small graphs: 1, 2, 3, 8, 13, 16, 17 row blocks (odd / even counts, antipodal pairs, a ragged last
-    block, a lone last super-block) against the fp64 closed form and against the row-sweep kernel."""
+    """The tensor-core decoder forced onto small graphs: 1, 2, 3, 8, 13, 16, 17 row blocks (odd / even counts, a ragged last
+    block) against the fp64 closed form and against the CUDA-core kernel."""
     from dance_b200 import ops
     gen = torch.Generator(device=cuda).manual_seed(n * 31 + d)
     z = (torch.randn(n, d, device=cuda, generator=gen) * 0.6).contiguous()
@@ -452,7 +452,7 @@ def test_gae_symmetric_decoder_small_graphs(cuda, n, d):
     L = ops.CSR(A.rowptr, A.colidx, None, A.shape)
     norm, pw = 0.51, 37.0
     ref_loss, ref_dz = gae_reference_rows(z, A.rowptr, A.colidx, norm, pw, torch.arange(n, device=cuda))
-    ops.set_path("gae", "sym")
+    ops.set_path("gae", "tc")
     try:
         loss, dz, _, _ = ops.gae_loss_grad(z, L, norm, pw)
         loss2, dz2, _, _ = ops.gae_loss_grad(z, L, norm, pw)
@@ -461,7 +461,7 @@ def test_gae_symmetric_decoder_small_graphs(cuda, n, d):
     assert abs(loss.item() - ref_loss) < 2e-6 * abs(ref_loss), (loss.item(), ref_loss)
     assert rel_err(dz, ref_dz) < 2e-5
     assert rel_err(dz2, dz) < 1e-6 and abs(loss2.item() - loss.item()) < 1e-6 * abs(loss.item())   # atomics reorder sums only
-    ops.set_path("gae", "f16")
+    ops.set_path("gae", "cuda")
     try:
         loss_r, dz_r, _, _ = ops.gae_loss_grad(z, L, norm, pw)
     finally:
@@ -483,7 +483,7 @@ def test_gae_symmetric_decoder_step_splits(cuda, n, splits):
     norm, pw = 0.5, 55.0
     rows = torch.arange(n, device=cuda) if n <= 2049 else torch.randint(0, n, (300, ), device=cuda, generator=gen)
     _, ref_rows = gae_reference_rows(z, A.rowptr, A.colidx, norm, pw, rows)
-    ops.set_path("gae", "sym")
+    ops.set_path("gae", "tc")
     try:
         ops.set_tuning("gae_splits", 1)
         loss1, dz1, _, _ = ops.gae_loss_grad(z, L, norm, pw)
@@ -496,11 +496,11 @@ def test_gae_symmetric_decoder_step_splits(cuda, n, splits):
     assert abs(loss.item() - loss1.item()) < 2e-6 * abs(loss1.item())
 
 
-@pytest.mark.parametrize("n,path,scale", [(4500, "sym", 3.0e4), (4500, "sym", 40.0), (3000, "f16", 3.0e4), (3000, "cuda", 3.0e4)])
+@pytest.mark.parametrize("n,path,scale", [(4500, "tc", 3.0e4), (4500, "tc", 40.0), (3000, "cuda", 3.0e4)])
 def test_gae_decoder_large_embedding(cuda, n, path, scale):
     """Embeddings far beyond the fp16 operand range (an untrained Graph-AE at 1 M cells draws z = mu + eps·exp(logvar) with logvar ≈ 14,
-    |z| ~ 1e6): the symmetric kernel switches to its scaled-operand variant, the row-sweep kernel steps aside for the fp32 kernel —
-    finite and equal to the fp64 closed form either way (the reference's BCE-with-logits is finite for any logit)."""
+    |z| ~ 1e6): the tensor-core kernel's tf32 hi/lo operands keep the fp32 exponent range, so its result stays finite and equal to
+    the fp64 closed form, like the CUDA-core kernel's (the reference's BCE-with-logits is finite for any logit)."""
     from dance_b200 import ops
     gen = torch.Generator(device=cuda).manual_seed(n)
     z = (torch.randn(n, 16, device=cuda, generator=gen) * scale).contiguous()
@@ -556,7 +556,7 @@ def test_gae_symmetric_decoder_pair_sharded(cuda, n, parts):
 
 @pytest.mark.parametrize("n,d", [(3000, 16), (2500, 16), (4133, 8), (2304, 32)])
 def test_gae_loss_tensor_core_path(cuda, n, d):
-    """tcgen05 decoder (S in TMEM → SFU → G in TMEM → dZ) vs the dense fp64 formula and vs the CUDA-core kernel."""
+    """Tensor-core decoder (S in registers → SFU → G in registers → dZ) vs the dense fp64 formula and vs the CUDA-core kernel."""
     import os
     from dance_b200 import ops
     from oracle import port

@@ -98,7 +98,7 @@ def test_feature_feature_graph_spearman_and_rbf(cuda, score_func, kw):
     if score_func == "spearman":      # fp64 correlations on both sides → the thresholded structure is exact
         assert np.array_equal(src.numpy(), src_r) and np.array_equal(dst.numpy(), dst_r)
         assert np.allclose(gph.edata["weight"].numpy(), w_r, rtol=1e-6)
-    else:                             # fp32 Gram on both sides (BLAS vs tcgen05 tf32x3): entries within round-off of the threshold may flip
+    else:                             # fp32 Gram on both sides (BLAS vs tensor-core tf32x3): entries within round-off of the threshold may flip
         mine = set(zip(src.numpy().tolist(), dst.numpy().tolist()))
         ref = set(zip(src_r.tolist(), dst_r.tolist()))
         assert len(mine ^ ref) <= max(2, len(ref) // 500)

@@ -135,7 +135,7 @@ def test_fit_sgd_and_fit_with_init(cuda, golden):
 
 
 def test_spagcn_module_end_to_end_larger(cuda):
-    """N large enough for the tcgen05 GEMM to build adj·X; compared with the torch restatement of the reference loop."""
+    """N large enough for the tensor-core GEMM to build adj·X; compared with the torch restatement of the reference loop."""
     from dance_b200.modules.spagcn import SpaGCN
     from dance_b200 import ops
     from oracle import port

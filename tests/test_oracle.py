@@ -1,6 +1,5 @@
-"""Pin the oracle (oracle/port.py): against the reference's own known-answer tests, against the
-committed fixtures generated from the reference (tests/golden, oracle/make_golden.py) and — when
-/root/reference is present (build container) — against the reference code executed live."""
+"""Pin the oracle (oracle/port.py): against the reference's own known-answer tests and against the
+committed fixtures generated from the reference's code (tests/golden, oracle/make_golden.py)."""
 import itertools
 
 import numpy as np
@@ -9,7 +8,7 @@ import scipy.sparse as sp
 import scipy.spatial
 import torch
 
-from oracle import port, ref_loader
+from oracle import port
 
 from conftest import rel_err
 
@@ -131,33 +130,29 @@ def test_feature_ae_golden(golden):
         assert np.allclose(v.reshape(-1)[sample_index(v.size)], g[f"after.{k}.sample"], rtol=1e-4, atol=1e-6)
 
 
-# ---- live against the reference (build container only) -----------------------------------------
-needs_ref = pytest.mark.skipif(not ref_loader.available(), reason="/root/reference not present (GPU box)")
+# ---- against the reference's feature2adj / preprocess_graph (fixture: oracle/make_golden.py::_feature2adj_fixture) --------------
+def _csr(g, key, n):
+    return sp.csr_matrix((g[f"{key}.adj_data"], g[f"{key}.adj_indices"], g[f"{key}.adj_indptr"]), shape=(n, n))
 
 
-@needs_ref
-def test_port_vs_live_reference_knn_graph():
-    ref = ref_loader.scgnn2()
+def test_port_vs_live_reference_knn_graph(golden):
+    g = golden("scgnn_feature2adj")
     X = port.synthetic_embedding(257, d=24, n_clusters=5, seed=3)
     for k in (3, 15):
-        _, adj_train_ref, edges = ref.feature2adj(X, k, False)
         adj, idx = port.feature2adj(X, k)
-        assert np.array_equal(idx.reshape(-1), np.array([e[1] for e in edges]))
-        assert (sp.csr_matrix(adj_train_ref) != adj).nnz == 0
-        an_ref = ref.preprocess_graph(adj_train_ref).coalesce()
+        assert np.array_equal(idx.reshape(-1), g[f"k{k}.edges_dst"])
+        assert (_csr(g, f"k{k}", len(X)) != adj).nnz == 0
         an = port.preprocess_graph(adj).tocoo()
-        assert np.array_equal(an_ref.values().numpy(), an.data)
-        assert np.array_equal(an_ref.indices().numpy(), np.vstack((an.row, an.col)))
+        assert np.array_equal(g[f"k{k}.norm_values"], an.data)
+        assert np.array_equal(g[f"k{k}.norm_indices"], np.vstack((an.row, an.col)))
 
 
-@needs_ref
-def test_port_vs_live_reference_fractional_neighbourhood():
+def test_port_vs_live_reference_fractional_neighbourhood(golden):
     # neighborhood_factor <= 1 means a fraction of N (scgnn2.py:651-654); default 0.05
-    ref = ref_loader.scgnn2()
+    g = golden("scgnn_feature2adj")
     X = port.synthetic_embedding(120, d=8, n_clusters=3, seed=9)
-    _, adj_train_ref, _ = ref.feature2adj(X, 0.05, False)
     adj, idx = port.feature2adj(X, 0.05)
-    assert idx.shape[1] == 6 and (sp.csr_matrix(adj_train_ref) != adj).nnz == 0
+    assert idx.shape[1] == 6 and (_csr(g, "frac", len(X)) != adj).nnz == 0
 
 
 def test_graph_ae_gat_golden(golden):
@@ -393,7 +388,7 @@ def test_umap_connectivities_against_closed_forms():
 
 
 def _trunc32(x):
-    """Round a float64 array toward zero to fp32 precision (the accumulate behaviour measured for tcgen05 + TMEM)."""
+    """Round a float64 array toward zero to fp32 precision (the worst case assumed for the tensor-core accumulate)."""
     y = x.astype(np.float32)
     over = np.abs(y.astype(np.float64)) > np.abs(x)
     return np.where(over, np.nextafter(y, np.float32(0)), y).astype(np.float32)
@@ -419,7 +414,7 @@ def test_knn_tensor_core_filter_error_bound_is_sound(d, scale):
     hi64, lo64 = hi.astype(np.float64), lo.astype(np.float64)
     q = slice(0, 60)
     acc = np.zeros((60, n), np.float32)
-    for k0 in range(0, dp, 16):                                  # one tcgen05.mma per product and 16-feature step
+    for k0 in range(0, dp, 16):                                  # one MMA per product and 16-feature step
         ks = slice(k0, k0 + 16)
         for a, b in ((lo64, hi64), (hi64, lo64), (hi64, hi64)):
             acc = _trunc32(acc.astype(np.float64) + a[q, ks] @ b[:, ks].T)
@@ -435,46 +430,44 @@ def test_knn_tensor_core_filter_error_bound_is_sound(d, scale):
     assert worst.max() < 0.5                                                 # comfortable margin, not a knife edge
 
 
-def test_decoder_fp16_split_scheme_precision_on_host():
-    """Host emulation of the arithmetic of gae_tch.cu (the fp16 hi/lo-split tcgen05 decoder): logits from
-    [fp16 pairs of log2(e)·z_i] · [fp16 pairs of z_j] with truncating fp32 accumulation, σ·2^11 split by mantissa mask into an
-    exact fp16 hi and a rounded fp16 lo, gradient product against fp16 pairs of 2^e·z_j — against fp64.  Shows the scheme
-    carries fp32-grade precision (what lets the GPU tests hold 2e-6 on the loss and 2e-5 on dz)."""
+def _tf32(x):
+    """Truncate fp32 values to tf32 (the operand precision of the tensor-core MMA: top 19 bits of the fp32 container)."""
+    return (np.ascontiguousarray(x, dtype=np.float32).view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
+
+
+def test_decoder_tf32_split_scheme_precision_on_host():
+    """Host emulation of the arithmetic of gae_tc.cu (the tf32 hi/lo-split tensor-core decoder): logits from the three products
+    lo·hi + hi·lo + hi·hi of hi = x & 0xFFFFE000 and lo = x − hi (lo truncated to tf32 by the MMA), per-tile accumulation with
+    truncating adds; σ split the same way for the gradient product against Z_J, tiles summed in fp32 — against fp64.  Shows the
+    scheme carries fp32-grade precision (what lets the GPU tests hold 2e-6 on the loss and 2e-5 on dz)."""
     rng = np.random.default_rng(3)
-    n, d = 512, 16
+    n, d, bt = 512, 16, 128
     z = (rng.normal(size=(n, d)) * 0.4).astype(np.float32)
-    LOG2E = np.float32(1.4426950408889634)
 
-    def split16(x):
-        h = x.astype(np.float16)
-        return h, (x - h.astype(np.float32)).astype(np.float16)
+    def split(x):
+        h = _tf32(x)
+        return h, _tf32(x - h)
 
-    ah, al = split16(z * LOG2E)                     # A operand of the S product
-    bh, bl = split16(z)                             # B operand of the S product
+    zh, zl = split(z)
     acc = np.zeros((n, n), np.float32)
-    for a, b in ((al, bh), (ah, bl), (ah, bh)):     # one K = 16 step, three products, truncating adds
-        acc = _trunc32(acc.astype(np.float64) + a.astype(np.float64) @ b.astype(np.float64).T)
+    for k0 in range(0, d, 8):                       # K = 8 per instruction, three products, truncating adds
+        ks = slice(k0, k0 + 8)
+        for a, b in ((zl, zh), (zh, zl), (zh, zh)):
+            acc = _trunc32(acc.astype(np.float64) + a[:, ks].astype(np.float64) @ b[:, ks].astype(np.float64).T)
     x_true = z.astype(np.float64) @ z.astype(np.float64).T
-    v_true = x_true * 1.4426950408889634
-    assert np.abs(acc - v_true).max() < 4e-6 * np.abs(v_true).max()            # logits: ≈ 2^-18 relative to the largest logit
-    # σ(x)·2048 → hi by mantissa mask (exact in fp16), lo rounded to fp16
-    g = (2048.0 / (1.0 + np.exp2(-np.abs(acc.astype(np.float64))))).astype(np.float32)
-    g = np.where(acc >= 0, g, (np.exp2(-np.abs(acc.astype(np.float64))) * g).astype(np.float32)).astype(np.float32)
-    hi = (g.view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
-    assert np.array_equal(hi.astype(np.float16).astype(np.float32), hi)        # the masked value IS an fp16 number
-    lo = (g - hi).astype(np.float16)
-    assert np.abs(hi.astype(np.float64) + lo.astype(np.float64) - g).max() <= 2.0**-21 * 2048     # 22 significant bits of σ
-    # dZ = G · Z with the ZT operand scaled by 2^e
-    e = 9 - int(np.frexp(np.abs(z).max())[1])
-    th, tl = split16(z * np.float32(2.0**e))
-    big = np.zeros((n, d), np.float32)
-    small = np.zeros((n, d), np.float32)
-    for k0 in range(0, n, 16):                      # K = 16 columns j per instruction, separate big / small accumulators
-        ks = slice(k0, k0 + 16)
-        big = _trunc32(big.astype(np.float64) + hi[:, ks].astype(np.float64) @ th[ks].astype(np.float64))
-        small = _trunc32(small.astype(np.float64) + lo[:, ks].astype(np.float64) @ th[ks].astype(np.float64))
-        small = _trunc32(small.astype(np.float64) + hi[:, ks].astype(np.float64) @ tl[ks].astype(np.float64))
-    dz = (big.astype(np.float64) + small) * 2.0**-e / 2048.0
+    assert np.abs(acc - x_true).max() < 4e-6 * np.abs(x_true).max()            # logits: ≈ 2^-18 relative to the largest logit
+    g = (1.0 / (1.0 + np.exp(-acc.astype(np.float64)))).astype(np.float32)
+    gh, gl = split(g)
+    dz = np.zeros((n, d), np.float32)
+    for j0 in range(0, n, bt):                      # one J tile: 16 k-steps of 8 columns accumulate in the MMA registers
+        big = np.zeros((n, d), np.float32)
+        small = np.zeros((n, d), np.float32)
+        for k0 in range(j0, j0 + bt, 8):
+            ks = slice(k0, k0 + 8)
+            big = _trunc32(big.astype(np.float64) + gh[:, ks].astype(np.float64) @ zh[ks].astype(np.float64))
+            small = _trunc32(small.astype(np.float64) + gl[:, ks].astype(np.float64) @ zh[ks].astype(np.float64))
+            small = _trunc32(small.astype(np.float64) + gh[:, ks].astype(np.float64) @ zl[ks].astype(np.float64))
+        dz = (dz + (big + small)).astype(np.float32)  # the tile's sum joins the fp32 total (round to nearest)
     sig = 1.0 / (1.0 + np.exp(-x_true))
     dz_true = sig @ z.astype(np.float64)
     assert np.linalg.norm(dz - dz_true) / np.linalg.norm(dz_true) < 2e-6

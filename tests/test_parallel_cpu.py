@@ -161,8 +161,8 @@ def _dp_feature_ae_case(rank, world):
 
 
 def test_symmetric_decoder_schedule_covers_every_block_pair_once():
-    """gsym::Sweep (csrc/gae_sym.cu) restated on the host: over all super-blocks every unordered pair of 128-row blocks appears
-    exactly once, the work per super-block is balanced, and contiguous super-block ranges (the multi-GPU shards) partition it."""
+    """The decoder's super-blocks (csrc/gae_tc.cu) restated on the host: over all super-blocks every ordered pair of 128-row blocks
+    appears exactly once, the work per super-block is balanced, and contiguous super-block ranges (the multi-GPU shards) partition it."""
     from dance_b200.parallel import shard_bounds, sym_schedule, sym_super_blocks
     for nb in list(range(1, 14)) + [31, 32, 61]:
         nsb = (nb + 1) // 2
@@ -173,12 +173,12 @@ def test_symmetric_decoder_schedule_covers_every_block_pair_once():
             tiles = sym_schedule(nb, sb)
             loads.append(len(tiles))
             for I, J in tiles:
-                key = (min(I, J), max(I, J))
+                key = (I, J)
                 assert key not in seen, (nb, key)
                 seen[key] = sb
-                assert I in (2 * sb, 2 * sb + 1)
-        assert len(seen) == nb * (nb + 1) // 2, nb
-        full = [l for l, sb in zip(loads, range(nsb)) if 2 * sb + 1 < nb]
+                assert I in (sb, nb - 1 - sb)
+        assert len(seen) == nb * nb, nb
+        full = [l for l, sb in zip(loads, range(nsb)) if sb != nb - 1 - sb]
         if full:
             assert max(full) - min(full) <= 2, (nb, loads)
         for world in (2, 3):
@@ -188,8 +188,8 @@ def test_symmetric_decoder_schedule_covers_every_block_pair_once():
 
 def _pair_sharded_decoder_case(rank, world):
     """Pair-sharded decoder gradient (GraphAEEngine.train_step under sharding): each rank evaluates the tiles of its super-blocks —
-    dZ_I += G·Z_J and dZ_J += Gᵀ·Z_I for I ≠ J — into a full-size buffer; the all-reduced sum equals the dense gradient and the
-    loss shares (off-diagonal tiles counted twice) add up to the dense loss.  torch-CPU arithmetic in place of the CUDA kernel."""
+    dZ_I += G·Z_J — into a full-size buffer; the all-reduced sum equals the dense gradient and the loss shares add up to the dense
+    loss.  torch-CPU arithmetic in place of the CUDA kernel."""
     from dance_b200.parallel import Comm, shard_bounds, sym_schedule, sym_super_blocks
     comm = Comm()
     torch.manual_seed(0)
@@ -206,9 +206,7 @@ def _pair_sharded_decoder_case(rank, world):
             S = z[ri] @ z[rj].t()
             G = torch.sigmoid(S)
             dz[ri] += G @ z[rj]
-            if I != J:
-                dz[rj] += G.t() @ z[ri]
-            loss += torch.nn.functional.softplus(S).sum() * (1 if I == J else 2)
+            loss += torch.nn.functional.softplus(S).sum()
     dz *= 2
     comm.allreduce_sum_(dz)
     comm.allreduce_sum_(loss)
@@ -300,8 +298,9 @@ def test_symmetric_decoder_step_ranges_cover_every_tile_once():
                 assert parts[0][0] == 0 and parts[-1][1] == len(steps) and all(a[1] == b[0] for a, b in zip(parts, parts[1:]))
                 got = [t for s0, s1 in parts for st in steps[s0:s1] for t in st]
                 assert got == flat
-            seen.update((min(i, j), max(i, j)) for i, j in flat)
-        assert len(seen) == nb * (nb + 1) // 2          # every unordered block pair exactly once over all super-blocks
+            assert not seen.intersection(flat)
+            seen.update(flat)
+        assert len(seen) == nb * nb                     # every ordered block pair exactly once over all super-blocks
 
 
 def test_spmm_stream_partition_balances_rows_and_nonzeros():

@@ -74,10 +74,11 @@ _SIGNATURES = {
     "b2_gat_aggregate_fwd_f32": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_i32, C.c_int, c_f32, C.c_int,
                                            c_vp, c_vp, c_i64, c_vp, c_vp]),
     "b2_gat_aggregate_bwd_f32": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64,
-                                           c_i32, c_i32, c_i32, C.c_int, c_f32, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+                                           c_i32, c_i32, c_i32, C.c_int, c_f32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                           c_vp, c_vp]),
     "b2_gat_aggregate_bwd_tied_f32": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64,
-                                                c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_i32, C.c_int, c_f32, c_vp, c_i64, c_vp, c_i64,
-                                                c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+                                                c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_i32, C.c_int, c_f32, c_vp, c_vp, c_i64, c_vp,
+                                                c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "b2_gat_combine_fwd_f32": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i32, c_i32, c_i32, C.c_int, C.c_int, c_vp, c_i64, c_vp]),
     "b2_gat_combine_bwd_f32": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_i32, C.c_int, C.c_int, c_vp, c_i64, c_vp, c_i64,
                                          c_vp]),

@@ -47,8 +47,9 @@ gat_scores_kernel(const float* __restrict__ H, int64_t ldh, const float* __restr
 }
 
 __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
-  // total order on floats via signed/unsigned integer views
-  if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
+  // total order on floats via signed/unsigned integer views, chosen by the sign BIT: -0.0 compares >= 0 but its int view is
+  // INT_MIN, which would never replace the initial -inf under the signed max
+  if (!signbit(v)) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
   else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 
@@ -188,16 +189,22 @@ gat_aggregate_fwd_kernel(const int32_t* __restrict__ rowptr, const int32_t* __re
 
 // Backward, part 1 (by target): dα_e,h = <dOut[v,h,:], H[u,h,:]> ; dscore = α (dα - Σ α dα) ;
 // dpre = dscore · act'(pre) → dpre_edge[p,h] ; ds_trg[v,h] = Σ_e dpre.
+// With a global shift c (gmax != NULL) the softmax is shift-invariant only up to the +1e-16 of the denominator:
+// ∂α_e/∂c = -α_e ε/(S+ε) with S = Σ_e exp(score - c), so ∂L/∂c = -Σ_{v,h} (Σ α dα) ε/(S+ε).  That sum goes to
+// shift_acc[0] and the number of (edge, head) scores equal to c to shift_acc[1]; gat_bwd_shift_kernel routes it.
 __global__ void __launch_bounds__(256)
 gat_bwd_target_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
                       const float* __restrict__ H, int64_t ldh, const float* __restrict__ s_src,
                       const float* __restrict__ s_trg, const float* __restrict__ alpha,
                       const float* __restrict__ dOut, int64_t lddo, const float* __restrict__ H2, int64_t ldh2,
                       const float* __restrict__ dOut2, int64_t lddo2, int32_t n, int32_t nh, int32_t F, int act,
-                      float slope, float* __restrict__ dpre_edge, float* __restrict__ ds_trg) {
+                      float slope, const float* __restrict__ gmax, float* __restrict__ dpre_edge, float* __restrict__ ds_trg,
+                      float* __restrict__ shift_acc) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const float gm = gmax ? *gmax : 0.f;
+  float dshift = 0.f, ties = 0.f;
   for (int64_t v = warp; v < n; v += nwarps) {
     const int32_t s = rowptr[v], e = rowptr[v + 1];
     for (int h = 0; h < nh; ++h) {
@@ -213,7 +220,7 @@ gat_bwd_target_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restr
         t = fmaf(alpha[(int64_t)p * nh + h], d, t);
       }
       __syncwarp();
-      float st = 0.f;
+      float st = 0.f, S = 0.f;
       for (int32_t p = s; p < e; ++p) {
         const int32_t u = colidx[p];
         const float d = dpre_edge[(int64_t)p * nh + h];      // the dot of the first sweep (written by lane 0, visible after __syncwarp)
@@ -222,8 +229,50 @@ gat_bwd_target_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restr
         const float g = a * (d - t) * score_act_grad(pre, act, slope);
         if (lane == 0) dpre_edge[(int64_t)p * nh + h] = g;
         st += g;
+        if (gmax) {
+          const float sc = score_act_f(pre, act, slope);
+          S += expf(sc - gm);
+          ties += (sc == gm) ? 1.f : 0.f;
+        }
       }
       if (lane == 0) ds_trg[v * nh + h] = st;
+      // ε/(S+ε) directly: 1 - Σα would cancel catastrophically wherever S ≫ ε
+      if (gmax && e > s) dshift = fmaf(-t, 1e-16f / (S + 1e-16f), dshift);
+    }
+  }
+  if (gmax && lane == 0 && (dshift != 0.f || ties != 0.f)) {
+    atomicAdd(shift_acc, dshift);
+    atomicAdd(shift_acc + 1, ties);
+  }
+}
+
+// Backward of the global shift c = max over every (edge, head) score: ∂L/∂c (shift_acc[0]) is split evenly over the
+// scores equal to c (shift_acc[1] of them), as torch's full-reduction max does, then taken through the score activation
+// into dpre_edge and ds_trg (gat_bwd_source_kernel sums dpre_edge into ds_src afterwards).
+__global__ void __launch_bounds__(256)
+gat_bwd_shift_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
+                     const float* __restrict__ s_src, const float* __restrict__ s_trg, int32_t n, int32_t nh, int act,
+                     float slope, const float* __restrict__ gmax, const float* __restrict__ shift_acc,
+                     float* __restrict__ dpre_edge, float* __restrict__ ds_trg) {
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const float gm = *gmax, ties = shift_acc[1];
+  if (ties == 0.f) return;
+  const float dc = shift_acc[0] / ties;
+  if (dc == 0.f) return;
+  for (int64_t v = warp; v < n; v += nwarps) {
+    const int32_t s = rowptr[v], e = rowptr[v + 1];
+    for (int32_t p = s + lane; p < e; p += 32) {
+      const int32_t u = colidx[p];
+      for (int h = 0; h < nh; ++h) {
+        const float pre = s_src[(int64_t)u * nh + h] + s_trg[v * nh + h];
+        if (score_act_f(pre, act, slope) == gm) {
+          const float g = dc * score_act_grad(pre, act, slope);
+          dpre_edge[(int64_t)p * nh + h] += g;
+          atomicAdd(ds_trg + v * nh + h, g);
+        }
+      }
     }
   }
 }
@@ -376,9 +425,9 @@ using namespace b2;
 
 extern "C" int b2_gat_scores_f32(const float* H, int64_t ldh, const float* a_src, const float* a_trg, int32_t n,
                                  int32_t nheads, int32_t F, float* s_src, float* s_trg, void* stream) {
-  B2_REQUIRE(H && a_src && a_trg && s_src && s_trg && n >= 0 && nheads > 0 && F > 0 && ldh >= (int64_t)nheads * F,
-             "b2_gat_scores_f32: bad arguments");
+  B2_REQUIRE(n >= 0 && nheads > 0 && F > 0 && ldh >= (int64_t)nheads * F, "b2_gat_scores_f32: bad arguments");
   if (n == 0) return B2_OK;
+  B2_REQUIRE(H && a_src && a_trg && s_src && s_trg, "b2_gat_scores_f32: null pointer");
   gat_scores_kernel<<<warp_rows_grid(n), 256, 0, as_stream(stream)>>>(H, ldh, a_src, a_trg, n, nheads, F, s_src, s_trg);
   B2_CHECK_LAUNCH("gat_scores_kernel");
   return B2_OK;
@@ -387,11 +436,12 @@ extern "C" int b2_gat_scores_f32(const float* H, int64_t ldh, const float* a_src
 extern "C" int b2_gat_edge_max_f32(const int32_t* rowptr, const int32_t* colidx, const float* s_src,
                                    const float* s_trg, int32_t n, int32_t nheads, int score_act, float slope,
                                    float* gmax_dev, void* stream) {
-  B2_REQUIRE(rowptr && colidx && s_src && s_trg && gmax_dev && n >= 0 && nheads > 0, "b2_gat_edge_max_f32: bad arguments");
+  B2_REQUIRE(gmax_dev && n >= 0 && nheads > 0, "b2_gat_edge_max_f32: bad arguments");
   cudaStream_t st = as_stream(stream);
   set_neg_inf_kernel<<<1, 1, 0, st>>>(gmax_dev);
   B2_CHECK_LAUNCH("set_neg_inf_kernel");
   if (n == 0) return B2_OK;
+  B2_REQUIRE(rowptr && colidx && s_src && s_trg, "b2_gat_edge_max_f32: null pointer");
   gat_edge_max_kernel<<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, s_src, s_trg, n, nheads, score_act, slope, gmax_dev);
   B2_CHECK_LAUNCH("gat_edge_max_kernel");
   return B2_OK;
@@ -401,11 +451,11 @@ extern "C" int b2_gat_aggregate_fwd_f32(const int32_t* rowptr, const int32_t* co
                                         const float* s_src, const float* s_trg, int32_t n, int32_t nheads, int32_t F,
                                         int score_act, float slope, int shift_mode, const float* gmax_dev, float* out,
                                         int64_t ldo, float* alpha_out, void* stream) {
-  B2_REQUIRE(rowptr && colidx && H && s_src && s_trg && out, "b2_gat_aggregate_fwd_f32: null pointer");
   B2_REQUIRE(n >= 0 && nheads > 0 && F > 0 && (int64_t)nheads * F <= 512 && ldh >= (int64_t)nheads * F && ldo >= (int64_t)nheads * F,
              "b2_gat_aggregate_fwd_f32: nheads*F must be <= 512 and leading dimensions >= nheads*F");
   B2_REQUIRE(shift_mode == 1 || gmax_dev, "b2_gat_aggregate_fwd_f32: global shift needs gmax_dev");
   if (n == 0) return B2_OK;
+  B2_REQUIRE(rowptr && colidx && H && s_src && s_trg && out, "b2_gat_aggregate_fwd_f32: null pointer");
   gat_aggregate_fwd_kernel<<<warp_rows_grid(n), 256, 0, as_stream(stream)>>>(rowptr, colidx, H, ldh, s_src, s_trg, n, nheads, F,
                                                                            score_act, slope, shift_mode, gmax_dev, out, ldo,
                                                                            alpha_out);
@@ -418,23 +468,33 @@ static int gat_aggregate_bwd_impl(const int32_t* rowptr, const int32_t* colidx, 
                                   const float* a_src, const float* a_trg, const float* s_src, const float* s_trg,
                                   const float* alpha, const float* dOut, int64_t lddo, const float* H2, int64_t ldh2,
                                   const float* dOut2, int64_t lddo2, int32_t n, int32_t nheads, int32_t F, int score_act,
-                                  float slope, float* dH, int64_t lddh, float* dH2, int64_t lddh2, float* da_src,
-                                  float* da_trg, float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws, void* stream) {
-  B2_REQUIRE(rowptr && colidx && t_rowptr && t_colidx && t_perm && H && a_src && a_trg && s_src && s_trg && alpha && dOut &&
-                 dH && da_src && da_trg && ds_src_ws && ds_trg_ws && dpre_edge_ws,
-             "b2_gat_aggregate_bwd_f32: null pointer");
+                                  float slope, const float* gmax_dev, float* dH, int64_t lddh, float* dH2, int64_t lddh2,
+                                  float* da_src, float* da_trg, float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws,
+                                  float* shift_ws, void* stream) {
   B2_REQUIRE(n >= 0 && nheads > 0 && nheads <= 32 && F > 0 && (int64_t)nheads * F <= 512, "b2_gat_aggregate_bwd_f32: bad shape");
-  if (n == 0) return B2_OK;
+  B2_REQUIRE(a_src && a_trg && da_src && da_trg, "b2_gat_aggregate_bwd_f32: null pointer");
+  B2_REQUIRE(!gmax_dev || shift_ws, "b2_gat_aggregate_bwd_f32: a global shift (gmax_dev) needs shift_ws");
   cudaStream_t st = as_stream(stream);
   const int W = nheads * F;
+  B2_CHECK_CUDA(cudaMemsetAsync(da_src, 0, sizeof(float) * W, st));
+  B2_CHECK_CUDA(cudaMemsetAsync(da_trg, 0, sizeof(float) * W, st));
+  if (n == 0) return B2_OK;
+  B2_REQUIRE(rowptr && colidx && t_rowptr && t_colidx && t_perm && H && s_src && s_trg && alpha && dOut && dH && ds_src_ws &&
+                 ds_trg_ws && dpre_edge_ws,
+             "b2_gat_aggregate_bwd_f32: null pointer");
+  if (gmax_dev) B2_CHECK_CUDA(cudaMemsetAsync(shift_ws, 0, sizeof(float) * 2, st));
   gat_bwd_target_kernel<<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, H, ldh, s_src, s_trg, alpha, dOut, lddo, H2, ldh2, dOut2,
-                                                          lddo2, n, nheads, F, score_act, slope, dpre_edge_ws, ds_trg_ws);
+                                                          lddo2, n, nheads, F, score_act, slope, gmax_dev, dpre_edge_ws, ds_trg_ws,
+                                                          shift_ws);
   B2_CHECK_LAUNCH("gat_bwd_target_kernel");
+  if (gmax_dev) {
+    gat_bwd_shift_kernel<<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, s_src, s_trg, n, nheads, score_act, slope, gmax_dev,
+                                                           shift_ws, dpre_edge_ws, ds_trg_ws);
+    B2_CHECK_LAUNCH("gat_bwd_shift_kernel");
+  }
   gat_bwd_source_kernel<<<warp_rows_grid(n), 256, 0, st>>>(t_rowptr, t_colidx, t_perm, alpha, dpre_edge_ws, dOut, lddo,
                                                           dH2 ? dOut2 : nullptr, lddo2, n, nheads, F, dH, lddh, dH2, lddh2, ds_src_ws);
   B2_CHECK_LAUNCH("gat_bwd_source_kernel");
-  B2_CHECK_CUDA(cudaMemsetAsync(da_src, 0, sizeof(float) * W, st));
-  B2_CHECK_CUDA(cudaMemsetAsync(da_trg, 0, sizeof(float) * W, st));
   int splits = ceil_div(sm_count() * 2, ceil_div(W, 32));
   const int max_splits = n / 256 > 0 ? n / 256 : 1;
   if (splits > max_splits) splits = max_splits;
@@ -449,12 +509,12 @@ extern "C" int b2_gat_aggregate_bwd_f32(const int32_t* rowptr, const int32_t* co
                                         const int32_t* t_colidx, const int32_t* t_perm, const float* H, int64_t ldh,
                                         const float* a_src, const float* a_trg, const float* s_src, const float* s_trg,
                                         const float* alpha, const float* dOut, int64_t lddo, int32_t n, int32_t nheads,
-                                        int32_t F, int score_act, float slope, float* dH, int64_t lddh, float* da_src,
-                                        float* da_trg, float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws,
-                                        void* stream) {
+                                        int32_t F, int score_act, float slope, const float* gmax_dev, float* dH, int64_t lddh,
+                                        float* da_src, float* da_trg, float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws,
+                                        float* shift_ws, void* stream) {
   return gat_aggregate_bwd_impl(rowptr, colidx, t_rowptr, t_colidx, t_perm, H, ldh, a_src, a_trg, s_src, s_trg, alpha, dOut, lddo,
-                                nullptr, 0, nullptr, 0, n, nheads, F, score_act, slope, dH, lddh, nullptr, 0, da_src, da_trg,
-                                ds_src_ws, ds_trg_ws, dpre_edge_ws, stream);
+                                nullptr, 0, nullptr, 0, n, nheads, F, score_act, slope, gmax_dev, dH, lddh, nullptr, 0, da_src,
+                                da_trg, ds_src_ws, ds_trg_ws, dpre_edge_ws, shift_ws, stream);
 }
 
 extern "C" int b2_gat_aggregate_bwd_tied_f32(const int32_t* rowptr, const int32_t* colidx, const int32_t* t_rowptr,
@@ -462,20 +522,21 @@ extern "C" int b2_gat_aggregate_bwd_tied_f32(const int32_t* rowptr, const int32_
                                              const float* a_src, const float* a_trg, const float* s_src, const float* s_trg,
                                              const float* alpha, const float* dOut, int64_t lddo, const float* H2, int64_t ldh2,
                                              const float* dOut2, int64_t lddo2, int32_t n, int32_t nheads, int32_t F,
-                                             int score_act, float slope, float* dH, int64_t lddh, float* dH2, int64_t lddh2,
-                                             float* da_src, float* da_trg, float* ds_src_ws, float* ds_trg_ws,
-                                             float* dpre_edge_ws, void* stream) {
-  B2_REQUIRE(H2 && dOut2, "b2_gat_aggregate_bwd_tied_f32: the second layer's H2 / dOut2 are required (dH2 may be NULL)");
+                                             int score_act, float slope, const float* gmax_dev, float* dH, int64_t lddh,
+                                             float* dH2, int64_t lddh2, float* da_src, float* da_trg, float* ds_src_ws,
+                                             float* ds_trg_ws, float* dpre_edge_ws, float* shift_ws, void* stream) {
+  B2_REQUIRE(n == 0 || (H2 && dOut2), "b2_gat_aggregate_bwd_tied_f32: the second layer's H2 / dOut2 are required (dH2 may be NULL)");
   return gat_aggregate_bwd_impl(rowptr, colidx, t_rowptr, t_colidx, t_perm, H, ldh, a_src, a_trg, s_src, s_trg, alpha, dOut, lddo,
-                                H2, ldh2, dOut2, lddo2, n, nheads, F, score_act, slope, dH, lddh, dH2, lddh2, da_src, da_trg,
-                                ds_src_ws, ds_trg_ws, dpre_edge_ws, stream);
+                                H2, ldh2, dOut2, lddo2, n, nheads, F, score_act, slope, gmax_dev, dH, lddh, dH2, lddh2, da_src,
+                                da_trg, ds_src_ws, ds_trg_ws, dpre_edge_ws, shift_ws, stream);
 }
 
 extern "C" int b2_gat_combine_fwd_f32(const float* agg, int64_t ldagg, const float* skip, int64_t ldskip, const float* bias,
                                       int32_t n, int32_t nheads, int32_t F, int concat, int act, float* out, int64_t ldo,
                                       void* stream) {
-  B2_REQUIRE(agg && out && n >= 0 && nheads > 0 && F > 0, "b2_gat_combine_fwd_f32: bad arguments");
+  B2_REQUIRE(n >= 0 && nheads > 0 && F > 0, "b2_gat_combine_fwd_f32: bad arguments");
   if (n == 0) return B2_OK;
+  B2_REQUIRE(agg && out, "b2_gat_combine_fwd_f32: null pointer");
   gat_combine_fwd_kernel<<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
       agg, ldagg, skip, ldskip, bias, n, nheads, F, concat, act, out, ldo);
   B2_CHECK_LAUNCH("gat_combine_fwd_kernel");
@@ -485,8 +546,9 @@ extern "C" int b2_gat_combine_fwd_f32(const float* agg, int64_t ldagg, const flo
 extern "C" int b2_gat_combine_bwd_f32(const float* dout, int64_t lddo, const float* out, int64_t ldo, int32_t n,
                                       int32_t nheads, int32_t F, int concat, int act, float* dpre, int64_t ldp, float* dact,
                                       int64_t ldact, void* stream) {
-  B2_REQUIRE(dout && out && dpre && n >= 0 && nheads > 0 && F > 0, "b2_gat_combine_bwd_f32: bad arguments");
+  B2_REQUIRE(n >= 0 && nheads > 0 && F > 0, "b2_gat_combine_bwd_f32: bad arguments");
   if (n == 0) return B2_OK;
+  B2_REQUIRE(dout && out && dpre, "b2_gat_combine_bwd_f32: null pointer");
   gat_combine_bwd_kernel<<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
       dout, lddo, out, ldo, n, nheads, F, concat, act, dpre, ldp, dact, ldact);
   B2_CHECK_LAUNCH("gat_combine_bwd_kernel");

@@ -128,13 +128,14 @@ extern "C" size_t b2_csr_transpose_workspace_bytes(int32_t n_rows, int32_t n_col
 extern "C" int b2_csr_transpose(const int32_t* rowptr, const int32_t* colidx, const float* vals, int32_t n_rows,
                                 int32_t n_cols, int64_t nnz, int32_t* t_rowptr, int32_t* t_colidx, float* t_vals,
                                 int32_t* perm_out, void* workspace, size_t workspace_bytes, void* stream) {
-  B2_REQUIRE(rowptr && colidx && t_rowptr && t_colidx, "b2_csr_transpose: null pointer");
+  B2_REQUIRE(rowptr && t_rowptr, "b2_csr_transpose: null pointer");
   B2_REQUIRE(nnz >= 0 && nnz < (1ll << 31), "b2_csr_transpose: nnz out of range");
   cudaStream_t st = as_stream(stream);
-  if (nnz == 0) {
+  if (nnz == 0) {   // an edgeless matrix: colidx / t_colidx may have no storage
     B2_CHECK_CUDA(cudaMemsetAsync(t_rowptr, 0, sizeof(int32_t) * ((size_t)n_cols + 1), st));
     return B2_OK;
   }
+  B2_REQUIRE(colidx && t_colidx, "b2_csr_transpose: null pointer");
   B2_REQUIRE(workspace && workspace_bytes >= b2_csr_transpose_workspace_bytes(n_rows, n_cols, nnz),
              "b2_csr_transpose: workspace too small");
   WsCarver ws(workspace, workspace_bytes);

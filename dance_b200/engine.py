@@ -420,10 +420,10 @@ class GATEngine:
             hs = ops.gemm(h, P[f"l{l}.projskip"], transB=True, precision=pr)         # [n, 2W]: projection | skip projection
             H, skip = hs[:, :W], hs[:, W:]
             s_src, s_trg = ops.gat_scores(H, P[f"l{l}.a_src"], P[f"l{l}.a_trg"], nh)
-            agg, alpha, _ = ops.gat_aggregate_fwd(T, H, s_src, s_trg, nh, "leakyrelu", 0.2, "global", keep_alpha=keep)
+            agg, alpha, gmax = ops.gat_aggregate_fwd(T, H, s_src, s_trg, nh, "leakyrelu", 0.2, "global", keep_alpha=keep)
             out = ops.gat_combine_fwd(agg, skip, P[f"l{l}.bias"], nh, L["concat"], L["act"])
             if keep:
-                self._cache[l] = dict(x=h, hs=hs, s_src=s_src, s_trg=s_trg, alpha=alpha, out=out)
+                self._cache[l] = dict(x=h, hs=hs, s_src=s_src, s_trg=s_trg, alpha=alpha, gmax=gmax, out=out)
             h = out
         return h
 
@@ -448,7 +448,7 @@ class GATEngine:
             ops.colsum(dact, out=G[f"l{l}.bias"])
             H = c["hs"][:, :W]
             dHm, da_src, da_trg = ops.gat_aggregate_bwd(T, Tt, t_perm, H, P[f"l{l}.a_src"], P[f"l{l}.a_trg"], c["s_src"], c["s_trg"],
-                                                        c["alpha"], dskip, nh)
+                                                        c["alpha"], dskip, nh, gmax=c["gmax"])
             dH.copy_(dHm)
             G[f"l{l}.a_src"].copy_(da_src)
             G[f"l{l}.a_trg"].copy_(da_trg)

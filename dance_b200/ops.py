@@ -506,11 +506,17 @@ SCORE_ACT = {"leakyrelu": 0, "sigmoid": 1}
 SHIFT = {"global": 0, "segment": 1}
 
 
+def _head_width(W: int, nheads: int, what: str) -> int:
+    if nheads <= 0 or W % nheads:
+        raise B2Error(f"{what}: width {W} is not a multiple of nheads={nheads}")
+    return W // nheads
+
+
 def gat_scores(H, a_src, a_trg, nheads: int):
     """s_src[n,h] = <H[n,h,:], a_src[h,:]> (scgnn2.py:1016-1017)."""
     _chk(H, torch.float32, "H", 2)
     n, W = H.shape
-    F = W // nheads
+    F = _head_width(W, nheads, "gat_scores")
     s_src = torch.empty((n, nheads), dtype=torch.float32, device=H.device)
     s_trg = torch.empty((n, nheads), dtype=torch.float32, device=H.device)
     check(lib().b2_gat_scores_f32(_p(H), _rowmajor(H, "H"), _p(a_src), _p(a_trg), n, nheads, F, _p(s_src), _p(s_trg), _stream()),
@@ -520,28 +526,35 @@ def gat_scores(H, a_src, a_trg, nheads: int):
 
 def gat_aggregate_fwd(T: CSR, H, s_src, s_trg, nheads: int, score_act="leakyrelu", slope=0.2, shift="global",
                       out=None, keep_alpha=True):
-    """Fused edge softmax + aggregate on the target-indexed CSR ``T``; returns (out, alpha, gmax)."""
+    """Fused edge softmax + aggregate on the target-indexed CSR ``T``; returns (out, alpha, gmax).
+
+    ``gmax`` [1] is the global shift (``shift="global"``; -inf for a graph without edges) and is what
+    :func:`gat_aggregate_bwd` needs to differentiate through it."""
     n, W = H.shape
-    F = W // nheads
+    F = _head_width(W, nheads, "gat_aggregate_fwd")
     if out is None:
         out = torch.empty((n, W), dtype=torch.float32, device=H.device)
     gmax = torch.empty(1, dtype=torch.float32, device=H.device)
     act, sm = SCORE_ACT[score_act], SHIFT[shift]
+    colidx = _p(T.colidx) if T.nnz else _p(T.rowptr)  # an edgeless graph has no colidx storage; never dereferenced
     if sm == 0:
-        check(lib().b2_gat_edge_max_f32(_p(T.rowptr), _p(T.colidx), _p(s_src), _p(s_trg), n, nheads, act, slope, _p(gmax),
+        check(lib().b2_gat_edge_max_f32(_p(T.rowptr), colidx, _p(s_src), _p(s_trg), n, nheads, act, slope, _p(gmax),
                                         _stream()), "b2_gat_edge_max_f32")
     alpha = torch.empty((T.nnz, nheads), dtype=torch.float32, device=H.device) if keep_alpha else None
-    check(lib().b2_gat_aggregate_fwd_f32(_p(T.rowptr), _p(T.colidx), _p(H), _rowmajor(H, "H"), _p(s_src), _p(s_trg), n, nheads,
-                                         F, act, slope, sm, _p(gmax), _p(out), _rowmajor(out, "out"), _p(alpha), _stream()),
-          "b2_gat_aggregate_fwd_f32")
+    check(lib().b2_gat_aggregate_fwd_f32(_p(T.rowptr), colidx, _p(H), _rowmajor(H, "H"), _p(s_src), _p(s_trg), n, nheads,
+                                         F, act, slope, sm, _p(gmax), _p(out), _rowmajor(out, "out"), _p(alpha) if T.nnz else None,
+                                         _stream()), "b2_gat_aggregate_fwd_f32")
     return out, alpha, gmax
 
 
 def gat_aggregate_bwd(T: CSR, Tt: CSR, t_perm, H, a_src, a_trg, s_src, s_trg, alpha, dOut, nheads: int,
-                      score_act="leakyrelu", slope=0.2, H2=None, dOut2=None, want_dH2=True):
-    """Returns (dH, da_src, da_trg), or (dH, da_src, da_trg, dH2 | None) with a tied second layer (H2, dOut2)."""
+                      score_act="leakyrelu", slope=0.2, H2=None, dOut2=None, want_dH2=True, gmax=None):
+    """Returns (dH, da_src, da_trg), or (dH, da_src, da_trg, dH2 | None) with a tied second layer (H2, dOut2).
+
+    ``gmax``: the forward's global shift (third result of :func:`gat_aggregate_fwd` with ``shift="global"``), whose
+    gradient the backward then includes, as the reference does not detach its max; None for ``shift="segment"``."""
     n, W = H.shape
-    F = W // nheads
+    F = _head_width(W, nheads, "gat_aggregate_bwd")
     dev = H.device
     dH = torch.empty((n, W), dtype=torch.float32, device=dev)
     da_src = torch.empty(W, dtype=torch.float32, device=dev)
@@ -549,26 +562,27 @@ def gat_aggregate_bwd(T: CSR, Tt: CSR, t_perm, H, a_src, a_trg, s_src, s_trg, al
     ds_s = torch.empty(n * nheads, dtype=torch.float32, device=dev)
     ds_t = torch.empty(n * nheads, dtype=torch.float32, device=dev)
     dpre = torch.empty(max(T.nnz, 1) * nheads, dtype=torch.float32, device=dev)
+    shift_ws = torch.empty(2, dtype=torch.float32, device=dev) if gmax is not None else None
+    # an edgeless graph has no colidx / t_perm / alpha storage: any non-NULL pointer stands in, never dereferenced
+    edge = (lambda t: _p(t)) if T.nnz else (lambda t: _p(T.rowptr))
+    head = (_p(T.rowptr), edge(T.colidx), _p(Tt.rowptr), edge(Tt.colidx), edge(t_perm), _p(H), _rowmajor(H, "H"), _p(a_src),
+            _p(a_trg), _p(s_src), _p(s_trg), edge(alpha), _p(dOut), _rowmajor(dOut, "dOut"))
     if H2 is not None:
         dH2 = torch.empty((n, W), dtype=torch.float32, device=dev) if want_dH2 else None
-        check(lib().b2_gat_aggregate_bwd_tied_f32(_p(T.rowptr), _p(T.colidx), _p(Tt.rowptr), _p(Tt.colidx), _p(t_perm), _p(H),
-                                                  _rowmajor(H, "H"), _p(a_src), _p(a_trg), _p(s_src), _p(s_trg), _p(alpha), _p(dOut),
-                                                  _rowmajor(dOut, "dOut"), _p(H2), _rowmajor(H2, "H2"), _p(dOut2),
-                                                  _rowmajor(dOut2, "dOut2"), n, nheads, F, SCORE_ACT[score_act], slope, _p(dH),
-                                                  _rowmajor(dH, "dH"), _p(dH2), _rowmajor(dH2, "dH2") if want_dH2 else 0, _p(da_src), _p(da_trg),
-                                                  _p(ds_s), _p(ds_t), _p(dpre), _stream()), "b2_gat_aggregate_bwd_tied_f32")
+        check(lib().b2_gat_aggregate_bwd_tied_f32(*head, _p(H2), _rowmajor(H2, "H2"), _p(dOut2), _rowmajor(dOut2, "dOut2"), n, nheads,
+                                                  F, SCORE_ACT[score_act], slope, _p(gmax), _p(dH), _rowmajor(dH, "dH"), _p(dH2),
+                                                  _rowmajor(dH2, "dH2") if want_dH2 else 0, _p(da_src), _p(da_trg), _p(ds_s), _p(ds_t),
+                                                  _p(dpre), _p(shift_ws), _stream()), "b2_gat_aggregate_bwd_tied_f32")
         return dH, da_src, da_trg, dH2
-    check(lib().b2_gat_aggregate_bwd_f32(_p(T.rowptr), _p(T.colidx), _p(Tt.rowptr), _p(Tt.colidx), _p(t_perm), _p(H),
-                                         _rowmajor(H, "H"), _p(a_src), _p(a_trg), _p(s_src), _p(s_trg), _p(alpha), _p(dOut),
-                                         _rowmajor(dOut, "dOut"), n, nheads, F, SCORE_ACT[score_act], slope, _p(dH),
-                                         _rowmajor(dH, "dH"), _p(da_src), _p(da_trg), _p(ds_s), _p(ds_t), _p(dpre), _stream()),
+    check(lib().b2_gat_aggregate_bwd_f32(*head, n, nheads, F, SCORE_ACT[score_act], slope, _p(gmax), _p(dH), _rowmajor(dH, "dH"),
+                                         _p(da_src), _p(da_trg), _p(ds_s), _p(ds_t), _p(dpre), _p(shift_ws), _stream()),
           "b2_gat_aggregate_bwd_f32")
     return dH, da_src, da_trg
 
 
 def gat_combine_fwd(agg, skip, bias, nheads: int, concat: bool, act=None):
     n, W = agg.shape
-    F = W // nheads
+    F = _head_width(W, nheads, "gat_combine_fwd")
     out = torch.empty((n, W if concat else F), dtype=torch.float32, device=agg.device)
     check(lib().b2_gat_combine_fwd_f32(_p(agg), _rowmajor(agg, "agg"), _p(skip), _rowmajor(skip, "skip") if skip is not None else 0,
                                        _p(bias), n, nheads, F, int(concat), ACT[act], _p(out), _rowmajor(out, "out"), _stream()),

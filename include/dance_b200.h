@@ -277,15 +277,20 @@ int b2_gat_aggregate_fwd_f32(const int32_t* rowptr, const int32_t* colidx,
 /* Backward of scores + aggregate.  (t_rowptr, t_colidx, t_perm) = b2_csr_transpose of the target
  * CSR.  Outputs: dH [n, nheads*F] (overwritten: message path + score path), da_src/da_trg
  * [nheads*F] (overwritten).  ds_src_ws/ds_trg_ws [n*nheads] and dpre_edge_ws [nnz*nheads] are
- * caller-provided scratch. */
+ * caller-provided scratch.
+ *   gmax_dev : the forward's global shift (shift_mode 0) or NULL (per-target shift, whose max is detached
+ *              as in PyG).  The global max is NOT detached in scgnn2.py:1076; since α = p/(Σp + 1e-16) is
+ *              shift-invariant only up to the 1e-16, its gradient reaches the argmax score(s) — split evenly
+ *              over ties, as torch's max — and matters for targets whose scores lie ~37+ below the max.
+ *   shift_ws : [2] caller-provided scratch, needed when gmax_dev is set. */
 int b2_gat_aggregate_bwd_f32(const int32_t* rowptr, const int32_t* colidx,
                              const int32_t* t_rowptr, const int32_t* t_colidx, const int32_t* t_perm,
                              const float* H, int64_t ldh, const float* a_src, const float* a_trg,
                              const float* s_src, const float* s_trg, const float* alpha,
                              const float* dOut, int64_t lddo, int32_t n, int32_t nheads, int32_t F,
-                             int score_act, float slope,
+                             int score_act, float slope, const float* gmax_dev,
                              float* dH, int64_t lddh, float* da_src, float* da_trg,
-                             float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws, void* stream);
+                             float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws, float* shift_ws, void* stream);
 /* Tied attention (STAGATE, stagate.py:197: conv3 reuses conv1's node scores, so the SAME edge coefficients α weight
  * two layers' messages).  As above, plus the second layer's projected features H2 / upstream gradient dOut2:
  *   dα_e = <dOut[v],H[u]> + <dOut2[v],H2[u]> ;  dH2[u] = Σ α dOut2[v] (message path only — the scores depend on H;
@@ -296,9 +301,9 @@ int b2_gat_aggregate_bwd_tied_f32(const int32_t* rowptr, const int32_t* colidx,
                                   const float* s_src, const float* s_trg, const float* alpha,
                                   const float* dOut, int64_t lddo, const float* H2, int64_t ldh2,
                                   const float* dOut2, int64_t lddo2, int32_t n, int32_t nheads, int32_t F,
-                                  int score_act, float slope,
+                                  int score_act, float slope, const float* gmax_dev,
                                   float* dH, int64_t lddh, float* dH2, int64_t lddh2, float* da_src, float* da_trg,
-                                  float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws, void* stream);
+                                  float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws, float* shift_ws, void* stream);
 /* skip connection + concat | head-mean + bias + activation (scgnn2.py:1189-1215):
  *   concat: out[n, nheads*F] = act(agg + skip + bias) ; else out[n,F] = act(mean_h(agg + skip) + bias)
  *   skip may be NULL.  Backward: dpre [n, nheads*F] = d(agg) = d(skip); dact [n, OW] (optional) is the

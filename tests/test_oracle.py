@@ -236,6 +236,77 @@ def test_pyg_lite_primitives_against_dense_formulas():
     assert ei3.tolist() == [[1, 0, 1, 2], [2, 0, 1, 2]]
 
 
+@pytest.mark.parametrize("concat,act", [(True, "elu"), (False, None)])
+def test_gat_fp64_reference_matches_port_and_pyg(concat, act):
+    """oracle/gat_ref.py, the arbiter of tests/test_gpu_gat.py, against oracle.port.gat_layer (global shift, max not detached) and
+    oracle.pyg_lite.softmax (per-target shift) in float64: values and autograd gradients, on a graph with empty targets."""
+    from oracle import gat_ref, pyg_lite
+    rng = np.random.default_rng(7)
+    n, fin, nh, F = 40, 7, 3, 5
+    A = (sp.diags((np.arange(n) >= 4).astype(float)) @ sp.random(n, n, density=0.12, random_state=3)).tocsr()  # 4 empty targets
+    A.eliminate_zeros()
+    A.sort_indices()
+    src, trg = gat_ref.csr_edges(A.indptr, A.indices)
+    assert np.array_equal(src.numpy(), A.indices) and np.array_equal(trg.numpy(), A.tocoo().row)
+    t = lambda *s: torch.from_numpy(rng.normal(scale=0.4, size=s)).requires_grad_()
+    x, proj, skip, a_s, a_t, bias = t(n, fin), t(nh * F, fin), t(nh * F, fin), t(1, nh, F), t(1, nh, F), t(nh * F if concat else F)
+    fact = torch.nn.functional.elu if act == "elu" else None
+    leaves = (x, proj, skip, a_s, a_t, bias)
+    want = port.gat_layer(x, torch.stack([src, trg]), proj, skip, a_s, a_t, bias, concat, fact)
+    up = torch.from_numpy(rng.normal(size=tuple(want.shape)))
+    g_want = torch.autograd.grad((want * up).sum(), leaves)
+
+    def mine(detach_max):
+        H = x @ proj.t()
+        s_src, s_trg = gat_ref.scores(H, a_s, a_t, nh)
+        agg, _ = gat_ref.aggregate(H, s_src, s_trg, src, trg, nh, "leakyrelu", 0.2, "global", detach_max=detach_max)
+        return gat_ref.combine(agg, x @ skip.t(), bias, nh, concat, act)
+
+    got = mine(False)
+    assert torch.allclose(got, want, rtol=1e-12, atol=1e-12)
+    for a, b in zip(torch.autograd.grad((got * up).sum(), leaves), g_want):
+        assert torch.allclose(a, b, rtol=1e-10, atol=1e-12)
+    # at O(1) score spreads the max's gradient is ~ε/S: detaching it changes nothing visible
+    for a, b in zip(torch.autograd.grad((mine(True) * up).sum(), leaves), g_want):
+        assert torch.allclose(a, b, rtol=1e-10, atol=1e-12)
+
+    e = torch.from_numpy(rng.normal(size=(len(src), nh))).requires_grad_()
+    a_want = pyg_lite.softmax(e, trg, None, n)
+    a_got = gat_ref.edge_softmax(e, trg, n, "segment")
+    assert torch.allclose(a_got, a_want, rtol=1e-14, atol=1e-15)
+    w = torch.from_numpy(rng.normal(size=a_want.shape))
+    assert torch.allclose(torch.autograd.grad((a_got * w).sum(), e)[0], torch.autograd.grad((a_want * w).sum(), e)[0], rtol=1e-12, atol=1e-14)
+
+
+def test_gat_fp64_reference_global_shift_gradient_and_tied_layer():
+    """The literal global shift differs from the detached one where a target's scores lie far below the max (Σ exp ≲ 1e-16, so
+    its α no longer sum to 1), and its gradient is then -Σ t ε/(S+ε) at the argmax; the tied layer reuses the same α."""
+    from oracle import gat_ref
+    src = torch.tensor([0, 1, 2, 3, 0])
+    trg = torch.tensor([0, 0, 1, 1, 2])
+    # LeakyReLU(0.2) scores 0, 1 | -36, -38 | 0: the global max is edge 1 (1 → 0); target 1 sits 37 and 39 below it
+    s_src = torch.tensor([[0.0], [1.0], [-180.0], [-190.0]], dtype=torch.float64, requires_grad=True)
+    s_trg = torch.zeros(4, 1, dtype=torch.float64, requires_grad=True)                             # target 3 has no in-edge
+    gen = torch.Generator().manual_seed(0)
+    H, H2, dOut = (torch.randn(4, 2, dtype=torch.float64, generator=gen) for _ in range(3))
+    out, alpha, out2 = gat_ref.aggregate(H, s_src, s_trg, src, trg, 1, H2=H2)
+    assert torch.equal(out2, gat_ref.aggregate(H2, s_src, s_trg, src, trg, 1)[0])
+    S_v = torch.tensor([1.0 + np.exp(-1.0), np.exp(-37.0) + np.exp(-39.0), np.exp(-1.0), 0.0], dtype=torch.float64)
+    assert torch.allclose(alpha.detach()[2:4, 0].sum(), S_v[1] / (S_v[1] + gat_ref.EPS), rtol=1e-12)
+    assert 0.1 < alpha[2:4, 0].sum().item() < 0.9
+    lit = torch.autograd.grad((out * dOut).sum(), (s_src, s_trg))
+    det = torch.autograd.grad((gat_ref.aggregate(H, s_src, s_trg, src, trg, 1, detach_max=True)[0] * dOut).sum(), (s_src, s_trg))
+    # the only difference is ∂L/∂c on the argmax edge 1 → 0, where LeakyReLU' = 1
+    dalpha = (dOut[trg] * H[src]).sum(-1)
+    t_v = torch.zeros(4, dtype=torch.float64).index_add(0, trg, alpha.detach()[:, 0] * dalpha)
+    dc = -(t_v * gat_ref.EPS / (S_v + gat_ref.EPS)).sum()
+    expect_src, expect_trg = det[0].clone(), det[1].clone()
+    expect_src[1, 0] += dc
+    expect_trg[0, 0] += dc
+    assert torch.allclose(lit[0], expect_src, rtol=1e-9, atol=1e-15) and torch.allclose(lit[1], expect_trg, rtol=1e-9, atol=1e-15)
+    assert abs(dc.item()) > 1e-2 * lit[0].abs().max().item()
+
+
 def test_dgl_lite_graphconv_against_dense_formula():
     """oracle/dgl_lite.GraphConv(norm="both") = D_in^-1/2 A D_out^-1/2 applied on the side dgl chooses."""
     from oracle import dgl_lite

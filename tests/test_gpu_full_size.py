@@ -64,7 +64,7 @@ def test_decoder_loss_additive_over_row_shards_at_one_million_cells(cuda, embedd
     assert float((both - dz).norm() / dz.norm()) < 2e-3
     assert np.isfinite(full.item())
     # absolute check of the exact path the benchmark times: sampled rows against the fp64 closed form
-    from test_gpu_kernels import gae_reference_rows
+    from oracle.scgnn_step_ref import gae_reference_rows
     rows = torch.tensor([0, 1, 127, 128, 4097, 437_518, 437_519, 999_999] + list(range(600_000, 600_056)), device=cuda)
     _, ref_rows = gae_reference_rows(z, A.rowptr, A.colidx, 0.5, 100.0, rows)
     err = float((dz[rows].double() - ref_rows).norm() / ref_rows.norm())

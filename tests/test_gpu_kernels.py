@@ -5,6 +5,7 @@ import scipy.sparse as sp
 import torch
 
 from conftest import rel_err
+from oracle.scgnn_step_ref import gae_reference_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -382,36 +383,6 @@ def _dense_gae_reference(z, L_dense, norm, pw, mu=None, lv=None):
     cost = norm * F.binary_cross_entropy_with_logits(logits, L_dense, pos_weight=L_dense * pw)
     cost.backward()
     return cost.item(), z.grad
-
-
-def gae_reference_rows(z, rowptr, colidx, norm, pw, rows, chunk=512):
-    """fp64 closed form of gae_loss_function (scgnn2.py:603-612) restricted to `rows` × all columns, evaluated on the device with
-    torch in row chunks: returns (Σ over those rows of the per-logit cost · norm / n², the gradient rows).  With labels y (pattern
-    of the CSR, unit values) and pos_weight = y·pw:  cost = y·pw·softplus(−x) + (1−y)·softplus(x);  ∂/∂z_i = 2·Σ_j c_ij z_j with
-    c = σ(x) off the pattern and −pw·σ(−x) on it (labels symmetric)."""
-    import torch.nn.functional as F
-    zd = z.double()
-    n = zd.shape[0]
-    rp = rowptr.long()
-    loss = 0.0
-    out = torch.empty(len(rows), zd.shape[1], dtype=torch.float64, device=z.device)
-    for a in range(0, len(rows), chunk):
-        r = rows[a:a + chunk]
-        x = zd[r] @ zd.t()
-        c = torch.sigmoid(x)
-        cost = F.softplus(x)
-        # label pattern of these rows
-        cnt = rp[r + 1] - rp[r]
-        loc = torch.repeat_interleave(torch.arange(len(r), device=z.device), cnt)
-        start = torch.repeat_interleave(rp[r], cnt)
-        within = torch.arange(int(cnt.sum()), device=z.device) - torch.repeat_interleave(torch.cumsum(cnt, 0) - cnt, cnt)
-        cols = colidx.long()[start + within]
-        xe = x[loc, cols]
-        cost[loc, cols] = pw * F.softplus(-xe)
-        c[loc, cols] = -pw * torch.sigmoid(-xe)
-        loss += float(cost.sum())
-        out[a:a + chunk] = 2.0 * (c @ zd)
-    return norm * loss / (float(n) * n), out * (norm / (float(n) * n))
 
 
 def test_gae_loss_tensor_core_single_column_range(cuda):

@@ -569,3 +569,56 @@ def test_plain_c_restatements_agree_with_the_port(golden):
     c_loss, c_dz = c_oracle.gae_loss_grad(z.detach().numpy(), L.indptr, L.indices, norm, pw)
     assert abs(c_loss - loss.item()) < 1e-5 * abs(loss.item())
     assert np.linalg.norm(c_dz - z.grad.numpy()) / np.linalg.norm(z.grad.numpy()) < 1e-4      # torch side is fp32
+
+
+def test_scgnn_step_restatement_matches_port_autograd():
+    """oracle/scgnn_step_ref.py (the fp64 arbiter of the engines' training steps, whose Graph-AE decoder term is the row-chunked
+    closed form injected at z) against plain autograd through oracle.port: the Feature-AE loss in the noregu, LTMG with the
+    all-zero TRS and LTMG with a random TRS forms, and the Graph-AE loss over the dense n² logits, with and without noise."""
+    from oracle import scgnn_step_ref as R
+    n, g = 200, 48
+    X = torch.from_numpy(port.synthetic_expression(n, g, density=0.3, seed=8)).double()
+    torch.manual_seed(0)
+    fae = port.FeatureAE(g).double()
+    params = dict(fae.named_parameters())
+    trs = torch.rand(n, g, generator=torch.Generator().manual_seed(1), dtype=torch.float64)
+    for reg, ltmg in (("noregu", None), ("LTMG", None), ("LTMG", trs)):
+        fae.zero_grad()
+        z, r = fae(X)
+        loss = port.feature_ae_loss(r, X, reg, 0.9, torch.zeros_like(X) if ltmg is None else ltmg)
+        loss.backward()
+        out = R.feature_ae_step(X, params, reg, 0.9, ltmg)
+        assert abs(out["loss"].item() - loss.item()) <= 1e-12 * loss.item(), reg
+        assert rel_err(out["z"], z) < 1e-12 and rel_err(out["recon"], r) < 1e-12
+        for k in R.FEATURE_AE_PARAMS:
+            assert rel_err(out["grads"][k], params[k].grad) < 1e-12, (reg, k)
+
+    emb = np.abs(port.synthetic_embedding(n, d=g, seed=3)) * 0.1
+    adj, _ = port.feature2adj(emb, 6)
+    an = port.preprocess_graph(adj)
+    lab = (adj + sp.eye(n)).tocsr()
+    lab.sort_indices()
+    pw, norm = port.gae_norm_constants(adj)
+    A = torch.sparse_coo_tensor(torch.from_numpy(np.vstack(an.nonzero())), torch.from_numpy(an.data.astype(np.float64)), (n, n),
+                                check_invariants=True)
+    gen = torch.Generator().manual_seed(2)
+    weights = {"gc1.weight": torch.randn(g, 32, generator=gen, dtype=torch.float64) * 0.3,
+               "gc2.weight": torch.randn(32, 16, generator=gen, dtype=torch.float64) * 0.3,
+               "gc3.weight": torch.randn(32, 16, generator=gen, dtype=torch.float64) * 0.3}
+    x = torch.from_numpy(emb).double()
+    t = lambda a: torch.from_numpy(np.asarray(a))
+    for eps in (torch.randn(n, 16, generator=gen, dtype=torch.float64), torch.zeros(n, 16, dtype=torch.float64)):
+        w = [weights[k].clone().requires_grad_() for k in ("gc1.weight", "gc2.weight", "gc3.weight")]
+        z, mu, lv, _ = port.graph_ae_gcn_forward(x, *w, A, eps)
+        for v in (z, mu, lv):
+            v.retain_grad()
+        loss = port.gae_loss(z @ z.t(), torch.from_numpy(lab.toarray()), mu, lv, n, norm, pw)
+        loss.backward()
+        out = R.graph_ae_step(x, t(an.indptr), t(an.indices), t(an.data), t(lab.indptr), t(lab.indices), norm, pw, weights, eps)
+        assert abs(out["loss"] - loss.item()) <= 1e-11 * abs(loss.item())   # n² terms summed in another order and form
+        for key, ref in (("z", z), ("mu", mu), ("logvar", lv), ("dz", z.grad), ("dmu", mu.grad), ("dlogvar", lv.grad)):
+            assert rel_err(out[key], ref) < 1e-12, key
+        for k, wk in zip(("gc1.weight", "gc2.weight", "gc3.weight"), w):
+            assert rel_err(out["grads"][k], wk.grad) < 1e-12, k
+    # with eps = 0 the logvar gradient is the KLD term alone: 2·(exp(lv)² − 1) / (2·n²) per element
+    assert rel_err(out["dlogvar"], (torch.exp(out["logvar"])**2 - 1) / n**2) < 1e-12

@@ -6,8 +6,14 @@
 //   G  = σ(S), loss       SFU math on the accumulator registers (e = 2^(−|x|·log2e), r = 1/(1+e), one lg2 per 32 logits)
 //   dZ_I += G · Z_J       wgmma m64nDk8 tf32 with A = G taken straight from the registers (hi / lo split of G and Z_J, three
 //                          products) and B = Z_Jᵀ from shared memory
-// A producer warp copies the pre-split J tiles into a two-stage ring with 1-D bulk copies (the tiles are laid out in global
-// memory exactly as wgmma reads them: K-major, 128-byte swizzle).
+// A producer warpgroup (one thread of it) copies the pre-split J tiles into a three-stage ring with 1-D bulk copies (the tiles
+// are laid out in global memory exactly as wgmma reads them: K-major, 128-byte swizzle).
+//
+// Schedule: each product is issued as one batch of wgmmas with one commit and one wait (S: 3·DP/8, dZ: 3·16), which needs S,
+// both halves of G and the dZ accumulators live in registers at once; the producer warpgroup gives its registers to the
+// consumers (setmaxnreg) to make room.  The two consumer warpgroups run out of phase ("ping-pong"): while one does σ / softplus
+// on the SFU, the other's products run on the tensor cores.  Tiles with no masked logit take an elementwise loop without the
+// per-logit mask.
 //
 // Register fragment trick: the accumulator of S gives a thread columns (2t, 2t+1) of each 8-column block, the tf32 A fragment
 // wants columns (t, t+4).  The sum over j does not care about order, so the 8 columns of each block are fed to the second
@@ -28,8 +34,11 @@ using namespace tc;
 
 constexpr int BT = 128;                 // rows per block / tile
 constexpr int CONSUMERS = 256;          // two warpgroups
-constexpr int THREADS = CONSUMERS + 32; // + producer warp
-constexpr int STAGES = 2;
+constexpr int THREADS = CONSUMERS + 128; // + producer warpgroup
+// Register split (setmaxnreg): the consumers hold S, both halves of G and the dZ accumulators while a dZ batch is in flight.
+// 128 · 40 + 256 · 232 = 64 512 of the 65 536 registers of an SM.
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+constexpr int STAGES = 3;               // DP = 32: 32 KB + 3 x 64 KB, just inside the 227 KB a CTA may have
 constexpr int MAX_D = 32;
 constexpr uint32_t ZS_BYTES = BT * 128; // one plane of a tile for S (K-major, 128-byte rows)
 constexpr int ZS_PLANES = 2;            // hi, lo
@@ -90,6 +99,38 @@ __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
+// σ and softplus of one thread's 64 logits S (the m64n128 accumulator), in place: S becomes the hi part of G = σ(S) and L its
+// lo part, ready to be the register A operand of the dZ product.  Returns the thread's share of Σ softplus.  MASKED zeroes G
+// and drops the loss of columns j ≥ n and of rows past the range (the last J tile, a partial I block); interior tiles skip the
+// per-logit mask and its selects.
+template <bool MASKED>
+__device__ __forceinline__ float sigmoid_softplus(float (&S)[BT / 2], float (&L)[BT / 2], int jbase, int n, bool live_a, bool live_b) {
+  constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
+  float relu = 0.f, lg = 0.f, prod = 1.f;
+#pragma unroll
+  for (int v = 0; v < BT / 2; ++v) {
+    if ((v & 31) == 31) { lg += lg2_approx(prod); prod = 1.f; }
+    const float x = S[v];
+    const float e = ex2_approx(-fabsf(x) * LOG2E);
+    const float inv = rcp_approx(1.f + e);
+    float sg = x >= 0.f ? inv : e * inv;
+    if constexpr (MASKED) {
+      const int j = jbase + 8 * (v >> 2) + (v & 1);
+      const bool ok = j < n && (((v >> 1) & 1) ? live_b : live_a);
+      relu += ok ? fmaxf(x, 0.f) : 0.f;
+      prod *= ok ? 1.f + e : 1.f;
+      sg = ok ? sg : 0.f;
+    } else {
+      relu += fmaxf(x, 0.f);
+      prod *= 1.f + e;
+    }
+    const float hi = tf32_trunc(sg);
+    S[v] = hi;
+    L[v] = sg - hi;
+  }
+  return relu + LN2 * (lg + lg2_approx(prod));
+}
+
 template <int DP>
 __global__ void __launch_bounds__(THREADS, 1)
 gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
@@ -125,7 +166,9 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
   __syncthreads();
 
   if (tid >= CONSUMERS) {
-    // ===================== producer warp =====================
+    // ===================== producer warpgroup =====================
+    // One thread issues the copies; the warpgroup exists so that it can hand its registers to the consumers.
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
     if (tid == CONSUMERS) {
       for (int i = 0; i < nt; ++i) {
         const int s = i % STAGES;
@@ -143,6 +186,7 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
   }
 
   // ===================== consumers =====================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
   // Z_I planes from z (rows past the range are zero: their logits are masked below)
   for (int e = tid; e < BT * DP; e += CONSUMERS) {
     const int r = e / DP, k = e % DP;
@@ -160,7 +204,7 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
   const int ra = row0 + wg * 64 + warp * 16 + (lane >> 2);       // rows of this thread: ra, ra + 8
   const bool live_a = ra < row_end, live_b = ra + 8 < row_end;
   const uint32_t ai_hi = smem_u32(zi_hi) + wg * 64 * 128, ai_lo = smem_u32(zi_lo) + wg * 64 * 128;
-  constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
+  const bool full_rows = row0 + BT <= row_end;                   // no dead rows in this block: only the last J tile is masked
 
   // The accumulation inside the tensor core truncates, and the hi·hi product carries almost all of dZ: over a whole J sweep one
   // accumulator would drift by ~1e-5 relative (~6e-5 for |z| ~ 1e5).  So the hi·hi products of a tile go round-robin into NB
@@ -172,12 +216,20 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
   for (int v = 0; v < DP / 2; ++v) dzt[v] = 0.f;
   double loss = 0.0;
 
-  for (int i = 0; i < nt; ++i) {
+  // Ping-pong: the two warpgroups take turns on the tensor cores.  A turn is the dZ product of the previous tile followed by the
+  // S product of the next one, each issued as one batch with one commit and one wait.  The turn passes on once both are done
+  // (named barrier 2 + wg means "wg may issue"), and the warpgroup works through σ / softplus of its S while the other one's
+  // products run.  Warpgroup 0 takes the first turn.  Each warpgroup takes nt + 1 turns and passes nt of them on; warpgroup 0
+  // passes its last one as well, so that every bar.arrive meets one bar.sync.
+  float S[BT / 2], L[BT / 2];   // S: accumulator of S, then the hi part of G; L: the lo part of G
+  auto take_turn = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(2 + wg), "n"(CONSUMERS) : "memory"); };
+  auto pass_turn = [&]() { asm volatile("bar.arrive %0, %1;" ::"r"(3 - wg), "n"(CONSUMERS) : "memory"); };
+
+  // S = Z_I · Z_Jᵀ of tile i: one batch of 3·DP/8 products, committed (the caller waits)
+  auto issue_s = [&](int i) {
     const int s = i % STAGES;
     mbar_wait(full_bar + 8 * s, (uint32_t)((i / STAGES) & 1));
-    const uint32_t st = smem_u32(ring + s * STAGE);
-    const uint32_t bs_hi = st, bs_lo = st + ZS_BYTES, bt_hi = st + 2 * ZS_BYTES, bt_lo = bt_hi + ZT;
-    float S[BT / 2];
+    const uint32_t bs_hi = smem_u32(ring + s * STAGE), bs_lo = bs_hi + ZS_BYTES;
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < DP / 8; ++kk) {
@@ -187,38 +239,18 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
       wgmma_tf32_ss_n128(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_hi + o), 1);
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(S);
-
-    // ---- σ and softplus on the registers ----
-    const int jbase = (jt0 + i) * BT + 2 * (lane & 3);
-    float relu = 0.f, lg = 0.f, prod = 1.f;
-#pragma unroll
-    for (int v = 0; v < BT / 2; ++v) {
-      if ((v & 31) == 31) { lg += lg2_approx(prod); prod = 1.f; }
-      const int j = jbase + 8 * (v >> 2) + (v & 1);
-      const bool ok = j < p.n && (((v >> 1) & 1) ? live_b : live_a);
-      const float x = S[v];
-      const float e = ex2_approx(-fabsf(x) * LOG2E);
-      const float inv = rcp_approx(1.f + e);
-      const float sg = x >= 0.f ? inv : e * inv;
-      relu += ok ? fmaxf(x, 0.f) : 0.f;
-      prod *= ok ? 1.f + e : 1.f;
-      S[v] = ok ? sg : 0.f;
-    }
-    loss += (double)(relu + LN2 * (lg + lg2_approx(prod)));
-
-    // ---- dZ_I += G · Z_J ----
+  };
+  // dZ_I += G · Z_J of tile i: one batch of 3·16 products with A = (S, L) from the registers, waited for (S is overwritten next)
+  auto run_dz = [&](int i) {
+    const uint32_t bt_hi = smem_u32(ring + (i % STAGES) * STAGE) + 2 * ZS_BYTES, bt_lo = bt_hi + ZT;
     wgmma_fence();
 #pragma unroll
     for (int kb = 0; kb < BT / 8; ++kb) {
-      const float g[4] = {S[4 * kb], S[4 * kb + 2], S[4 * kb + 1], S[4 * kb + 3]};   // (r, 2t) (r+8, 2t) (r, 2t+1) (r+8, 2t+1)
-      uint32_t ahi[4], alo[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        ahi[q] = __float_as_uint(g[q]) & 0xFFFFE000u;
-        alo[q] = __float_as_uint(g[q] - __uint_as_float(ahi[q]));
-      }
+      // A fragment (r, t) (r+8, t) (r, t+4) (r+8, t+4) in the permuted column order: (r, 2t) (r+8, 2t) (r, 2t+1) (r+8, 2t+1)
+      const uint32_t ahi[4] = {__float_as_uint(S[4 * kb]), __float_as_uint(S[4 * kb + 2]), __float_as_uint(S[4 * kb + 1]),
+                               __float_as_uint(S[4 * kb + 3])};
+      const uint32_t alo[4] = {__float_as_uint(L[4 * kb]), __float_as_uint(L[4 * kb + 2]), __float_as_uint(L[4 * kb + 1]),
+                               __float_as_uint(L[4 * kb + 3])};
       const uint32_t o = (uint32_t)(kb >> 2) * (DP * 128) + (uint32_t)(kb & 3) * 32;
       mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
       mma_rs<DP>(dzs, ahi, wgmma_desc_sw128(bt_lo + o), 1);
@@ -229,6 +261,9 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
 #pragma unroll
     for (int b = 0; b < NB; ++b) reg_fence(dzb[b]);
     reg_fence(dzs);
+  };
+  // the tile's dZ joins the fp32 total, and its stage goes back to the producer
+  auto retire_dz = [&](int i) {
 #pragma unroll
     for (int v = 0; v < DP / 2; ++v) {
       float t = dzs[v];
@@ -237,8 +272,33 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
       dzt[v] += t;
     }
     __syncwarp();
-    if (lane == 0) mbar_arrive(empty_bar + 8 * s);
+    if (lane == 0) mbar_arrive(empty_bar + 8 * (i % STAGES));
+  };
+  // wait for S of tile i, pass the turn on, then σ / softplus on the registers
+  auto elementwise = [&](int i) {
+    wgmma_wait<0>();
+    reg_fence(S);
+    pass_turn();
+    const int jbase = (jt0 + i) * BT + 2 * (lane & 3);
+    const float l = full_rows && (jt0 + i + 1) * BT <= p.n ? sigmoid_softplus<false>(S, L, jbase, p.n, live_a, live_b)
+                                                           : sigmoid_softplus<true>(S, L, jbase, p.n, live_a, live_b);
+    loss += (double)l;
+  };
+
+  if (wg == 1) take_turn();
+  issue_s(0);
+  elementwise(0);
+  for (int i = 1; i < nt; ++i) {
+    take_turn();
+    run_dz(i - 1);
+    issue_s(i);          // S runs while the previous tile's dZ is summed
+    retire_dz(i - 1);
+    elementwise(i);
   }
+  take_turn();
+  run_dz(nt - 1);
+  retire_dz(nt - 1);
+  if (wg == 0) pass_turn();
 
   // ---- epilogue ----
   const float c2 = 2.f * p.coef;

@@ -5,12 +5,13 @@ config 4, scGNN 1 M × 2 000 — is bench.py).  Device-event timed on synthetic 
             per-epoch train / validation evaluation the reference performs)
   config 2  scGNN 100 k × 2 k, k = 15: `python bench.py --cells 100000` (same step as the headline)
   config 3  GraphSCI, N cells × 3 000 genes (default N = 500 000): one training epoch of GraphSCI.train (AE + gene-graph GNN, ZINB
-            loss).  The GEMMs run in single-pass TF32 (`precision="tf32"`, at least bf16's 8-bit mantissa), the aggregate has the
-            bf16-operand kernel available; there is no bf16 GEMM mode — dtype is reported as what ran
+            loss).  The GEMMs run in the precision BASELINE names, bf16 (`--precision3 bf16`, the default: operands rounded to
+            bfloat16 in the kernel, fp32 accumulate and fp32 tensors); `--precision3 tf32` gives the earlier single-pass TF32
+            line, `tf32x3` the fp32-accurate one.  dtype is reported as what ran
   config 5  SpaGCN: the reference model multiplies a DENSE N × N adjacency (spagcn.py:357-363); 200 k spots would need a 160 GB
             matrix, so the line is measured at --spots (default 20 000) on one GPU and says so
 
-    python benchmarks/configs.py --only 1,3 [--cells3 500000]
+    python benchmarks/configs.py --only 1,3 [--cells3 500000] [--precision3 bf16|tf32|tf32x3]
 """
 from __future__ import annotations
 
@@ -76,7 +77,7 @@ def config3(args):
     graph = sample.data.uns["FeatureFeatureGraph"]
     graph.ndata["feat"] = X.t().contiguous()       # node features of the gene graph = (log-)expression of ALL cells ([G, N], graphsci.py:126)
     del sample
-    model = GraphSCI(num_cells=N, num_genes=G, dataset="synthetic", dropout=0.1, gpu=0, seed=0, precision="tf32")
+    model = GraphSCI(num_cells=N, num_genes=G, dataset="synthetic", dropout=0.1, gpu=0, seed=0, precision=args.precision3)
     model._bind_graph(graph)
     n_counts = Xraw.sum(1)
     model.size_factors = (n_counts / torch.median(n_counts)).contiguous()      # what fit() sets up (graphsci.py:270-276)
@@ -95,8 +96,15 @@ def config3(args):
     ms = s.elapsed_time(e) / epochs
     return {"config": 3, "workload": f"GraphSCI {N} cells × {G} genes: one training epoch (AE + gene-graph GNN, ZINB + adjacency losses)",
             "metric": "cells/sec per training epoch", "value": N / (ms / 1e3), "unit": "cells/s", "ms_per_epoch": ms,
-            "dtype": "tf32 single-pass GEMMs (no bf16 GEMM mode is built; the aggregate's bf16-operand kernel is available)", "n_gpus": 1,
+            "dtype": DTYPE3[args.precision3], "n_gpus": 1,
             "data": "synthetic", "gene_graph_edges": int(graph.num_edges())}
+
+
+DTYPE3 = {
+    "bf16": "bf16 GEMMs (operands rounded to bfloat16 in the kernel, fp32 accumulate; fp32 tensors and epilogue)",
+    "tf32": "tf32 single-pass GEMMs",
+    "tf32x3": "f32 (tf32x3 GEMMs)",
+}
 
 
 def config5(args):
@@ -136,6 +144,7 @@ def main():
     ap.add_argument("--only", type=str, default="1,3,5")
     ap.add_argument("--cells3", type=int, default=500_000)
     ap.add_argument("--spots", type=int, default=20_000)
+    ap.add_argument("--precision3", choices=sorted(DTYPE3), default="bf16", help="GEMM precision of config 3")
     args = ap.parse_args()
     fns = {"1": config1, "3": config3, "5": config5}
     for k in args.only.split(","):

@@ -1,4 +1,4 @@
-// b2_gemm_f32 dispatcher: tensor-core wgmma (TF32 / 3xTF32) kernel when the shape qualifies,
+// b2_gemm_f32 dispatcher: tensor-core wgmma (TF32 / 3xTF32 / BF16) kernel when the shape qualifies,
 // CUDA-core fp32 kernel otherwise (or when B2_PREC_FP32_SIMT is requested).
 #include "common.cuh"
 
@@ -28,7 +28,8 @@ extern "C" int b2_gemm_f32(const float* A, int64_t lda, int transA, const float*
   B2_REQUIRE(M >= 0 && N >= 0 && K >= 0, "b2_gemm_f32: negative shape");
   B2_REQUIRE(lda >= (transA ? M : K) && ldb >= (transB ? K : N) && ldc >= N, "b2_gemm_f32: leading dimension too small");
   B2_REQUIRE(!mask || ldmask >= N, "b2_gemm_f32: ldmask too small");
-  B2_REQUIRE(precision == B2_PREC_FP32_SIMT || precision == B2_PREC_TF32X3 || precision == B2_PREC_TF32,
+  B2_REQUIRE(precision == B2_PREC_FP32_SIMT || precision == B2_PREC_TF32X3 || precision == B2_PREC_TF32 ||
+                 precision == B2_PREC_BF16,
              "b2_gemm_f32: unknown precision %d", precision);
   B2_REQUIRE(beta == 0.f || beta == 1.f, "b2_gemm_f32: beta must be 0 or 1");
   if (M == 0 || N == 0) return B2_OK;

@@ -2,20 +2,25 @@
 //   C[M,N] = epilogue( op(A)[M,K] · op(B)[K,N] )
 // Hopper structure: one CTA per 128 x BN output tile (and K split), two consumer warpgroups of 64 rows each.  TMA
 // (cp.async.bulk.tensor) stages the raw fp32 operand tiles of each 32-wide k-block into a ring; all 256 threads then rewrite the
-// stage as K-major, 128B-swizzled tf32 planes (wgmma reads tf32 operands only K-major, so this one pass also serves the
-// transposed layouts: nothing is transposed in global memory) and issue wgmma.mma_async m64nBNk8 with fp32 accumulators in
-// registers.  The rewrite of k-block i+1 overlaps the asynchronous MMAs of k-block i (two plane buffers); the epilogue applies
-// bias / activation / ReLU-mask / accumulate straight from the accumulator registers.
+// stage as K-major swizzled planes (wgmma reads tf32 operands only K-major, so this one pass also serves the transposed layouts:
+// nothing is transposed in global memory) and issue wgmma.mma_async with fp32 accumulators in registers.  The rewrite of k-block
+// i+1 overlaps the asynchronous MMAs of k-block i (two plane buffers); the epilogue applies bias / activation / ReLU-mask /
+// accumulate straight from the accumulator registers.
 //
-// Precision modes
-//   TF32   : one wgmma per k-step (tf32 operands: 10-bit mantissa)
+// Precision modes (a bound on how the operands are rounded; accumulation, inputs, outputs and the epilogue are fp32 in all)
+//   TF32   : 128B-swizzled tf32 planes, one m64nBNk8 wgmma per k-step (tf32 operands: 10-bit mantissa, low bits ignored)
 //   TF32X3 : fp32-accurate. The rewrite also splits each value into hi = x & 0xFFFFE000 (exactly representable in tf32) and
 //            lo = x - hi, and the MMAs accumulate lo·hi + hi·lo into one accumulator and hi·hi into another, summed in the
 //            epilogue (error ~2^-21 relative).
+//   BF16   : the rewrite rounds each operand to bfloat16 (round-to-nearest-even, cvt.rn.bf16x2.f32: subnormals kept, as
+//            torch's .to(torch.bfloat16)) into 64B-swizzled planes (a 32-wide k-block is a 64-byte row), one m64nBNk16
+//            .f32.bf16.bf16 wgmma per 16 k.  Same k-block, ring, split-K plan and workspace as TF32.
+// Shapes the tensor-core kernel does not take (see gemm_tc's qualification) run on the CUDA-core fp32 kernel in every mode.
 //
 // Replaces torch.mm / nn.Linear on the reference path (scgnn2.py:352-370, 499).
 #include "tc_common.cuh"
 
+#include <cuda_bf16.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -23,11 +28,13 @@ namespace b2 {
 namespace tc {
 
 constexpr int BM = 128;            // two warpgroups x 64 rows
-constexpr int BK = 32;             // k-block: 32 tf32 = 128 B = one swizzle span
-constexpr int UK = 8;              // wgmma K for tf32
+constexpr int BK = 32;             // k-block: 32 tf32 = 128 B = one 128B swizzle span (32 bf16 = 64 B = one 64B span)
 constexpr int THREADS = 256;
 constexpr int MAX_STAGES = 4;
 constexpr int SMEM_LIMIT = 227 * 1024;
+
+enum Mode { MODE_TF32 = 0, MODE_TF32X3 = 1, MODE_BF16 = 2 };
+__host__ __device__ constexpr int plane_row_bytes(int mode) { return mode == MODE_BF16 ? BK * 2 : BK * 4; }
 
 struct Params {
   CUtensorMap tmA;
@@ -39,31 +46,34 @@ struct Params {
   long long ldc, ldmask;
   int M, N, K;
   int a_mn, b_mn;          // raw tile layout: 0 = K contiguous, 1 = M / N contiguous
-  int x3;                  // 3xTF32 split
+  int mode;                // Mode
   int act;
   float beta;
   int tiles_m, tiles_n, splits, kb_per_split, kb_total, stages;
 };
 
 // shared memory: [2 plane buffers: A hi | A lo | B hi | B lo] [ring: stages x (A raw | B raw)] [barriers]
+// (A lo / B lo only in TF32X3; BF16 planes are half the size of tf32 ones, the raw fp32 stage is the same in every mode)
 struct SmemLayout {
   uint32_t a_plane, b_plane, plane_buf, raw_a, raw_stage, ring, bars, total;
 };
-__host__ __device__ inline SmemLayout smem_layout(int BN, int x3, int stages) {
+__host__ __device__ inline SmemLayout smem_layout(int BN, int mode, int stages) {
   SmemLayout L;
-  L.a_plane = BM * BK * 4;
-  L.b_plane = (uint32_t)BN * BK * 4;
-  L.plane_buf = (x3 ? 2u : 1u) * (L.a_plane + L.b_plane);
+  L.a_plane = BM * plane_row_bytes(mode);
+  L.b_plane = (uint32_t)BN * plane_row_bytes(mode);
+  L.plane_buf = (mode == MODE_TF32X3 ? 2u : 1u) * (L.a_plane + L.b_plane);
   L.raw_a = BM * BK * 4;
-  L.raw_stage = L.raw_a + L.b_plane;
+  L.raw_stage = L.raw_a + (uint32_t)BN * BK * 4;
   L.ring = 2 * L.plane_buf;
   L.bars = L.ring + (uint32_t)stages * L.raw_stage;
   L.total = L.bars + 8 * MAX_STAGES;
   return L;
 }
 
-// raw tile (rows x 32 k, K-contiguous [row][k] or row-contiguous [k][row]) → K-major swizzled tf32 plane(s)
-__device__ __forceinline__ void convert_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int rows, int mn, int x3, int tid) {
+// raw tile (rows x 32 k, K-contiguous [row][k] or row-contiguous [k][row]) → K-major swizzled plane(s): tf32 (128B swizzle) or
+// bf16 rounded to nearest even (64B swizzle)
+template <int MODE>
+__device__ __forceinline__ void convert_tile(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int rows, int mn, int tid) {
   for (int c = tid; c < rows * (BK / 4); c += THREADS) {
     int r, kc;
     float4 v;
@@ -75,8 +85,14 @@ __device__ __forceinline__ void convert_tile(const uint8_t* raw, uint8_t* hi, ui
       const float* col = reinterpret_cast<const float*>(raw) + r;
       v = make_float4(col[(kc * 4 + 0) * rows], col[(kc * 4 + 1) * rows], col[(kc * 4 + 2) * rows], col[(kc * 4 + 3) * rows]);
     }
+    if constexpr (MODE == MODE_BF16) {
+      const __nv_bfloat162 p0 = __floats2bfloat162_rn(v.x, v.y), p1 = __floats2bfloat162_rn(v.z, v.w);   // .x at the lower address
+      *reinterpret_cast<uint2*>(hi + sw64_offset16((uint32_t)r, (uint32_t)kc * 4)) =
+          make_uint2(*reinterpret_cast<const uint32_t*>(&p0), *reinterpret_cast<const uint32_t*>(&p1));
+      continue;
+    }
     const uint32_t off = sw128_offset32((uint32_t)r, (uint32_t)kc * 4);
-    if (x3) {
+    if constexpr (MODE == MODE_TF32X3) {
       const float4 h = make_float4(__uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u), __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u),
                                    __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u), __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u));
       *reinterpret_cast<float4*>(hi + off) = h;
@@ -93,14 +109,20 @@ __device__ __forceinline__ void mma_ss(float (&d)[BN / 2], uint64_t a, uint64_t 
   else if constexpr (BN == 64) wgmma_tf32_ss_n64(d, a, b, scale_d);
   else wgmma_tf32_ss_n128(d, a, b, scale_d);
 }
+template <int BN>
+__device__ __forceinline__ void mma_bf16_ss(float (&d)[BN / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
+  if constexpr (BN == 32) wgmma_bf16_ss_n32(d, a, b, scale_d);
+  else if constexpr (BN == 64) wgmma_bf16_ss_n64(d, a, b, scale_d);
+  else wgmma_bf16_ss_n128(d, a, b, scale_d);
+}
 
-template <int BN, bool X3>
+template <int BN, int MODE>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // 1024-byte alignment is required by the 128B swizzle atoms
+  // 1024-byte alignment is required by the 128B swizzle atoms (the 64B ones need 512)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const SmemLayout L = smem_layout(BN, p.x3, p.stages);
+  const SmemLayout L = smem_layout(BN, MODE, p.stages);
   const uint32_t full_bar = smem_u32(smem + L.bars);
   const int tid = threadIdx.x, wg = tid >> 7, lt = tid & 127;
 
@@ -132,34 +154,47 @@ gemm_tc_kernel(const __grid_constant__ Params p) {
     for (int i = 0; i < min(nk, p.stages); ++i) issue(i);
 
   float acc[BN / 2], acc_s[BN / 2];     // hi·hi and the two cross terms (3xTF32)
+  // BF16: the first MMA overwrites acc (scale_d = 0) instead of adding to zeros written here; ptxas serialises the wgmmas of a
+  // kernel (C7515) whose accumulators are also defined by ordinary instructions
 #pragma unroll
-  for (int j = 0; j < BN / 2; ++j) { acc[j] = 0.f; acc_s[j] = 0.f; }
+  for (int j = 0; j < BN / 2; ++j) {
+    if constexpr (MODE != MODE_BF16) acc[j] = 0.f;
+    acc_s[j] = 0.f;
+  }
 
   for (int i = 0; i < nk; ++i) {
     const int s = i % p.stages;
     uint8_t* planes = smem + (i & 1) * L.plane_buf;
     uint8_t* a_hi = planes;
     uint8_t* a_lo = planes + L.a_plane;
-    uint8_t* b_hi = planes + (p.x3 ? 2 : 1) * L.a_plane;
+    uint8_t* b_hi = planes + (MODE == MODE_TF32X3 ? 2 : 1) * L.a_plane;
     uint8_t* b_lo = b_hi + L.b_plane;
     mbar_wait(full_bar + 8 * s, (uint32_t)((i / p.stages) & 1));
     const uint8_t* raw = smem + L.ring + s * L.raw_stage;
-    convert_tile(raw, a_hi, a_lo, BM, p.a_mn, p.x3, tid);
-    convert_tile(raw + L.raw_a, b_hi, b_lo, BN, p.b_mn, p.x3, tid);
+    convert_tile<MODE>(raw, a_hi, a_lo, BM, p.a_mn, tid);
+    convert_tile<MODE>(raw + L.raw_a, b_hi, b_lo, BN, p.b_mn, tid);
     fence_proxy_async();                       // generic-proxy plane writes → visible to the tensor core (async proxy)
     __syncthreads();                           // planes complete; the raw stage is free again
     if (tid == 0 && i + p.stages < nk) issue(i + p.stages);
     wgmma_fence();
-    const uint32_t ah = smem_u32(a_hi) + wg * 64 * 128, al = smem_u32(a_lo) + wg * 64 * 128;
+    const uint32_t ah = smem_u32(a_hi) + wg * 64 * plane_row_bytes(MODE), al = smem_u32(a_lo) + wg * 64 * plane_row_bytes(MODE);
     const uint32_t bh = smem_u32(b_hi), bl = smem_u32(b_lo);
+    if constexpr (MODE == MODE_BF16) {
 #pragma unroll
-    for (int k = 0; k < BK / UK; ++k) {
-      const uint32_t ko = k * UK * 4;
-      if (X3) {
-        mma_ss<BN>(acc_s, wgmma_desc_sw128(al + ko), wgmma_desc_sw128(bh + ko), 1);
-        mma_ss<BN>(acc_s, wgmma_desc_sw128(ah + ko), wgmma_desc_sw128(bl + ko), 1);
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint32_t ko = k * 16 * 2;
+        mma_bf16_ss<BN>(acc, wgmma_desc_sw64(ah + ko), wgmma_desc_sw64(bh + ko), (i | k) != 0);
       }
-      mma_ss<BN>(acc, wgmma_desc_sw128(ah + ko), wgmma_desc_sw128(bh + ko), 1);
+    } else {
+#pragma unroll
+      for (int k = 0; k < BK / 8; ++k) {
+        const uint32_t ko = k * 8 * 4;
+        if constexpr (MODE == MODE_TF32X3) {
+          mma_ss<BN>(acc_s, wgmma_desc_sw128(al + ko), wgmma_desc_sw128(bh + ko), 1);
+          mma_ss<BN>(acc_s, wgmma_desc_sw128(ah + ko), wgmma_desc_sw128(bl + ko), 1);
+        }
+        mma_ss<BN>(acc, wgmma_desc_sw128(ah + ko), wgmma_desc_sw128(bh + ko), 1);
+      }
     }
     wgmma_commit();
     wgmma_wait<1>();                           // the MMAs of k-block i-1 are done: their plane buffer may be rewritten
@@ -273,17 +308,17 @@ struct Plan {
   size_t smem;
 };
 
-static Plan make_plan(int M, int N, int K, int x3) {
+static Plan make_plan(int M, int N, int K, int mode) {
   Plan pl;
   pl.BN = N <= 32 ? 32 : (N <= 64 ? 64 : 128);
-  const SmemLayout L0 = smem_layout(pl.BN, x3, 0);
+  const SmemLayout L0 = smem_layout(pl.BN, mode, 0);
   int stages = (int)((SMEM_LIMIT - 1024 - L0.total) / L0.raw_stage);
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   pl.stages = stages;               // ≥ 2 for every BN (128 KB of planes + 2 x 32 KB raw stages at BN = 128, 3xTF32)
-  pl.smem = (size_t)smem_layout(pl.BN, x3, stages).total + 1024 /*align slack*/;
+  pl.smem = (size_t)smem_layout(pl.BN, mode, stages).total + 1024 /*align slack*/;
   pl.tiles_m = ceil_div(M, BM);
   pl.tiles_n = ceil_div(N, pl.BN);
-  pl.kb_total = ceil_div(K, BK);
+  pl.kb_total = ceil_div(K, BK);     // the k-block, and so the split-K plan and its workspace, is the same in every mode
   const int tiles = pl.tiles_m * pl.tiles_n;
   const int sms = sm_count();
   int splits = 1;
@@ -298,23 +333,32 @@ static Plan make_plan(int M, int N, int K, int x3) {
   return pl;
 }
 
-template <int BN, bool X3>
+template <int BN, int MODE>
 static int launch_gemm(const Params& p, const Plan& pl, cudaStream_t st) {
   static bool attr_set = false;
   if (!attr_set) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    B2_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
     attr_set = true;
   }
-  gemm_tc_kernel<BN, X3><<<pl.tiles_m * pl.tiles_n * pl.splits, THREADS, pl.smem, st>>>(p);
+  gemm_tc_kernel<BN, MODE><<<pl.tiles_m * pl.tiles_n * pl.splits, THREADS, pl.smem, st>>>(p);
   B2_CHECK_LAUNCH("gemm_tc_kernel");
   return B2_OK;
+}
+
+template <int MODE>
+static int launch_gemm_mode(const Params& p, const Plan& pl, cudaStream_t st) {
+  return pl.BN == 32 ? launch_gemm<32, MODE>(p, pl, st) : (pl.BN == 64 ? launch_gemm<64, MODE>(p, pl, st) : launch_gemm<128, MODE>(p, pl, st));
+}
+
+static int mode_of(int precision) {
+  return precision == B2_PREC_TF32X3 ? MODE_TF32X3 : (precision == B2_PREC_BF16 ? MODE_BF16 : MODE_TF32);
 }
 
 }  // namespace tc
 
 size_t gemm_tc_workspace_bytes(int M, int N, int K, int transA, int transB, int precision) {
   if (M <= 0 || N <= 0 || K <= 0) return 0;
-  const tc::Plan pl = tc::make_plan(M, N, K, precision == B2_PREC_TF32X3);
+  const tc::Plan pl = tc::make_plan(M, N, K, tc::mode_of(precision));
   return pl.splits > 1 ? (size_t)pl.splits * M * N * sizeof(float) : 0;
 }
 
@@ -328,8 +372,8 @@ int gemm_tc(const float* A, int64_t lda, int transA, const float* B, int64_t ldb
     return B2_ERR_UNSUPPORTED;
   if (!get_encode()) return B2_ERR_UNSUPPORTED;
 
-  const int x3 = precision == B2_PREC_TF32X3;
-  const Plan pl = make_plan(M, N, K, x3);
+  const int mode = mode_of(precision);
+  const Plan pl = make_plan(M, N, K, mode);
   Params p;
   memset(&p, 0, sizeof(p));
   // raw tiles, unswizzled: A is [M,K] row-major (box 32 k x 128 rows) or stored [K,M] (box 128 rows x 32 k); B likewise
@@ -343,7 +387,7 @@ int gemm_tc(const float* A, int64_t lda, int transA, const float* B, int64_t ldb
   p.M = M; p.N = N; p.K = K;
   p.a_mn = transA ? 1 : 0;
   p.b_mn = transB ? 0 : 1;
-  p.x3 = x3; p.act = act; p.beta = beta;
+  p.mode = mode; p.act = act; p.beta = beta;
   p.tiles_m = pl.tiles_m; p.tiles_n = pl.tiles_n; p.splits = pl.splits; p.kb_per_split = pl.kb_per_split;
   p.kb_total = pl.kb_total; p.stages = pl.stages;
   p.partial = nullptr;
@@ -355,8 +399,8 @@ int gemm_tc(const float* A, int64_t lda, int transA, const float* B, int64_t ldb
     }
     p.partial = reinterpret_cast<float*>(workspace);
   }
-  const int rc = x3 ? (pl.BN == 32 ? launch_gemm<32, true>(p, pl, st) : (pl.BN == 64 ? launch_gemm<64, true>(p, pl, st) : launch_gemm<128, true>(p, pl, st)))
-                    : (pl.BN == 32 ? launch_gemm<32, false>(p, pl, st) : (pl.BN == 64 ? launch_gemm<64, false>(p, pl, st) : launch_gemm<128, false>(p, pl, st)));
+  const int rc = mode == MODE_TF32X3 ? launch_gemm_mode<MODE_TF32X3>(p, pl, st)
+               : (mode == MODE_BF16 ? launch_gemm_mode<MODE_BF16>(p, pl, st) : launch_gemm_mode<MODE_TF32>(p, pl, st));
   if (rc != B2_OK) return rc;
   if (pl.splits > 1) {
     size_t total = (size_t)M * N;

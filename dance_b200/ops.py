@@ -15,7 +15,7 @@ from ._lib import B2Error, check
 from ._lib import lib as _raw_lib
 
 ACT = {"none": 0, None: 0, "relu": 1, "elu": 2, "tanh": 3}
-PREC = {"fp32": 0, "simt": 0, "tf32x3": 1, "tf32": 2}
+PREC = {"fp32": 0, "simt": 0, "tf32x3": 1, "tf32": 2, "bf16": 3}
 
 _DEFAULT_PRECISION = "tf32x3"
 
@@ -77,7 +77,7 @@ def kernel_times():
 
 
 def set_default_precision(p: str):
-    """GEMM precision used when a call does not name one: 'fp32' | 'tf32x3' | 'tf32'."""
+    """GEMM precision used when a call does not name one: 'fp32' | 'tf32x3' | 'tf32' | 'bf16' (see :func:`gemm`)."""
     global _DEFAULT_PRECISION
     if p not in PREC:
         raise ValueError(f"unknown precision {p!r}; choose from {sorted(PREC)}")
@@ -266,7 +266,13 @@ def csr_transpose(A: CSR) -> Tuple[CSR, torch.Tensor]:
 def gemm(A: torch.Tensor, B: torch.Tensor, *, transA: bool = False, transB: bool = False,
          bias: Optional[torch.Tensor] = None, act: Optional[str] = None, mask: Optional[torch.Tensor] = None,
          out: Optional[torch.Tensor] = None, accumulate: bool = False, precision: Optional[str] = None) -> torch.Tensor:
-    """``C = act(op(A) @ op(B) + bias) * (mask > 0)``; ``accumulate`` adds into ``out``."""
+    """``C = act(op(A) @ op(B) + bias) * (mask > 0)``; ``accumulate`` adds into ``out``.
+
+    All tensors are float32.  ``precision`` (default: :func:`set_default_precision`, initially 'tf32x3') bounds how the
+    tensor cores round the operands: 'tf32x3' is fp32-accurate (3-product split), 'tf32' uses 10-bit mantissas, 'bf16'
+    rounds each operand to bfloat16 (round-to-nearest-even, 8-bit mantissa) inside the kernel; all three accumulate in
+    fp32.  'fp32' forces the CUDA-core kernel.  Shapes the tensor-core kernel does not take (K < 8, M·N·K < 2^18, a base
+    not 16-byte aligned or a row pitch not a multiple of 4) run on the CUDA-core fp32 kernel whatever the mode."""
     _chk(A, torch.float32, "A", 2)
     _chk(B, torch.float32, "B", 2)
     lda, ldb = _rowmajor(A, "A"), _rowmajor(B, "B")

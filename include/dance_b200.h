@@ -44,6 +44,7 @@ extern "C" {
 #define B2_PREC_FP32_SIMT 0 /* CUDA-core FFMA, exact fp32 accumulate            */
 #define B2_PREC_TF32X3 1    /* wgmma tf32, 3-product split, ~fp32 accuracy      */
 #define B2_PREC_TF32 2      /* wgmma tf32, single product                        */
+#define B2_PREC_BF16 3      /* wgmma bf16 (operands rounded RNE), fp32 accumulate */
 
 /* Kernel-path selectors for A/B tests: every selectable path returns the same result (bit-exact for the kNN filter, to
  * rounding for the decoder); mode 0 = automatic choice by problem size. */
@@ -120,6 +121,12 @@ int b2_csr_transpose(const int32_t* rowptr, const int32_t* colidx, const float* 
  *   beta   : 0 overwrite, 1 accumulate into C (weight-gradient accumulation)
  *   colsum : optional length-N output, += column sums of the epilogue result
  *            is NOT provided here; see b2_colsum_f32.
+ *   precision: B2_PREC_*.  A, B, C, bias and mask are fp32 in every mode; the mode
+ *            bounds how the operands are rounded for the tensor cores (BF16:
+ *            round-to-nearest-even to bfloat16, fp32 accumulate).  Shapes the
+ *            tensor-core kernel does not take (K < 8, M·N·K < 2^18, a base not
+ *            16-byte aligned or a row pitch not a multiple of 4 elements) run on
+ *            the CUDA-core fp32 kernel in every mode.
  * ---------------------------------------------------------------------- */
 size_t b2_gemm_workspace_bytes(int M, int N, int K, int transA, int transB, int precision);
 int b2_gemm_f32(const float* A, int64_t lda, int transA,

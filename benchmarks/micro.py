@@ -63,18 +63,27 @@ def main():
 
     n = args.n
     if want("spmm"):
+        # fp32 rows of 64 / 128 bytes (F = 16, 32) take the nnz-stream kernel; every other width, and every 16-bit width here,
+        # the row-group kernel: one width per (G, VPL) instantiation, plus the widths the models run (GraphSCI F = 256).
+        widths = [(torch.float32, F) for F in (4, 12, 16, 24, 32, 64, 128, 200, 256, 400, 512)]
+        widths += [(dt, F) for dt in (torch.bfloat16, torch.float16) for F in (8, 104, 128, 256)]
         for local in (None, 100_000, 4096):
             A = random_knn_graph(n, 15, dev, local=local)
-            for F in (16, 32, 64, 128):
+            for dt, F in widths:
                 X = torch.randn(n, F, device=dev)
+                if dt != torch.float32:
+                    X = ops.to_x16(X, dt)
                 Y = torch.empty(n, F, device=dev)
                 med, best = timeit(lambda: ops.spmm(A, X, out=Y), flush=flush)
-                alg = A.nnz * 8 + (n + 1) * 4 + 2 * n * F * 4
-                gather = A.nnz * F * 4
-                out.append(dict(kernel="spmm_csr_f32", n=n, nnz=A.nnz, F=F, locality=local, ms=med, ms_best=best,
-                                alg_GB=alg / 1e9, alg_GBps=alg / med / 1e6, frac_hbm=alg / med / 1e6 / PEAKS["hbm_gbs"],
-                                gather_GBps=gather / med / 1e6))
+                esz = X.element_size()
+                alg = A.nnz * 8 + (n + 1) * 4 + n * F * (esz + 4)
+                gather = A.nnz * F * esz
+                kernel = {torch.float32: "spmm_csr_f32", torch.bfloat16: "spmm_csr_bf16", torch.float16: "spmm_csr_f16"}[dt]
+                out.append(dict(kernel=kernel, n=n, nnz=A.nnz, F=F,
+                                locality=local, ms=med, ms_best=best, alg_GB=alg / 1e9, alg_GBps=alg / med / 1e6,
+                                frac_hbm=alg / med / 1e6 / PEAKS["hbm_gbs"], gather_GBps=gather / med / 1e6))
                 print(json.dumps(out[-1]), flush=True)
+                del X, Y
     if want("gemm"):
         for prec in ("fp32", "tf32x3", "tf32"):
             for (M, N, K, tA, tB) in ((12800, 512, 2000, 0, 1), (12800, 2000, 512, 0, 1), (12800, 128, 512, 0, 1),

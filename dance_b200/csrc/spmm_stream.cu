@@ -1,8 +1,8 @@
 // CSR SpMM, nnz-stream form:  Y = act(reduce(A · X) + bias)  for operand rows of 32 / 64 / 128 bytes
 // (fp32 F = 8 / 16 / 32, bf16 / fp16 F = 16 / 32 / 64) — the scGNN aggregate Â·support (scgnn2.py:500) and its backward.
 //
-// Why a second kernel.  The row-per-lane-group kernels (spmm.cu, spmm16.cu) chain rowptr → (col, val) → gathers → FMA per row and
-// per 8-entry chunk; partial-mask shuffles in loops of per-row trip count cost them ~65 SASS instructions per four non-zeros and
+// Why a second kernel.  The row-per-lane-group kernel (spmm.cu) chains rowptr → (col, val) → gathers → FMA per row and
+// per 8-entry chunk; partial-mask shuffles in loops of per-row trip count cost it ~65 SASS instructions per four non-zeros and
 // low occupancy: latency- and issue-bound, not bandwidth-bound.  Here every warp owns a contiguous range of rows — hence a contiguous stream of non-zeros —
 // and runs a software pipeline over 32-entry blocks of that stream:
 //
@@ -20,10 +20,7 @@
 //
 // TMA row copies (tile::gather4, per-row cp.async.bulk) are a poor fit for this pipeline: 64–128-byte rows are too small for the
 // TMA unit to pay off.
-#include "common.cuh"
-
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
+#include "spmm.cuh"
 
 namespace b2 {
 namespace {
@@ -77,25 +74,6 @@ __device__ __forceinline__ int warp_partition_point(const int32_t* __restrict__ 
     }
   }
   return lo;
-}
-
-template <int DT> __device__ __forceinline__ void unpack2(uint32_t u, float& a, float& b) {
-  if (DT == 0) {                       // bf16: the fp32 value is the 16 bits shifted into the high half
-    a = __uint_as_float(u << 16);
-    b = __uint_as_float(u & 0xffff0000u);
-  } else {
-    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&u));
-    a = f.x;
-    b = f.y;
-  }
-}
-template <int DT> __device__ __forceinline__ uint32_t pack2(float a, float b) {
-  if (DT == 0) {
-    const __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<const uint32_t*>(&v);
-  }
-  const __half2 v = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&v);
 }
 
 struct StreamArgs {
@@ -197,15 +175,18 @@ spmm_stream_kernel(const StreamArgs a) {
                          "f"(o[(i + 3) % NV]) : "memory");
         }
       }
-      if (EPI && DT != 2 && a.Y16) {
-        uint8_t* y = a.Y16 + (int64_t)r * a.ldy16b + lane * NV * 2;
-        if (NV == 2) {
-          *reinterpret_cast<uint32_t*>(y) = pack2<DT>(o[0], o[1 % NV]);
-        } else if (NV == 4) {
-          *reinterpret_cast<uint2*>(y) = make_uint2(pack2<DT>(o[0], o[1 % NV]), pack2<DT>(o[2 % NV], o[3 % NV]));
-        } else if (NV == 8) {
-          *reinterpret_cast<uint4*>(y) = make_uint4(pack2<DT>(o[0], o[1 % NV]), pack2<DT>(o[2 % NV], o[3 % NV]), pack2<DT>(o[4 % NV], o[5 % NV]),
-                                                    pack2<DT>(o[6 % NV], o[7 % NV]));
+      if constexpr (EPI && DT != 2) {
+        if (a.Y16) {
+          uint8_t* y = a.Y16 + (int64_t)r * a.ldy16b + lane * NV * 2;
+          using E = Elem<DT>;
+          if (NV == 2) {
+            *reinterpret_cast<uint32_t*>(y) = E::pack2(o[0], o[1 % NV]);
+          } else if (NV == 4) {
+            *reinterpret_cast<uint2*>(y) = make_uint2(E::pack2(o[0], o[1 % NV]), E::pack2(o[2 % NV], o[3 % NV]));
+          } else if (NV == 8) {
+            *reinterpret_cast<uint4*>(y) = make_uint4(E::pack2(o[0], o[1 % NV]), E::pack2(o[2 % NV], o[3 % NV]), E::pack2(o[4 % NV], o[5 % NV]),
+                                                      E::pack2(o[6 % NV], o[7 % NV]));
+          }
         }
       }
     }
@@ -266,7 +247,7 @@ spmm_stream_kernel(const StreamArgs a) {
           const int slot = k - eb;
           const float wv = vb[slot];
           const uint8_t* src = blk + slot * RB + glc * CB;
-          if (DT == 2) {
+          if constexpr (DT == 2) {
             if (NV == 1) {
               acc[0] = fmaf(wv, *reinterpret_cast<const float*>(src), acc[0]);
             } else if (NV == 2) {
@@ -278,20 +259,21 @@ spmm_stream_kernel(const StreamArgs a) {
               acc[2 % NV] = fmaf(wv, x.z, acc[2 % NV]); acc[3 % NV] = fmaf(wv, x.w, acc[3 % NV]);
             }
           } else {
+            using E = Elem<DT>;
             float p, q;
             if (NV == 2) {
-              unpack2<DT>(*reinterpret_cast<const uint32_t*>(src), p, q);
+              E::unpack2(*reinterpret_cast<const uint32_t*>(src), p, q);
               acc[0] = fmaf(wv, p, acc[0]); acc[1 % NV] = fmaf(wv, q, acc[1 % NV]);
             } else if (NV == 4) {
               const uint2 x = *reinterpret_cast<const uint2*>(src);
-              unpack2<DT>(x.x, p, q); acc[0] = fmaf(wv, p, acc[0]); acc[1 % NV] = fmaf(wv, q, acc[1 % NV]);
-              unpack2<DT>(x.y, p, q); acc[2 % NV] = fmaf(wv, p, acc[2 % NV]); acc[3 % NV] = fmaf(wv, q, acc[3 % NV]);
+              E::unpack2(x.x, p, q); acc[0] = fmaf(wv, p, acc[0]); acc[1 % NV] = fmaf(wv, q, acc[1 % NV]);
+              E::unpack2(x.y, p, q); acc[2 % NV] = fmaf(wv, p, acc[2 % NV]); acc[3 % NV] = fmaf(wv, q, acc[3 % NV]);
             } else {
               const uint4 x = *reinterpret_cast<const uint4*>(src);
-              unpack2<DT>(x.x, p, q); acc[0] = fmaf(wv, p, acc[0]); acc[1 % NV] = fmaf(wv, q, acc[1 % NV]);
-              unpack2<DT>(x.y, p, q); acc[2 % NV] = fmaf(wv, p, acc[2 % NV]); acc[3 % NV] = fmaf(wv, q, acc[3 % NV]);
-              unpack2<DT>(x.z, p, q); acc[4 % NV] = fmaf(wv, p, acc[4 % NV]); acc[5 % NV] = fmaf(wv, q, acc[5 % NV]);
-              unpack2<DT>(x.w, p, q); acc[6 % NV] = fmaf(wv, p, acc[6 % NV]); acc[7 % NV] = fmaf(wv, q, acc[7 % NV]);
+              E::unpack2(x.x, p, q); acc[0] = fmaf(wv, p, acc[0]); acc[1 % NV] = fmaf(wv, q, acc[1 % NV]);
+              E::unpack2(x.y, p, q); acc[2 % NV] = fmaf(wv, p, acc[2 % NV]); acc[3 % NV] = fmaf(wv, q, acc[3 % NV]);
+              E::unpack2(x.z, p, q); acc[4 % NV] = fmaf(wv, p, acc[4 % NV]); acc[5 % NV] = fmaf(wv, q, acc[5 % NV]);
+              E::unpack2(x.w, p, q); acc[6 % NV] = fmaf(wv, p, acc[6 % NV]); acc[7 % NV] = fmaf(wv, q, acc[7 % NV]);
             }
           }
         }
@@ -333,8 +315,6 @@ int launch_stream(const StreamArgs& a, cudaStream_t st) {
 
 }  // namespace
 
-// Returns B2_OK when the nnz-stream kernel took the call, 1 when the shape is not one it handles (caller falls back), < 0 on error.
-// dtype: 2 fp32, 0 bf16, 1 fp16 operand.
 int spmm_stream_dispatch(int dtype, const int32_t* rowptr, const int32_t* colidx, const float* vals, const void* X, int64_t ldx, float* Y,
                          int64_t ldy, void* Y16, int64_t ldy16, int32_t n_rows, int32_t F, int reduce, int act, const float* bias,
                          cudaStream_t st) {

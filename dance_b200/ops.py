@@ -212,40 +212,32 @@ def to_x16(X: torch.Tensor, dtype=torch.bfloat16, out: Optional[torch.Tensor] = 
 
 def spmm(A: CSR, X: torch.Tensor, reduce: str = "sum", act: Optional[str] = None,
          out: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None, out16: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``Y = act(A @ X)`` (reduce='sum') or row-mean (reduce='mean').  A bf16 / fp16 ``X`` selects the 16-bit-operand kernel
-    (fp32 accumulation, fp32 ``out``; ``out16`` additionally receives the result in the operand's type)."""
-    if isinstance(X, torch.Tensor) and X.dtype in _X16:
-        fn, _ = _X16[X.dtype]
-        _chk(X, X.dtype, "X", 2)
-        n_rows, n_cols = A.shape
-        if X.shape[0] != n_cols:
-            raise B2Error(f"spmm: A is {A.shape} but X has {X.shape[0]} rows")
-        F = X.shape[1]
-        if out is None and out16 is None:
-            out = torch.empty((n_rows, F), dtype=torch.float32, device=X.device)
-        if out is not None:
-            _chk(out, torch.float32, "out", 2)
-        if out16 is not None:
-            _chk(out16, X.dtype, "out16", 2)
-        colidx_ptr = _p(A.colidx) if A.nnz else _p(A.rowptr)
-        check(getattr(lib(), fn)(_p(A.rowptr), colidx_ptr, _p(A.vals) if A.nnz else None, _p(X), _rowmajor(X, "X"),
-                                 _p(out), _rowmajor(out, "out") if out is not None else 0,
-                                 _p(out16), _rowmajor(out16, "out16") if out16 is not None else 0,
-                                 n_rows, n_cols, F, {"sum": 0, "mean": 1}[reduce], ACT[act], _p(bias), _stream()), fn)
-        return out if out is not None else out16
-    _chk(X, torch.float32, "X", 2)
-    ldx = _rowmajor(X, "X")
+    """``Y = act(A @ X)`` (reduce='sum') or row-mean (reduce='mean').  A bf16 / fp16 ``X`` is gathered in its 16-bit
+    type (fp32 accumulation, fp32 ``out``; ``out16`` additionally receives the result in the operand's type)."""
+    x16 = isinstance(X, torch.Tensor) and X.dtype in _X16
+    _chk(X, X.dtype if x16 else torch.float32, "X", 2)
     n_rows, n_cols = A.shape
     if X.shape[0] != n_cols:
         raise B2Error(f"spmm: A is {A.shape} but X has {X.shape[0]} rows")
     F = X.shape[1]
-    if out is None:
+    if not x16:
+        out16 = None  # an fp32 operand has no 16-bit result copy
+    if out is None and out16 is None:
         out = torch.empty((n_rows, F), dtype=torch.float32, device=X.device)
-    _chk(out, torch.float32, "out", 2)
+    if out is not None:
+        _chk(out, torch.float32, "out", 2)
+    if out16 is not None:
+        _chk(out16, X.dtype, "out16", 2)
     colidx_ptr = _p(A.colidx) if A.nnz else _p(A.rowptr)  # an empty matrix has no colidx storage; never dereferenced
-    check(lib().b2_spmm_csr_f32(_p(A.rowptr), colidx_ptr, _p(A.vals) if A.nnz else None, _p(X), ldx, _p(out), _rowmajor(out, "out"),
-                                n_rows, n_cols, F, {"sum": 0, "mean": 1}[reduce], ACT[act], _p(bias), _stream()), "b2_spmm_csr_f32")
-    return out
+    args = [_p(A.rowptr), colidx_ptr, _p(A.vals) if A.nnz else None, _p(X), _rowmajor(X, "X"),
+            _p(out), _rowmajor(out, "out") if out is not None else 0]
+    if x16:
+        fn = _X16[X.dtype][0]
+        args += [_p(out16), _rowmajor(out16, "out16") if out16 is not None else 0]
+    else:
+        fn = "b2_spmm_csr_f32"
+    check(getattr(lib(), fn)(*args, n_rows, n_cols, F, {"sum": 0, "mean": 1}[reduce], ACT[act], _p(bias), _stream()), fn)
+    return out if out is not None else out16
 
 
 def csr_transpose(A: CSR) -> Tuple[CSR, torch.Tensor]:

@@ -74,7 +74,8 @@ int b2_device_info(int* sm_count, int* cc_major, int* cc_minor);
  *   vals      : nnz edge weights, or NULL for an unweighted (0/1) graph
  *   reduce    : 0 = sum, 1 = mean over the row's nnz (0 for empty rows)
  *   act       : B2_ACT_* applied to the output row
- *   F must be a multiple of 4; X/Y rows must be 16-byte aligned.
+ *   F must be a multiple of 4; X/Y rows and bias must be 16-byte aligned.
+ *   F > 512 returns B2_ERR_UNSUPPORTED.
  * ---------------------------------------------------------------------- */
 int b2_spmm_csr_f32(const int32_t* rowptr, const int32_t* colidx, const float* vals,
                     const float* X, int64_t ldx, float* Y, int64_t ldy,
@@ -85,8 +86,9 @@ int b2_spmm_csr_f32(const int32_t* rowptr, const int32_t* colidx, const float* v
  * configurations (BASELINE config 3 "GraphSCI … bf16"; dglnn.GraphConv under autocast, graphsci.py:112-115) and the
  * bandwidth-optimised form of torch.spmm(adj, support) scgnn2.py:500: every non-zero gathers F·2 instead of F·4 bytes.
  *   X       : [n_cols, F] bf16 / fp16, leading dimension ldx (elements), rows 16-byte aligned, F % 8 == 0, F <= 256
- *   Y       : fp32 output or NULL;  Y16 : output in the operand's 16-bit type or NULL (feeds the next layer's aggregate
- *             without a conversion pass); at least one of the two. */
+ *   Y       : fp32 output or NULL;  Y16 : output in the operand's 16-bit type (round-to-nearest-even) or NULL (feeds the next
+ *             layer's aggregate without a conversion pass); at least one of the two, rows 16-byte aligned.
+ *   bias    : length F or NULL, 4-byte alignment suffices. */
 int b2_spmm_csr_bf16(const int32_t* rowptr, const int32_t* colidx, const float* vals,
                      const void* X, int64_t ldx, float* Y, int64_t ldy, void* Y16, int64_t ldy16,
                      int32_t n_rows, int32_t n_cols, int32_t F, int reduce, int act, const float* bias, void* stream);

@@ -1,7 +1,7 @@
 // Tensor-core version of the all-pairs part of the Graph-AE decoder loss (scgnn2.py:423-426, 603-619):
 //   loss += Σ_ij softplus(z_i · z_j),   dZ_i += 2·coef · Σ_j σ(z_i · z_j) · z_j
-// Flash-attention-shaped row sweep: a CTA owns 128 rows I (two consumer warpgroups of 64) and streams 128-row tiles J:
-//   S  = Z_I · Z_Jᵀ        wgmma m64n128k8 tf32, 3-product split (Z pre-split into hi = x & 0xFFFFE000 and lo = x − hi,
+// Flash-attention-shaped row sweep: a CTA owns 128 rows I (two consumer warpgroups of 64) and streams J tiles:
+//   S  = Z_I · Z_Jᵀ        wgmma m64nJWk8 tf32, 3-product split (Z pre-split into hi = x & 0xFFFFE000 and lo = x − hi,
 //                          lo·hi + hi·lo + hi·hi), fp32 accumulators in registers
 //   G  = σ(S), loss       SFU math on the accumulator registers (e = 2^(−|x|·log2e), r = 1/(1+e), one lg2 per 32 logits)
 //   dZ_I += G · Z_J       wgmma m64nDk8 tf32 with A = G taken straight from the registers (hi / lo split of G and Z_J, three
@@ -9,19 +9,30 @@
 // A producer warpgroup (one thread of it) copies the pre-split J tiles into a three-stage ring with 1-D bulk copies (the tiles
 // are laid out in global memory exactly as wgmma reads them: K-major, 128-byte swizzle).
 //
-// Schedule: each product is issued as one batch of wgmmas with one commit and one wait (S: 3·DP/8, dZ: 3·16), which needs S,
-// both halves of G and the dZ accumulators live in registers at once; the producer warpgroup gives its registers to the
-// consumers (setmaxnreg) to make room.  The two consumer warpgroups run out of phase ("ping-pong"): while one does σ / softplus
-// on the SFU, the other's products run on the tensor cores.  Tiles with no masked logit take an elementwise loop without the
-// per-logit mask.
+// Two kernels share that sweep:
+//   gae_allpairs_tc_kernel  J tiles of 128 columns over every column: row subsets (row shards) and the pair-sharded form.
+//   gae_tri_tc_kernel       the full-row call.  S is symmetric, so block I only sweeps J ≥ I in tiles of 64 columns.  The
+//                          128 x 128 diagonal block is evaluated as in the full sweep (it holds both orders of each pair); every
+//                          tile above it counts its loss twice and also yields dZ_J += Gᵀ · Z_I: G goes to shared memory as
+//                          hi / lo planes of Gᵀ (K-major in i, the A operand) and Z_Iᵀ is the B operand.  Both dZ products
+//                          issue their three products as two: hi·hi and hi·lo as one m64n(2·DP)k8 against a B operand laid
+//                          out [hi | lo], and lo·hi.  The tile's dZ_J leaves through red.global.add.
+//
+// Schedule: each product is issued as one batch of wgmmas with one commit and one wait, which needs S, both halves of G and
+// the dZ accumulators live in registers at once; the producer warpgroup gives its registers to the consumers (setmaxnreg) to
+// make room.  The two consumer warpgroups run out of phase ("ping-pong"): while one does σ / softplus on the SFU, the other's
+// products run on the tensor cores.  Tiles with no masked logit take an elementwise loop without the per-logit mask.
 //
 // Register fragment trick: the accumulator of S gives a thread columns (2t, 2t+1) of each 8-column block, the tf32 A fragment
 // wants columns (t, t+4).  The sum over j does not care about order, so the 8 columns of each block are fed to the second
-// MMA in the order (0, 2, 4, 6, 1, 3, 5, 7) and Z_Jᵀ is stored with its columns permuted the same way.
+// MMA in the order (0, 2, 4, 6, 1, 3, 5, 7) and Z_Jᵀ is stored with its columns permuted the same way.  Likewise the sum over i
+// of dZ_J: rows r and r + 8 of a thread's fragment are put side by side in the K order of Gᵀ and Z_Iᵀ (gt_pos), so that each
+// thread writes its two Gᵀ values of a column with one 64-bit store.
 //
 // Work units: row blocks.  The row form covers [row_begin, row_begin + n_rows); the pair-sharded form (multi-GPU) takes
 // "super-blocks" s = {block s, block nb−1−s} (a lone middle block when nb is odd), so that super-block ranges split the work
-// evenly over ranks.  The J sweep of a unit can be cut into step ranges (grid.y), which then add into dz atomically.
+// evenly over ranks; the triangle's block I carries nb − I blocks of work and blocks are launched in order, longest first.
+// The J sweep of a unit can be cut into step ranges (grid.y), which then add into dz atomically.
 #include "tc_common.cuh"
 
 #include <stdlib.h>
@@ -32,22 +43,40 @@ namespace gtc {
 
 using namespace tc;
 
-constexpr int BT = 128;                 // rows per block / tile
+constexpr int BT = 128;                 // rows per block / workspace tile
 constexpr int CONSUMERS = 256;          // two warpgroups
 constexpr int THREADS = CONSUMERS + 128; // + producer warpgroup
 // Register split (setmaxnreg): the consumers hold S, both halves of G and the dZ accumulators while a dZ batch is in flight.
 // 128 · 40 + 256 · 232 = 64 512 of the 65 536 registers of an SM.
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
-constexpr int STAGES = 3;               // DP = 32: 32 KB + 3 x 64 KB, just inside the 227 KB a CTA may have
+constexpr int STAGES = 3;
 constexpr int MAX_D = 32;
 constexpr uint32_t ZS_BYTES = BT * 128; // one plane of a tile for S (K-major, 128-byte rows)
 constexpr int ZS_PLANES = 2;            // hi, lo
+constexpr size_t MAX_SMEM = 227 * 1024; // dynamic shared memory a CTA may have on sm_90
 
 static int64_t padded_n(int32_t n) { return ((int64_t)n + BT - 1) / BT * BT; }
 template <int DP> constexpr uint32_t zt_bytes() { return (uint32_t)DP * 4 * 128; }   // one plane of Z_Jᵀ: 4 atoms of DP x 128 B
 
+// Shared memory of a sweep.  Full sweep (DP = 32): Z_I 32 KB + 3 x 64 KB stages.  Triangle (DP = 32): Z_I 32 KB, Z_Iᵀ 32 KB,
+// Gᵀ 64 KB, 3 x 32 KB stages; the 64-column J tiles are the halves of a 128-row workspace tile (contiguous in both planes).
+template <int DP, bool TRI>
+struct Tiles {
+  static constexpr int JW = TRI ? 64 : BT;                        // J tile width
+  static constexpr uint32_t JS = JW * 128;                        // one plane of a J tile for S
+  static constexpr uint32_t JT = zt_bytes<DP>() / (BT / JW);      // one plane of a J tile's Z_Jᵀ
+  static constexpr uint32_t STAGE = ZS_PLANES * JS + 2 * JT;
+  static constexpr uint32_t ZIT = TRI ? zt_bytes<DP>() : 0;       // one plane of Z_Iᵀ
+  static constexpr uint32_t GT = TRI ? 64 * 64 * 4 : 0;           // one plane of a warpgroup's Gᵀ: 64 j x 64 i, 2 atoms
+  static constexpr uint32_t RING = ZS_PLANES * ZS_BYTES + 2 * ZIT + 4 * GT;
+  static constexpr size_t SMEM = RING + STAGES * STAGE + 16 * STAGES + 1024;
+};
+static_assert(Tiles<MAX_D, false>::SMEM <= MAX_SMEM && Tiles<MAX_D, true>::SMEM <= MAX_SMEM, "decoder shared memory");
+
 // position of column jj of a tile in the permuted order of the dZ MMA (see header)
 __host__ __device__ __forceinline__ int zt_pos(int jj) { const int q = jj & 7; return (jj & ~7) | ((q & 1) ? 4 + (q >> 1) : (q >> 1)); }
+// position of row i (0..63) of a warpgroup in the K order of the dZ_J MMA: rows r and r + 8 of a 16-row group become neighbours
+__host__ __device__ __forceinline__ int gt_pos(int i) { return (i & ~15) | ((i & 7) << 1) | ((i >> 3) & 1); }
 
 __device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
@@ -92,23 +121,35 @@ template <int N>
 __device__ __forceinline__ void mma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
   if constexpr (N == 8) wgmma_tf32_rs_n8(d, a, b, scale_d);
   else if constexpr (N == 16) wgmma_tf32_rs_n16(d, a, b, scale_d);
-  else wgmma_tf32_rs_n32(d, a, b, scale_d);
+  else if constexpr (N == 32) wgmma_tf32_rs_n32(d, a, b, scale_d);
+  else wgmma_tf32_rs_n64(d, a, b, scale_d);
+}
+template <int N>
+__device__ __forceinline__ void mma_ss(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
+  if constexpr (N == 8) wgmma_tf32_ss_n8(d, a, b, scale_d);
+  else if constexpr (N == 16) wgmma_tf32_ss_n16(d, a, b, scale_d);
+  else if constexpr (N == 32) wgmma_tf32_ss_n32(d, a, b, scale_d);
+  else if constexpr (N == 64) wgmma_tf32_ss_n64(d, a, b, scale_d);
+  else wgmma_tf32_ss_n128(d, a, b, scale_d);
 }
 
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ void sts_v2(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
 
-// σ and softplus of one thread's 64 logits S (the m64n128 accumulator), in place: S becomes the hi part of G = σ(S) and L its
-// lo part, ready to be the register A operand of the dZ product.  Returns the thread's share of Σ softplus.  MASKED zeroes G
-// and drops the loss of columns j ≥ n and of rows past the range (the last J tile, a partial I block); interior tiles skip the
+// σ and softplus of one thread's logits S (the m64nJW accumulator), in place: S becomes the hi part of G = σ(S) and L its lo
+// part, ready to be the register A operand of the dZ product.  Returns the thread's share of Σ softplus.  MASKED zeroes G and
+// drops the loss of columns j ≥ n and of rows past the range (the last J tile, a partial I block); interior tiles skip the
 // per-logit mask and its selects.
-template <bool MASKED>
-__device__ __forceinline__ float sigmoid_softplus(float (&S)[BT / 2], float (&L)[BT / 2], int jbase, int n, bool live_a, bool live_b) {
+template <bool MASKED, int V>
+__device__ __forceinline__ float sigmoid_softplus(float (&S)[V], float (&L)[V], int jbase, int n, bool live_a, bool live_b) {
   constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
   float relu = 0.f, lg = 0.f, prod = 1.f;
 #pragma unroll
-  for (int v = 0; v < BT / 2; ++v) {
+  for (int v = 0; v < V; ++v) {
     if ((v & 31) == 31) { lg += lg2_approx(prod); prod = 1.f; }
     const float x = S[v];
     const float e = ex2_approx(-fabsf(x) * LOG2E);
@@ -131,32 +172,44 @@ __device__ __forceinline__ float sigmoid_softplus(float (&S)[BT / 2], float (&L)
   return relu + LN2 * (lg + lg2_approx(prod));
 }
 
-template <int DP>
-__global__ void __launch_bounds__(THREADS, 1)
-gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
+// The sweep of one work unit; TRI selects the triangle (see header).
+template <int DP, bool TRI>
+__device__ __forceinline__ void decoder_sweep(const Params& p) {
+  using T = Tiles<DP, TRI>;
+  constexpr int JW = T::JW;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr uint32_t ZT = zt_bytes<DP>();
-  constexpr uint32_t STAGE = ZS_PLANES * ZS_BYTES + 2 * ZT;
   uint8_t* zi_hi = smem;
   uint8_t* zi_lo = smem + ZS_BYTES;
-  uint8_t* ring = smem + ZS_PLANES * ZS_BYTES;
-  const uint32_t full_bar = smem_u32(ring + STAGES * STAGE), empty_bar = full_bar + 8 * STAGES;
+  uint8_t* zit = smem + ZS_PLANES * ZS_BYTES;      // triangle: Z_Iᵀ [warpgroup][atom][hi, lo]; then Gᵀ [warpgroup][hi, lo]
+  uint8_t* ring = smem + T::RING;
+  constexpr uint32_t ATOM = DP * 128;              // DP rows of 32 tf32 along K
+  constexpr int NB = DP <= 16 ? 4 : 2;             // full sweep: hi·hi accumulators
+  constexpr int NBM = DP <= 16 ? 2 : 1;            // triangle: [hi·hi | hi·lo] accumulators
+  const uint32_t full_bar = smem_u32(ring + STAGES * T::STAGE), empty_bar = full_bar + 8 * STAGES;
 
   // ---- work unit ----
-  int row0, row_end, dz_row0;
-  if (p.sym) {
-    const int sb = p.sb_begin + (int)(blockIdx.x >> 1);
-    const int blk = (blockIdx.x & 1) ? p.nb - 1 - sb : sb;
-    if ((blockIdx.x & 1) && blk == sb) return;           // lone middle block: one unit only
-    row0 = blk * BT; row_end = min(p.n, row0 + BT); dz_row0 = 0;
+  int row0, row_end, dz_row0, jt0, jt1;
+  if constexpr (TRI) {
+    row0 = (int)blockIdx.x * BT; row_end = min(p.n, row0 + BT); dz_row0 = 0;
+    const int first = row0 / JW;                         // J tiles from the diagonal block on
+    const int per = (p.n_jt - first + (int)gridDim.y - 1) / (int)gridDim.y;
+    jt0 = first + (int)blockIdx.y * per; jt1 = min(p.n_jt, jt0 + per);
   } else {
-    row0 = p.row_begin + (int)blockIdx.x * BT; row_end = min(p.row_end, row0 + BT); dz_row0 = p.row_begin;
+    if (p.sym) {
+      const int sb = p.sb_begin + (int)(blockIdx.x >> 1);
+      const int blk = (blockIdx.x & 1) ? p.nb - 1 - sb : sb;
+      if ((blockIdx.x & 1) && blk == sb) return;         // lone middle block: one unit only
+      row0 = blk * BT; row_end = min(p.n, row0 + BT); dz_row0 = 0;
+    } else {
+      row0 = p.row_begin + (int)blockIdx.x * BT; row_end = min(p.row_end, row0 + BT); dz_row0 = p.row_begin;
+    }
+    const int per = (p.n_jt + (int)gridDim.y - 1) / (int)gridDim.y;
+    jt0 = (int)blockIdx.y * per; jt1 = min(p.n_jt, jt0 + per);
   }
-  const int per = (p.n_jt + (int)gridDim.y - 1) / (int)gridDim.y;
-  const int jt0 = (int)blockIdx.y * per, jt1 = min(p.n_jt, jt0 + per);
   if (jt0 >= jt1) return;
   const int nt = jt1 - jt0;
+  const int diag_end = (row0 + BT) / JW;                 // triangle: tiles below this one are the diagonal block's
 
   const int tid = threadIdx.x;
   if (tid == 0) {
@@ -173,13 +226,21 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
       for (int i = 0; i < nt; ++i) {
         const int s = i % STAGES;
         if (i >= STAGES) mbar_wait(empty_bar + 8 * s, (uint32_t)((i / STAGES - 1) & 1));
-        const uint32_t fb = full_bar + 8 * s, dst = smem_u32(ring + s * STAGE);
+        const uint32_t fb = full_bar + 8 * s, dst = smem_u32(ring + s * T::STAGE);
         const size_t t = (size_t)(jt0 + i);
-        mbar_expect_tx(fb, STAGE);
-        bulk_load(dst, p.zs_hi + t * ZS_BYTES, ZS_BYTES, fb);
-        bulk_load(dst + ZS_BYTES, p.zs_lo + t * ZS_BYTES, ZS_BYTES, fb);
-        bulk_load(dst + 2 * ZS_BYTES, p.zt_hi + t * ZT, ZT, fb);
-        bulk_load(dst + 2 * ZS_BYTES + ZT, p.zt_lo + t * ZT, ZT, fb);
+        mbar_expect_tx(fb, T::STAGE);
+        bulk_load(dst, p.zs_hi + t * T::JS, T::JS, fb);
+        bulk_load(dst + T::JS, p.zs_lo + t * T::JS, T::JS, fb);
+        if constexpr (TRI) {
+          // atom by atom, lo after hi: the B operand [Z_Jᵀ hi | Z_Jᵀ lo] of the merged dZ_I products
+          for (uint32_t a = 0; a < T::JT / ATOM; ++a) {
+            bulk_load(dst + 2 * T::JS + 2 * a * ATOM, p.zt_hi + t * T::JT + a * ATOM, ATOM, fb);
+            bulk_load(dst + 2 * T::JS + (2 * a + 1) * ATOM, p.zt_lo + t * T::JT + a * ATOM, ATOM, fb);
+          }
+        } else {
+          bulk_load(dst + 2 * T::JS, p.zt_hi + t * T::JT, T::JT, fb);
+          bulk_load(dst + 2 * T::JS + T::JT, p.zt_lo + t * T::JT, T::JT, fb);
+        }
       }
     }
     return;
@@ -187,7 +248,8 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
 
   // ===================== consumers =====================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
-  // Z_I planes from z (rows past the range are zero: their logits are masked below)
+  // Z_I planes from z (rows past the range are zero: their logits are masked below); the triangle also builds Z_Iᵀ, per
+  // warpgroup 2 atoms of [DP hi rows | DP lo rows] x 32 i in the gt_pos order
   for (int e = tid; e < BT * DP; e += CONSUMERS) {
     const int r = e / DP, k = e % DP;
     const int row = row0 + r;
@@ -196,6 +258,12 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
     const uint32_t o = sw128_offset32((uint32_t)r, (uint32_t)k);
     *reinterpret_cast<float*>(zi_hi + o) = h;
     *reinterpret_cast<float*>(zi_lo + o) = v - h;
+    if constexpr (TRI) {
+      const int q = gt_pos(r & 63);
+      const uint32_t ot = (uint32_t)(r >> 6) * (4 * ATOM) + (uint32_t)(q >> 5) * (2 * ATOM) + sw128_offset32((uint32_t)k, (uint32_t)(q & 31));
+      *reinterpret_cast<float*>(zit + ot) = h;
+      *reinterpret_cast<float*>(zit + ot + ATOM) = v - h;
+    }
   }
   fence_proxy_async();
   asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
@@ -205,13 +273,20 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
   const bool live_a = ra < row_end, live_b = ra + 8 < row_end;
   const uint32_t ai_hi = smem_u32(zi_hi) + wg * 64 * 128, ai_lo = smem_u32(zi_lo) + wg * 64 * 128;
   const bool full_rows = row0 + BT <= row_end;                   // no dead rows in this block: only the last J tile is masked
+  // triangle: this warpgroup's Gᵀ planes (A of dZ_J) and Z_Iᵀ (B of dZ_J)
+  uint8_t* gt_hi = zit + 2 * T::ZIT + wg * 2 * T::GT;
+  uint8_t* gt_lo = gt_hi + T::GT;
+  const uint32_t bi = smem_u32(zit) + wg * (4 * ATOM);
+  const float c2 = 2.f * p.coef;
 
   // The accumulation inside the tensor core truncates, and the hi·hi product carries almost all of dZ: over a whole J sweep one
-  // accumulator would drift by ~1e-5 relative (~6e-5 for |z| ~ 1e5).  So the hi·hi products of a tile go round-robin into NB
-  // accumulators (16 / NB adds each), the two cross terms into one more, and the tile's sum joins an fp32 total with
-  // round-to-nearest adds.
-  constexpr int NB = DP <= 16 ? 4 : 2;
-  float dzb[NB][DP / 2], dzs[DP / 2], dzt[DP / 2];
+  // accumulator would drift by ~1e-5 relative (~6e-5 for |z| ~ 1e5).  So the hi·hi products of a tile go round-robin into
+  // several accumulators (at most 4 k-steps each for DP ≤ 16, 8 at DP = 32), the cross terms into one more, and the tile's sum
+  // joins an fp32 total with round-to-nearest adds.  The full sweep issues the three products at N = DP (NB accumulators for
+  // hi·hi).  The triangle has twice the dZ products per logit and issues fewer, wider ones: hi·hi and hi·lo as one N = 2·DP
+  // product against [hi | lo] of the B operand (NBM accumulators), lo·hi alone; the same for dZ_J.
+  float dzb[TRI ? 1 : NB][DP / 2], dzs[DP / 2], dzt[DP / 2];
+  float dzm[TRI ? NBM : 1][DP], djm[TRI ? NBM : 1][DP], djs[DP / 2];
 #pragma unroll
   for (int v = 0; v < DP / 2; ++v) dzt[v] = 0.f;
   double loss = 0.0;
@@ -220,8 +295,9 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
   // S product of the next one, each issued as one batch with one commit and one wait.  The turn passes on once both are done
   // (named barrier 2 + wg means "wg may issue"), and the warpgroup works through σ / softplus of its S while the other one's
   // products run.  Warpgroup 0 takes the first turn.  Each warpgroup takes nt + 1 turns and passes nt of them on; warpgroup 0
-  // passes its last one as well, so that every bar.arrive meets one bar.sync.
-  float S[BT / 2], L[BT / 2];   // S: accumulator of S, then the hi part of G; L: the lo part of G
+  // passes its last one as well, so that every bar.arrive meets one bar.sync.  The bar.sync of a turn also orders this
+  // warpgroup's Gᵀ stores before the dZ_J product that reads them.
+  float S[JW / 2], L[JW / 2];   // S: accumulator of S, then the hi part of G; L: the lo part of G
   auto take_turn = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(2 + wg), "n"(CONSUMERS) : "memory"); };
   auto pass_turn = [&]() { asm volatile("bar.arrive %0, %1;" ::"r"(3 - wg), "n"(CONSUMERS) : "memory"); };
 
@@ -229,60 +305,131 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
   auto issue_s = [&](int i) {
     const int s = i % STAGES;
     mbar_wait(full_bar + 8 * s, (uint32_t)((i / STAGES) & 1));
-    const uint32_t bs_hi = smem_u32(ring + s * STAGE), bs_lo = bs_hi + ZS_BYTES;
+    const uint32_t bs_hi = smem_u32(ring + s * T::STAGE), bs_lo = bs_hi + T::JS;
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < DP / 8; ++kk) {
       const uint32_t o = kk * 32;
-      wgmma_tf32_ss_n128(S, wgmma_desc_sw128(ai_lo + o), wgmma_desc_sw128(bs_hi + o), kk > 0);
-      wgmma_tf32_ss_n128(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_lo + o), 1);
-      wgmma_tf32_ss_n128(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_hi + o), 1);
+      mma_ss<JW>(S, wgmma_desc_sw128(ai_lo + o), wgmma_desc_sw128(bs_hi + o), kk > 0);
+      mma_ss<JW>(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_lo + o), 1);
+      mma_ss<JW>(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_hi + o), 1);
     }
     wgmma_commit();
   };
-  // dZ_I += G · Z_J of tile i: one batch of 3·16 products with A = (S, L) from the registers, waited for (S is overwritten next)
+  // dZ_I += G · Z_J of tile i with A = (S, L) from the registers, and in the triangle dZ_J += Gᵀ · Z_I (on the diagonal block
+  // it is computed and dropped); one batch, waited for (S is overwritten next).  Full sweep: 3·16 products; triangle: 2·8 + 2·8.
   auto run_dz = [&](int i) {
-    const uint32_t bt_hi = smem_u32(ring + (i % STAGES) * STAGE) + 2 * ZS_BYTES, bt_lo = bt_hi + ZT;
+    const uint32_t bt_hi = smem_u32(ring + (i % STAGES) * T::STAGE) + 2 * T::JS, bt_lo = bt_hi + T::JT;
     wgmma_fence();
 #pragma unroll
-    for (int kb = 0; kb < BT / 8; ++kb) {
+    for (int kb = 0; kb < JW / 8; ++kb) {
       // A fragment (r, t) (r+8, t) (r, t+4) (r+8, t+4) in the permuted column order: (r, 2t) (r+8, 2t) (r, 2t+1) (r+8, 2t+1)
       const uint32_t ahi[4] = {__float_as_uint(S[4 * kb]), __float_as_uint(S[4 * kb + 2]), __float_as_uint(S[4 * kb + 1]),
                                __float_as_uint(S[4 * kb + 3])};
       const uint32_t alo[4] = {__float_as_uint(L[4 * kb]), __float_as_uint(L[4 * kb + 2]), __float_as_uint(L[4 * kb + 1]),
                                __float_as_uint(L[4 * kb + 3])};
-      const uint32_t o = (uint32_t)(kb >> 2) * (DP * 128) + (uint32_t)(kb & 3) * 32;
-      mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
-      mma_rs<DP>(dzs, ahi, wgmma_desc_sw128(bt_lo + o), 1);
-      mma_rs<DP>(dzb[kb % NB], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NB);
+      if constexpr (TRI) {
+        const uint32_t o = (uint32_t)(kb >> 2) * (2 * ATOM) + (uint32_t)(kb & 3) * 32;   // atom [hi | lo]
+        mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
+        mma_rs<2 * DP>(dzm[kb % NBM], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NBM);
+      } else {
+        const uint32_t o = (uint32_t)(kb >> 2) * ATOM + (uint32_t)(kb & 3) * 32;
+        mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
+        mma_rs<DP>(dzs, ahi, wgmma_desc_sw128(bt_lo + o), 1);
+        mma_rs<DP>(dzb[kb % NB], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NB);
+      }
+    }
+    if constexpr (TRI) {
+      const uint32_t ag_hi = smem_u32(gt_hi), ag_lo = smem_u32(gt_lo);
+#pragma unroll
+      for (int kk = 0; kk < 64 / 8; ++kk) {
+        const uint32_t oa = (uint32_t)(kk >> 2) * (64 * 128) + (uint32_t)(kk & 3) * 32;
+        const uint32_t ob = (uint32_t)(kk >> 2) * (2 * ATOM) + (uint32_t)(kk & 3) * 32;
+        mma_ss<DP>(djs, wgmma_desc_sw128(ag_lo + oa), wgmma_desc_sw128(bi + ob), kk > 0);
+        mma_ss<2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + oa), wgmma_desc_sw128(bi + ob), kk >= NBM);
+      }
     }
     wgmma_commit();
     wgmma_wait<0>();
-#pragma unroll
-    for (int b = 0; b < NB; ++b) reg_fence(dzb[b]);
     reg_fence(dzs);
+    if constexpr (TRI) {
+#pragma unroll
+      for (int b = 0; b < NBM; ++b) { reg_fence(dzm[b]); reg_fence(djm[b]); }
+      reg_fence(djs);
+    } else {
+#pragma unroll
+      for (int b = 0; b < NB; ++b) reg_fence(dzb[b]);
+    }
   };
-  // the tile's dZ joins the fp32 total, and its stage goes back to the producer
+  // sum of a tile's merged accumulators for output element v: columns c (hi·hi) and c + DP (hi·lo) sit DP / 2 elements apart
+  auto merged = [&](const float (&acc)[TRI ? NBM : 1][DP], const float (&s)[DP / 2], int v) {
+    float t = s[v];
+#pragma unroll
+    for (int b = 0; b < NBM; ++b) t += acc[b][v] + acc[b][v + DP / 2];
+    return t;
+  };
+  // the tile's dZ_I joins the fp32 total, its dZ_J (above the diagonal block) goes to dz, and its stage goes back to the producer
   auto retire_dz = [&](int i) {
 #pragma unroll
     for (int v = 0; v < DP / 2; ++v) {
-      float t = dzs[v];
+      if constexpr (TRI) {
+        dzt[v] += merged(dzm, dzs, v);
+      } else {
+        float t = dzs[v];
 #pragma unroll
-      for (int b = 0; b < NB; ++b) t += dzb[b][v];
-      dzt[v] += t;
+        for (int b = 0; b < NB; ++b) t += dzb[b][v];
+        dzt[v] += t;
+      }
+    }
+    if constexpr (TRI) {
+      if (jt0 + i >= diag_end) {
+        const int ja = (jt0 + i) * JW + warp * 16 + (lane >> 2);
+        const bool vec = (p.d & 1) == 0 && (reinterpret_cast<uintptr_t>(p.dz) & 7) == 0;
+#pragma unroll
+        for (int v = 0; v < DP / 2; v += 2) {
+          const int row = ja + 8 * ((v >> 1) & 1);
+          const int col = 8 * (v >> 2) + 2 * (lane & 3);
+          const float x = merged(djm, djs, v), y = merged(djm, djs, v + 1);
+          if (row >= p.n || col >= p.d) continue;
+          float* dst = p.dz + (int64_t)row * p.d + col;
+          if (vec) {
+            atomicAdd(reinterpret_cast<float2*>(dst), make_float2(c2 * x, c2 * y));
+          } else {
+            atomicAdd(dst, c2 * x);
+            if (col + 1 < p.d) atomicAdd(dst + 1, c2 * y);
+          }
+        }
+      }
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(empty_bar + 8 * (i % STAGES));
   };
-  // wait for S of tile i, pass the turn on, then σ / softplus on the registers
+  // wait for S of tile i, pass the turn on, then σ / softplus on the registers; the triangle then writes Gᵀ for dZ_J
   auto elementwise = [&](int i) {
     wgmma_wait<0>();
     reg_fence(S);
     pass_turn();
-    const int jbase = (jt0 + i) * BT + 2 * (lane & 3);
-    const float l = full_rows && (jt0 + i + 1) * BT <= p.n ? sigmoid_softplus<false>(S, L, jbase, p.n, live_a, live_b)
+    const int jbase = (jt0 + i) * JW + 2 * (lane & 3);
+    const float l = full_rows && (jt0 + i + 1) * JW <= p.n ? sigmoid_softplus<false>(S, L, jbase, p.n, live_a, live_b)
                                                            : sigmoid_softplus<true>(S, L, jbase, p.n, live_a, live_b);
-    loss += (double)l;
+    if constexpr (TRI) {
+      loss += (jt0 + i >= diag_end ? 2.0 : 1.0) * (double)l;   // a tile above the diagonal block stands for its mirror too
+      // column jj of G is row jj of Gᵀ; the thread's rows r, r + 8 sit at K positions gt_pos(r), gt_pos(r) + 1
+      const uint32_t k = (uint32_t)gt_pos(warp * 16 + (lane >> 2));
+      const uint32_t base = (k >> 5) * (64 * 128);
+#pragma unroll
+      for (int c = 0; c < JW / 8; ++c) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const uint32_t o = base + sw128_offset32((uint32_t)(8 * c + 2 * (lane & 3) + e), k & 31);
+          sts_v2(smem_u32(gt_hi) + o, S[4 * c + e], S[4 * c + 2 + e]);
+          sts_v2(smem_u32(gt_lo) + o, L[4 * c + e], L[4 * c + 2 + e]);
+        }
+      }
+      fence_proxy_async();
+    } else {
+      loss += (double)l;
+    }
   };
 
   if (wg == 1) take_turn();
@@ -301,8 +448,8 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
   if (wg == 0) pass_turn();
 
   // ---- epilogue ----
-  const float c2 = 2.f * p.coef;
-  const bool atomic = gridDim.y > 1;
+  // The triangle's rows also receive dZ_J from the CTAs of the blocks above, so it always adds atomically.
+  const bool atomic = TRI || gridDim.y > 1;
 #pragma unroll
   for (int v = 0; v < DP / 2; ++v) {
     const int row = ra + 8 * ((v >> 1) & 1);
@@ -317,6 +464,18 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
   if (lane == 0) atomicAdd(p.loss_acc, loss * (double)p.coef);
 }
 
+template <int DP>
+__global__ void __launch_bounds__(THREADS, 1)
+gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
+  decoder_sweep<DP, false>(p);
+}
+
+template <int DP>
+__global__ void __launch_bounds__(THREADS, 1)
+gae_tri_tc_kernel(const __grid_constant__ Params p) {
+  decoder_sweep<DP, true>(p);
+}
+
 size_t workspace_bytes(int32_t n) { return (size_t)padded_n(n) / BT * (ZS_PLANES * ZS_BYTES + 2 * zt_bytes<MAX_D>()); }
 
 int super_blocks(int32_t n) { return (int)((padded_n(n) / BT + 1) / 2); }
@@ -327,9 +486,29 @@ bool eligible(int32_t n, int32_t d, int32_t n_rows) {
   return mode == 2 || (int64_t)n * n_rows >= (1ll << 22);
 }
 
+template <int DP, bool TRI>
+static int launch_sweep(const Params& p, int units, cudaStream_t st) {
+  // J step ranges: b2_set_tuning(B2_TUNE_GAE_SPLITS) when set, else enough to fill one wave of SMs
+  int splits = tuning(B2_TUNE_GAE_SPLITS);
+  if (splits <= 0) splits = ceil_div(sm_count(), units);
+  if (splits > p.n_jt) splits = p.n_jt;
+  if (splits < 1) splits = 1;
+  auto kernel = TRI ? gae_tri_tc_kernel<DP> : gae_allpairs_tc_kernel<DP>;
+  constexpr size_t smem = Tiles<DP, TRI>::SMEM;
+  static bool attr_set = false;
+  if (!attr_set) {
+    B2_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_set = true;
+  }
+  kernel<<<dim3((unsigned)units, (unsigned)splits), THREADS, smem, st>>>(p);
+  B2_CHECK_LAUNCH(TRI ? "gae_tri_tc_kernel" : "gae_allpairs_tc_kernel");
+  return B2_OK;
+}
+
+// tri: every row against every column by the triangle (units must be the nb row blocks)
 template <int DP>
-static int launch_dp(const float* z, int64_t ldz, int32_t n, int32_t d, Params p, int units, float* dz, double* loss_acc, void* ws,
-                     cudaStream_t st) {
+static int launch_dp(const float* z, int64_t ldz, int32_t n, int32_t d, Params p, int units, bool tri, float* dz, double* loss_acc,
+                     void* ws, cudaStream_t st) {
   const int64_t npad = padded_n(n);
   const int nb = (int)(npad / BT);
   uint8_t* w = reinterpret_cast<uint8_t*>(ws);
@@ -344,38 +523,32 @@ static int launch_dp(const float* z, int64_t ldz, int32_t n, int32_t d, Params p
   B2_CHECK_LAUNCH("gae_split_kernel");
   if (units <= 0) return B2_OK;
   p.z = z; p.ldz = ldz; p.zs_hi = zs_hi; p.zs_lo = zs_lo; p.zt_hi = zt_hi; p.zt_lo = zt_lo;
-  p.dz = dz; p.loss_acc = loss_acc; p.n = n; p.d = d; p.nb = nb; p.n_jt = nb;
-  // J step ranges: b2_set_tuning(B2_TUNE_GAE_SPLITS) when set, else enough to fill one wave of SMs
-  int splits = tuning(B2_TUNE_GAE_SPLITS);
-  if (splits <= 0) splits = ceil_div(sm_count(), units);
-  if (splits > nb) splits = nb;
-  if (splits < 1) splits = 1;
-  const size_t smem = ZS_PLANES * ZS_BYTES + STAGES * (ZS_PLANES * ZS_BYTES + 2 * zt_bytes<DP>()) + 16 * STAGES + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(gae_allpairs_tc_kernel<DP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
+  p.dz = dz; p.loss_acc = loss_acc; p.n = n; p.d = d; p.nb = nb;
+  if (tri) {
+    p.n_jt = ceil_div(n, Tiles<DP, true>::JW);   // 64-column tiles holding at least one column j < n
+    return launch_sweep<DP, true>(p, units, st);
   }
-  gae_allpairs_tc_kernel<DP><<<dim3((unsigned)units, (unsigned)splits), THREADS, smem, st>>>(p);
-  B2_CHECK_LAUNCH("gae_allpairs_tc_kernel");
-  return B2_OK;
+  p.n_jt = nb;
+  return launch_sweep<DP, false>(p, units, st);
 }
 
-static int launch_any(const float* z, int64_t ldz, int32_t n, int32_t d, const Params& p, int units, float* dz, double* loss_acc,
-                      void* ws, size_t ws_bytes, cudaStream_t st) {
+static int launch_any(const float* z, int64_t ldz, int32_t n, int32_t d, const Params& p, int units, bool tri, float* dz,
+                      double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st) {
   if (ws_bytes < workspace_bytes(n)) return B2_ERR_UNSUPPORTED;
-  if (d <= 8) return launch_dp<8>(z, ldz, n, d, p, units, dz, loss_acc, ws, st);
-  if (d <= 16) return launch_dp<16>(z, ldz, n, d, p, units, dz, loss_acc, ws, st);
-  return launch_dp<32>(z, ldz, n, d, p, units, dz, loss_acc, ws, st);
+  if (d <= 8) return launch_dp<8>(z, ldz, n, d, p, units, tri, dz, loss_acc, ws, st);
+  if (d <= 16) return launch_dp<16>(z, ldz, n, d, p, units, tri, dz, loss_acc, ws, st);
+  return launch_dp<32>(z, ldz, n, d, p, units, tri, dz, loss_acc, ws, st);
 }
 
-// rows [row_begin, row_begin + n_rows) against all n columns; adds into dz[n_rows, d] and loss_acc
+// rows [row_begin, row_begin + n_rows) against all n columns; adds into dz[n_rows, d] and loss_acc.  The call over all rows
+// uses the symmetry of S (triangle); a row subset sweeps every column.
 int launch(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t row_begin, int32_t n_rows, float coef, float* dz,
            double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st) {
   Params p;
   memset(&p, 0, sizeof(p));
   p.coef = coef; p.row_begin = row_begin; p.row_end = row_begin + n_rows; p.sym = 0;
-  return launch_any(z, ldz, n, d, p, ceil_div(n_rows, BT), dz, loss_acc, ws, ws_bytes, st);
+  const bool tri = row_begin == 0 && n_rows == n;
+  return launch_any(z, ldz, n, d, p, ceil_div(n_rows, BT), tri, dz, loss_acc, ws, ws_bytes, st);
 }
 
 // super-blocks [sb_begin, sb_end) against all n columns; adds into dz[n, d] (the rows of those blocks) and loss_acc
@@ -384,7 +557,7 @@ int launch_super_blocks(const float* z, int64_t ldz, int32_t n, int32_t d, int32
   Params p;
   memset(&p, 0, sizeof(p));
   p.coef = coef; p.sym = 1; p.sb_begin = sb_begin;
-  return launch_any(z, ldz, n, d, p, 2 * (sb_end - sb_begin), dz, loss_acc, ws, ws_bytes, st);
+  return launch_any(z, ldz, n, d, p, 2 * (sb_end - sb_begin), false, dz, loss_acc, ws, ws_bytes, st);
 }
 
 }  // namespace gtc

@@ -292,17 +292,24 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   double loss = 0.0;
 
   // Ping-pong: the two warpgroups take turns on the tensor cores.  A turn is the dZ product of the previous tile followed by the
-  // S product of the next one, each issued as one batch with one commit and one wait.  The turn passes on once both are done
-  // (named barrier 2 + wg means "wg may issue"), and the warpgroup works through σ / softplus of its S while the other one's
-  // products run.  Warpgroup 0 takes the first turn.  Each warpgroup takes nt + 1 turns and passes nt of them on; warpgroup 0
-  // passes its last one as well, so that every bar.arrive meets one bar.sync.  The bar.sync of a turn also orders this
-  // warpgroup's Gᵀ stores before the dZ_J product that reads them.
+  // S product of the next one, each issued as one batch with one commit (named barrier 2 + wg means "wg may issue"), and the
+  // warpgroup works through σ / softplus of its S while the other one's products run.  Warpgroup 0 takes the first turn.  Each
+  // warpgroup takes nt + 1 turns and passes nt of them on; warpgroup 0 passes its last one as well, so that every bar.arrive
+  // meets one bar.sync.  The bar.sync of a turn also orders this warpgroup's Gᵀ stores before the dZ_J product that reads them.
+  //   Full sweep: the dZ batch is waited for before S is issued into the same registers, and the turn passes on once S is done.
+  //   Triangle at DP = 16 and 32: the same, but the turn passes on as soon as S is committed, so that the other warpgroup's
+  //     dZ batch queues behind it instead of waiting for it to finish.
+  //   Triangle at DP = 8 (OVERLAP): S alternates between two accumulators, so the dZ batch of tile i − 1 (A = the previous S
+  //     and L) and the S batch of tile i go out back to back and the turn passes on once both are committed; the tensor pipe
+  //     does not drain within a turn.  wait<1> then retires dZ while S still runs.  At DP = 16 and 32 the second accumulator
+  //     makes ptxas spill in the consumer loop, so those keep one.
+  constexpr bool OVERLAP = TRI && DP <= 8;
   float S[JW / 2], L[JW / 2];   // S: accumulator of S, then the hi part of G; L: the lo part of G
   auto take_turn = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(2 + wg), "n"(CONSUMERS) : "memory"); };
   auto pass_turn = [&]() { asm volatile("bar.arrive %0, %1;" ::"r"(3 - wg), "n"(CONSUMERS) : "memory"); };
 
-  // S = Z_I · Z_Jᵀ of tile i: one batch of 3·DP/8 products, committed (the caller waits)
-  auto issue_s = [&](int i) {
+  // S = Z_I · Z_Jᵀ of tile i into the accumulator S: one batch of 3·DP/8 products, committed (the caller waits)
+  auto issue_s = [&](int i, float (&S)[JW / 2]) {
     const int s = i % STAGES;
     mbar_wait(full_bar + 8 * s, (uint32_t)((i / STAGES) & 1));
     const uint32_t bs_hi = smem_u32(ring + s * T::STAGE), bs_lo = bs_hi + T::JS;
@@ -317,8 +324,9 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
     wgmma_commit();
   };
   // dZ_I += G · Z_J of tile i with A = (S, L) from the registers, and in the triangle dZ_J += Gᵀ · Z_I (on the diagonal block
-  // it is computed and dropped); one batch, waited for (S is overwritten next).  Full sweep: 3·16 products; triangle: 2·8 + 2·8.
-  auto run_dz = [&](int i) {
+  // it is computed and dropped); one batch, committed (the caller waits, then dz_fence).  Full sweep: 3·16 products; triangle:
+  // 2·8 + 2·8.
+  auto issue_dz = [&](int i, float (&S)[JW / 2]) {
     const uint32_t bt_hi = smem_u32(ring + (i % STAGES) * T::STAGE) + 2 * T::JS, bt_lo = bt_hi + T::JT;
     wgmma_fence();
 #pragma unroll
@@ -350,7 +358,8 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
       }
     }
     wgmma_commit();
-    wgmma_wait<0>();
+  };
+  auto dz_fence = [&]() {
     reg_fence(dzs);
     if constexpr (TRI) {
 #pragma unroll
@@ -404,11 +413,8 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
     __syncwarp();
     if (lane == 0) mbar_arrive(empty_bar + 8 * (i % STAGES));
   };
-  // wait for S of tile i, pass the turn on, then σ / softplus on the registers; the triangle then writes Gᵀ for dZ_J
-  auto elementwise = [&](int i) {
-    wgmma_wait<0>();
-    reg_fence(S);
-    pass_turn();
+  // σ / softplus of tile i on the registers once its S is done; the triangle then writes Gᵀ for dZ_J
+  auto elementwise = [&](int i, float (&S)[JW / 2]) {
     const int jbase = (jt0 + i) * JW + 2 * (lane & 3);
     const float l = full_rows && (jt0 + i + 1) * JW <= p.n ? sigmoid_softplus<false>(S, L, jbase, p.n, live_a, live_b)
                                                            : sigmoid_softplus<true>(S, L, jbase, p.n, live_a, live_b);
@@ -432,20 +438,78 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
     }
   };
 
-  if (wg == 1) take_turn();
-  issue_s(0);
-  elementwise(0);
-  for (int i = 1; i < nt; ++i) {
+  if constexpr (OVERLAP) {
+    float S2[JW / 2];
+    // the turn of tile i ≥ 1: dZ of tile i − 1 from (Sp, L), then S of tile i into Sn
+    auto turn = [&](int i, float (&Sp)[JW / 2], float (&Sn)[JW / 2]) {
+      take_turn();
+      issue_dz(i - 1, Sp);
+      issue_s(i, Sn);
+      pass_turn();
+      wgmma_wait<1>();     // dZ is done, S may still run
+      dz_fence();
+      retire_dz(i - 1);
+      wgmma_wait<0>();
+      reg_fence(Sn);
+      elementwise(i, Sn);
+    };
+    // the last turn: dZ of tile nt − 1 from (Sp, L)
+    auto last = [&](float (&Sp)[JW / 2]) {
+      take_turn();
+      issue_dz(nt - 1, Sp);
+      if (wg == 0) pass_turn();
+      wgmma_wait<0>();
+      dz_fence();
+      retire_dz(nt - 1);
+    };
+    if (wg == 1) take_turn();
+    issue_s(0, S);
+    pass_turn();
+    wgmma_wait<0>();
+    reg_fence(S);
+    elementwise(0, S);
+    // unrolled by two, so that which accumulator each batch reads and writes is known at compile time (ptxas serialises
+    // wgmmas whose register operands it cannot tell apart)
+    for (int i = 1;; i += 2) {
+      if (i == nt) { last(S); break; }
+      turn(i, S, S2);
+      if (i + 1 == nt) { last(S2); break; }
+      turn(i + 1, S2, S);
+    }
+  } else {
+    auto run_dz = [&](int i) {
+      issue_dz(i, S);
+      wgmma_wait<0>();
+      dz_fence();
+    };
+    // The triangle passes the turn on as soon as S is committed, so that the other warpgroup's dZ batch queues behind it; the
+    // full sweep once S is done.
+    auto start_s = [&](int i) {
+      issue_s(i, S);
+      if constexpr (TRI) pass_turn();
+    };
+    // wait for S of tile i, then σ / softplus
+    auto finish_s = [&](int i) {
+      wgmma_wait<0>();
+      reg_fence(S);
+      if constexpr (!TRI) pass_turn();
+      elementwise(i, S);
+    };
+    if (wg == 1) take_turn();
+    start_s(0);
+    finish_s(0);
+    for (int i = 1; i < nt; ++i) {
+      take_turn();
+      run_dz(i - 1);
+      start_s(i);          // S runs while the previous tile's dZ is summed
+      retire_dz(i - 1);
+      finish_s(i);
+    }
     take_turn();
-    run_dz(i - 1);
-    issue_s(i);          // S runs while the previous tile's dZ is summed
-    retire_dz(i - 1);
-    elementwise(i);
+    run_dz(nt - 1);
+    retire_dz(nt - 1);
+    if (wg == 0) pass_turn();
   }
-  take_turn();
-  run_dz(nt - 1);
-  retire_dz(nt - 1);
-  if (wg == 0) pass_turn();
 
   // ---- epilogue ----
   // The triangle's rows also receive dZ_J from the CTAs of the blocks above, so it always adds atomically.

@@ -544,9 +544,9 @@ size_t workspace_bytes(int32_t n) { return (size_t)padded_n(n) / BT * (ZS_PLANES
 
 int super_blocks(int32_t n) { return (int)((padded_n(n) / BT + 1) / 2); }
 
-bool eligible(int32_t n, int32_t d, int32_t n_rows) {
+bool eligible(int32_t n, int32_t d, int32_t n_rows, size_t ws_bytes) {
   const int mode = path_mode(B2_PATH_GAE_DECODER);           // 0 auto · 1 CUDA cores · 2 this kernel
-  if (d < 1 || d > MAX_D || mode == 1) return false;
+  if (d < 1 || d > MAX_D || mode == 1 || ws_bytes < workspace_bytes(n)) return false;
   return mode == 2 || (int64_t)n * n_rows >= (1ll << 22);
 }
 
@@ -569,59 +569,51 @@ static int launch_sweep(const Params& p, int units, cudaStream_t st) {
   return B2_OK;
 }
 
-// tri: every row against every column by the triangle (units must be the nb row blocks)
+// Splits z into the workspace planes, then sweeps `units` work units (none: the split only).  tri: every row against every
+// column by the triangle (units must be the nb row blocks).
 template <int DP>
-static int launch_dp(const float* z, int64_t ldz, int32_t n, int32_t d, Params p, int units, bool tri, float* dz, double* loss_acc,
-                     void* ws, cudaStream_t st) {
-  const int64_t npad = padded_n(n);
-  const int nb = (int)(npad / BT);
-  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
-  uint8_t* zs_hi = w;
-  uint8_t* zs_lo = zs_hi + (size_t)nb * ZS_BYTES;
-  uint8_t* zt_hi = zs_lo + (size_t)nb * ZS_BYTES;
-  uint8_t* zt_lo = zt_hi + (size_t)nb * zt_bytes<DP>();
+static int launch_dp(Params p, int units, bool tri, void* ws, cudaStream_t st) {
+  const int64_t npad = padded_n(p.n);
+  p.nb = (int)(npad / BT);
+  uint8_t* zs_hi = reinterpret_cast<uint8_t*>(ws);
+  uint8_t* zs_lo = zs_hi + (size_t)p.nb * ZS_BYTES;
+  uint8_t* zt_hi = zs_lo + (size_t)p.nb * ZS_BYTES;
+  uint8_t* zt_lo = zt_hi + (size_t)p.nb * zt_bytes<DP>();
   int64_t blocks = ceil_div<int64_t>(npad * DP, 256);
   const int64_t cap = (int64_t)sm_count() * 16;
   if (blocks > cap) blocks = cap;
-  gae_split_kernel<DP><<<(unsigned)blocks, 256, 0, st>>>(z, ldz, n, d, npad, zs_hi, zs_lo, zt_hi, zt_lo);
+  gae_split_kernel<DP><<<(unsigned)blocks, 256, 0, st>>>(p.z, p.ldz, p.n, p.d, npad, zs_hi, zs_lo, zt_hi, zt_lo);
   B2_CHECK_LAUNCH("gae_split_kernel");
   if (units <= 0) return B2_OK;
-  p.z = z; p.ldz = ldz; p.zs_hi = zs_hi; p.zs_lo = zs_lo; p.zt_hi = zt_hi; p.zt_lo = zt_lo;
-  p.dz = dz; p.loss_acc = loss_acc; p.n = n; p.d = d; p.nb = nb;
+  p.zs_hi = zs_hi; p.zs_lo = zs_lo; p.zt_hi = zt_hi; p.zt_lo = zt_lo;
   if (tri) {
-    p.n_jt = ceil_div(n, Tiles<DP, true>::JW);   // 64-column tiles holding at least one column j < n
+    p.n_jt = ceil_div(p.n, Tiles<DP, true>::JW);   // 64-column tiles holding at least one column j < n
     return launch_sweep<DP, true>(p, units, st);
   }
-  p.n_jt = nb;
+  p.n_jt = p.nb;
   return launch_sweep<DP, false>(p, units, st);
 }
 
-static int launch_any(const float* z, int64_t ldz, int32_t n, int32_t d, const Params& p, int units, bool tri, float* dz,
-                      double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st) {
-  if (ws_bytes < workspace_bytes(n)) return B2_ERR_UNSUPPORTED;
-  if (d <= 8) return launch_dp<8>(z, ldz, n, d, p, units, tri, dz, loss_acc, ws, st);
-  if (d <= 16) return launch_dp<16>(z, ldz, n, d, p, units, tri, dz, loss_acc, ws, st);
-  return launch_dp<32>(z, ldz, n, d, p, units, tri, dz, loss_acc, ws, st);
-}
-
-// rows [row_begin, row_begin + n_rows) against all n columns; adds into dz[n_rows, d] and loss_acc.  The call over all rows
-// uses the symmetry of S (triangle); a row subset sweeps every column.
-int launch(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t row_begin, int32_t n_rows, float coef, float* dz,
-           double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st) {
+// Adds the all-pairs part into dz and loss_acc; ws holds workspace_bytes(n) bytes.  Row form (sym = false): rows [begin, end)
+// against all n columns, dz[end - begin, d]; the call over all rows uses the symmetry of S (triangle), a row subset sweeps every
+// column.  Pair-sharded form (sym = true): super-blocks [begin, end) against all n columns, dz[n, d] (the rows of those blocks).
+int launch(const float* z, int64_t ldz, int32_t n, int32_t d, bool sym, int32_t begin, int32_t end, float coef, float* dz,
+           double* loss_acc, void* ws, cudaStream_t st) {
   Params p;
   memset(&p, 0, sizeof(p));
-  p.coef = coef; p.row_begin = row_begin; p.row_end = row_begin + n_rows; p.sym = 0;
-  const bool tri = row_begin == 0 && n_rows == n;
-  return launch_any(z, ldz, n, d, p, ceil_div(n_rows, BT), tri, dz, loss_acc, ws, ws_bytes, st);
-}
-
-// super-blocks [sb_begin, sb_end) against all n columns; adds into dz[n, d] (the rows of those blocks) and loss_acc
-int launch_super_blocks(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t sb_begin, int32_t sb_end, float coef, float* dz,
-                        double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st) {
-  Params p;
-  memset(&p, 0, sizeof(p));
-  p.coef = coef; p.sym = 1; p.sb_begin = sb_begin;
-  return launch_any(z, ldz, n, d, p, 2 * (sb_end - sb_begin), false, dz, loss_acc, ws, ws_bytes, st);
+  p.z = z; p.ldz = ldz; p.n = n; p.d = d; p.coef = coef; p.dz = dz; p.loss_acc = loss_acc; p.sym = sym;
+  int units;
+  if (sym) {
+    p.sb_begin = begin;
+    units = 2 * (end - begin);
+  } else {
+    p.row_begin = begin; p.row_end = end;
+    units = ceil_div(end - begin, BT);
+  }
+  const bool tri = !sym && begin == 0 && end == n;
+  if (d <= 8) return launch_dp<8>(p, units, tri, ws, st);
+  if (d <= 16) return launch_dp<16>(p, units, tri, ws, st);
+  return launch_dp<32>(p, units, tri, ws, st);
 }
 
 }  // namespace gtc

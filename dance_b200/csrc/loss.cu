@@ -5,6 +5,8 @@
 //     dense label matrix (scgnn2.py:557) are never materialised.
 #include "common.cuh"
 
+#include <type_traits>
+
 namespace b2 {
 
 // ---------------------------------------------------------------------------
@@ -240,12 +242,43 @@ __global__ void gae_finish_kernel(const double* acc, float* loss_out) { loss_out
 namespace gtc {   // gae_tc.cu: wgmma version of the all-pairs part
 size_t workspace_bytes(int32_t n);
 int super_blocks(int32_t n);
-bool eligible(int32_t n, int32_t d, int32_t n_rows);
-int launch(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t row_begin, int32_t n_rows, float coef, float* dz,
-           double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st);
-int launch_super_blocks(const float* z, int64_t ldz, int32_t n, int32_t d, int32_t sb_begin, int32_t sb_end, float coef, float* dz,
-                        double* loss_acc, void* ws, size_t ws_bytes, cudaStream_t st);
+bool eligible(int32_t n, int32_t d, int32_t n_rows, size_t ws_bytes);
+int launch(const float* z, int64_t ldz, int32_t n, int32_t d, bool sym, int32_t begin, int32_t end, float coef, float* dz,
+           double* loss_acc, void* ws, cudaStream_t st);
 }  // namespace gtc
+
+// The workspace starts with the loss accumulator; the tensor-core path's planes of z follow it.
+constexpr size_t GAE_ACC_BYTES = 256;
+
+// The embedding sizes the CUDA-core kernels are built for: f(std::integral_constant<int, D>()).  The caller has checked d.
+template <class F>
+static int with_d(int32_t d, F f) {
+  switch (d) {
+    case 8: return f(std::integral_constant<int, 8>());
+    case 16: return f(std::integral_constant<int, 16>());
+    case 32: return f(std::integral_constant<int, 32>());
+    default: return f(std::integral_constant<int, 64>());
+  }
+}
+
+template <int D>
+static int launch_gae_allpairs(const float* z, int64_t ldz, int32_t n, int32_t row_begin, int32_t n_rows, float coef, float* dz,
+                               double* acc, cudaStream_t st) {
+  if (n_rows == 0) return B2_OK;   // nothing to sweep, and no row blocks to spread the j range over
+  const int row_blocks = ceil_div(n_rows, GaeCfg<D>::ROWS);
+  // split the j range so that small graphs still fill the machine
+  int j_splits = 1;
+  const int target = sm_count() * 4;
+  if (row_blocks < target) j_splits = min(ceil_div(target, row_blocks), ceil_div(n, GL_JT));
+  if (j_splits < 1) j_splits = 1;
+  if (j_splits > 65535) j_splits = 65535;
+  int j_chunk = ceil_div(ceil_div(n, j_splits), GL_JT) * GL_JT;
+  j_splits = ceil_div(n, j_chunk);
+  dim3 grid(row_blocks, j_splits);
+  gae_allpairs_kernel<D><<<grid, GL_THREADS, 0, st>>>(z, ldz, n, row_begin, n_rows, j_chunk, coef, dz, acc);
+  B2_CHECK_LAUNCH("gae_allpairs_kernel");
+  return B2_OK;
+}
 
 template <int D>
 static int launch_gae_edges(const float* z, int64_t ldz, const int32_t* rp, const int32_t* ci, int32_t row_begin, int32_t n_rows,
@@ -259,24 +292,63 @@ static int launch_gae_edges(const float* z, int64_t ldz, const int32_t* rp, cons
   return B2_OK;
 }
 
-template <int D>
-static int launch_gae(const float* z, int64_t ldz, const int32_t* rp, const int32_t* ci, int32_t n, int32_t row_begin,
-                      int32_t n_rows, float coef, float pw, int use_pw, float* dz, double* acc, bool skip_allpairs,
-                      cudaStream_t st) {
-  if (skip_allpairs) return launch_gae_edges<D>(z, ldz, rp, ci, row_begin, n_rows, coef, pw, use_pw, dz, acc, st);
-  const int row_blocks = ceil_div(n_rows, GaeCfg<D>::ROWS);
-  // split the j range so that small graphs still fill the machine
-  int j_splits = 1;
-  const int target = sm_count() * 4;
-  if (row_blocks < target) j_splits = min(ceil_div(target, row_blocks), ceil_div(n, GL_JT));
-  if (j_splits < 1) j_splits = 1;
-  if (j_splits > 65535) j_splits = 65535;
-  int j_chunk = ceil_div(ceil_div(n, j_splits), GL_JT) * GL_JT;
-  j_splits = ceil_div(n, j_chunk);
-  dim3 grid(row_blocks, j_splits);
-  gae_allpairs_kernel<D><<<grid, GL_THREADS, 0, st>>>(z, ldz, n, row_begin, n_rows, j_chunk, coef, dz, acc);
-  B2_CHECK_LAUNCH("gae_allpairs_kernel");
-  return launch_gae_edges<D>(z, ldz, rp, ci, row_begin, n_rows, coef, pw, use_pw, dz, acc, st);
+// The all-pairs part of a call.  Row form: rows [row_begin, row_begin + n_rows) against every column, dz holds those rows.
+// Pair-sharded form (sym): super-blocks [sb_begin, sb_end) on the tensor cores, dz holds all n rows.
+struct AllPairs {
+  bool sym;
+  int32_t sb_begin, sb_end;
+};
+
+// Both decoder entry points; fn names the one called in error messages.
+static int gae_loss_grad(const char* fn, const AllPairs& ap, const float* z, int64_t ldz, const float* mu, const float* logvar,
+                         int64_t ldm, const int32_t* lab_rowptr, const int32_t* lab_colidx, int32_t n, int32_t d, int32_t row_begin,
+                         int32_t n_rows, float norm, float pos_weight, int use_pos_weight, float* dz, float* dmu, float* dlogvar,
+                         int64_t ldd, float* loss_out, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+  B2_REQUIRE(z && lab_rowptr && lab_colidx && dz && loss_out, "%s: null pointer", fn);
+  B2_REQUIRE(n > 0 && d > 0 && ldz >= d, "%s: bad shape", fn);
+  B2_REQUIRE(row_begin >= 0 && n_rows >= 0 && row_begin + n_rows <= n, "%s: bad row range", fn);
+  B2_REQUIRE((mu == nullptr) == (logvar == nullptr), "%s: mu/logvar must both be given or both NULL", fn);
+  if (mu) B2_REQUIRE(dmu && dlogvar && ldm >= d && ldd >= d, "%s: dmu/dlogvar required with mu/logvar", fn);
+  if (ap.sym) {
+    B2_REQUIRE(d <= 16, "%s: bad shape (d <= 16)", fn);
+    B2_REQUIRE(ap.sb_begin >= 0 && ap.sb_begin <= ap.sb_end && ap.sb_end <= gtc::super_blocks(n), "%s: bad super-block range", fn);
+  }
+  B2_REQUIRE(workspace && workspace_bytes >= GAE_ACC_BYTES + (ap.sym ? gtc::workspace_bytes(n) : 0), "%s: workspace too small", fn);
+  if (d != 8 && d != 16 && d != 32 && d != 64) {
+    set_error("%s: embedding size %d unsupported (%s)", fn, d, ap.sym ? "8, 16" : "8, 16, 32, 64");
+    return B2_ERR_UNSUPPORTED;
+  }
+
+  double* acc = reinterpret_cast<double*>(workspace);
+  void* tc_ws = reinterpret_cast<char*>(workspace) + GAE_ACC_BYTES;
+  float* dz_rows = ap.sym ? dz + (size_t)row_begin * d : dz;   // where this call's label terms go
+  B2_CHECK_CUDA(cudaMemsetAsync(acc, 0, sizeof(double), st));
+  B2_CHECK_CUDA(cudaMemsetAsync(dz, 0, sizeof(float) * (size_t)(ap.sym ? n : n_rows) * d, st));
+  const float coef = (use_pos_weight ? norm : 1.f) / ((float)n * (float)n);
+  // the all-pairs part: the pair-sharded form and large problems on the tensor cores (gae_tc.cu), small graphs on the CUDA cores
+  int rc;
+  if (ap.sym)
+    rc = gtc::launch(z, ldz, n, d, true, ap.sb_begin, ap.sb_end, coef, dz, acc, tc_ws, st);
+  else if (gtc::eligible(n, d, n_rows, workspace_bytes - GAE_ACC_BYTES))
+    rc = gtc::launch(z, ldz, n, d, false, row_begin, row_begin + n_rows, coef, dz, acc, tc_ws, st);
+  else
+    rc = with_d(d, [&](auto D) { return launch_gae_allpairs<D>(z, ldz, n, row_begin, n_rows, coef, dz, acc, st); });
+  if (rc != B2_OK) return rc;
+  rc = with_d(d, [&](auto D) {
+    return launch_gae_edges<D>(z, ldz, lab_rowptr, lab_colidx, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz_rows, acc, st);
+  });
+  if (rc != B2_OK) return rc;
+  if (mu) {
+    int64_t blocks = ceil_div<int64_t>((int64_t)n_rows * d, 256);
+    if (blocks < 1) blocks = 1;
+    const int64_t cap = (int64_t)sm_count() * 16;
+    if (blocks > cap) blocks = cap;
+    gae_kld_kernel<<<(unsigned)blocks, 256, 0, st>>>(mu, logvar, ldm, n, n_rows, d, dmu, dlogvar, ldd, acc);
+    B2_CHECK_LAUNCH("gae_kld_kernel");
+  }
+  gae_finish_kernel<<<1, 1, 0, st>>>(acc, loss_out);
+  B2_CHECK_LAUNCH("gae_finish_kernel");
+  return B2_OK;
 }
 
 }  // namespace b2
@@ -300,8 +372,7 @@ extern "C" int b2_mse_sum_loss_grad_f32(const float* recon, const float* target,
 }
 
 extern "C" size_t b2_gae_loss_workspace_bytes(int32_t n, int32_t d) {
-  // 256 B of accumulators + the hi/lo tf32 planes of z for the tensor-core path
-  return 256 + (d <= 32 ? gtc::workspace_bytes(n) : 0);
+  return GAE_ACC_BYTES + (d <= 32 ? gtc::workspace_bytes(n) : 0);
 }
 
 extern "C" int b2_gae_loss_grad_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
@@ -309,48 +380,10 @@ extern "C" int b2_gae_loss_grad_f32(const float* z, int64_t ldz, const float* mu
                                     int32_t row_begin, int32_t n_rows, float norm, float pos_weight, int use_pos_weight, float* dz, float* dmu,
                                     float* dlogvar, int64_t ldd, float* loss_out, void* workspace,
                                     size_t workspace_bytes, void* stream) {
-  B2_REQUIRE(z && lab_rowptr && lab_colidx && dz && loss_out, "b2_gae_loss_grad_f32: null pointer");
-  B2_REQUIRE(n > 0 && d > 0 && ldz >= d, "b2_gae_loss_grad_f32: bad shape");
-  B2_REQUIRE(row_begin >= 0 && n_rows >= 0 && row_begin + n_rows <= n, "b2_gae_loss_grad_f32: bad row range");
-  B2_REQUIRE(workspace && workspace_bytes >= 256, "b2_gae_loss_grad_f32: workspace too small");
-  B2_REQUIRE((mu == nullptr) == (logvar == nullptr), "b2_gae_loss_grad_f32: mu/logvar must both be given or both NULL");
-  if (mu) B2_REQUIRE(dmu && dlogvar && ldm >= d && ldd >= d, "b2_gae_loss_grad_f32: dmu/dlogvar required with mu/logvar");
-  cudaStream_t st = as_stream(stream);
-  double* acc = reinterpret_cast<double*>(workspace);
-  B2_CHECK_CUDA(cudaMemsetAsync(acc, 0, sizeof(double), st));
-  B2_CHECK_CUDA(cudaMemsetAsync(dz, 0, sizeof(float) * (size_t)n_rows * d, st));
-  const float coef = (use_pos_weight ? norm : 1.f) / ((float)n * (float)n);
-  int rc;
-  // large problems: the all-pairs part runs on the tensor cores (gae_tc.cu); the CUDA-core kernel serves small graphs
-  bool tc_done = false;
-  if (gtc::eligible(n, d, n_rows) && workspace_bytes >= 256 + gtc::workspace_bytes(n)) {
-    rc = gtc::launch(z, ldz, n, d, row_begin, n_rows, coef, dz, acc, reinterpret_cast<char*>(workspace) + 256, workspace_bytes - 256, st);
-    if (rc == B2_OK) tc_done = true;
-    else if (rc != B2_ERR_UNSUPPORTED) return rc;
-  }
-  switch (d) {
-    case 8: rc = launch_gae<8>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st); break;
-    case 16: rc = launch_gae<16>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st); break;
-    case 32: rc = launch_gae<32>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st); break;
-    case 64: rc = launch_gae<64>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz, acc, tc_done, st); break;
-    default:
-      set_error("b2_gae_loss_grad_f32: embedding size %d unsupported (8, 16, 32, 64)", d);
-      return B2_ERR_UNSUPPORTED;
-  }
-  if (rc != B2_OK) return rc;
-  if (mu) {
-    int64_t blocks = ceil_div<int64_t>((int64_t)n_rows * d, 256);
-    if (blocks < 1) blocks = 1;
-    const int64_t cap = (int64_t)sm_count() * 16;
-    if (blocks > cap) blocks = cap;
-    gae_kld_kernel<<<(unsigned)blocks, 256, 0, st>>>(mu, logvar, ldm, n, n_rows, d, dmu, dlogvar, ldd, acc);
-    B2_CHECK_LAUNCH("gae_kld_kernel");
-  }
-  gae_finish_kernel<<<1, 1, 0, st>>>(acc, loss_out);
-  B2_CHECK_LAUNCH("gae_finish_kernel");
-  return B2_OK;
+  return gae_loss_grad("b2_gae_loss_grad_f32", AllPairs{false, 0, 0}, z, ldz, mu, logvar, ldm, lab_rowptr, lab_colidx, n, d, row_begin,
+                       n_rows, norm, pos_weight, use_pos_weight, dz, dmu, dlogvar, ldd, loss_out, workspace, workspace_bytes,
+                       as_stream(stream));
 }
-
 
 // Pair-sharded form of b2_gae_loss_grad_f32 for multi-GPU runs.  Rank r evaluates the all-pairs part of the super-blocks
 // [sb_begin, sb_end) (b2_gae_sym_super_blocks(n) in total, equal work each: super-block s = the 128-row blocks s and nb−1−s)
@@ -365,42 +398,7 @@ extern "C" int b2_gae_loss_grad_sym_f32(const float* z, int64_t ldz, const float
                                         int32_t sb_begin, int32_t sb_end, int32_t row_begin, int32_t n_rows, float norm, float pos_weight,
                                         int use_pos_weight, float* dz_full, float* dmu, float* dlogvar, int64_t ldd, float* loss_out,
                                         void* workspace, size_t workspace_bytes, void* stream) {
-  B2_REQUIRE(z && lab_rowptr && lab_colidx && dz_full && loss_out, "b2_gae_loss_grad_sym_f32: null pointer");
-  B2_REQUIRE(n > 0 && d > 0 && d <= 16 && ldz >= d, "b2_gae_loss_grad_sym_f32: bad shape (d <= 16)");
-  B2_REQUIRE(row_begin >= 0 && n_rows >= 0 && row_begin + n_rows <= n, "b2_gae_loss_grad_sym_f32: bad row range");
-  B2_REQUIRE(sb_begin >= 0 && sb_begin <= sb_end && sb_end <= gtc::super_blocks(n), "b2_gae_loss_grad_sym_f32: bad super-block range");
-  B2_REQUIRE(workspace && workspace_bytes >= 256 + gtc::workspace_bytes(n), "b2_gae_loss_grad_sym_f32: workspace too small");
-  B2_REQUIRE((mu == nullptr) == (logvar == nullptr), "b2_gae_loss_grad_sym_f32: mu/logvar must both be given or both NULL");
-  if (mu) B2_REQUIRE(dmu && dlogvar && ldm >= d && ldd >= d, "b2_gae_loss_grad_sym_f32: dmu/dlogvar required with mu/logvar");
-  cudaStream_t st = as_stream(stream);
-  double* acc = reinterpret_cast<double*>(workspace);
-  B2_CHECK_CUDA(cudaMemsetAsync(acc, 0, sizeof(double), st));
-  B2_CHECK_CUDA(cudaMemsetAsync(dz_full, 0, sizeof(float) * (size_t)n * d, st));
-  const float coef = (use_pos_weight ? norm : 1.f) / ((float)n * (float)n);
-  int rc = gtc::launch_super_blocks(z, ldz, n, d, sb_begin, sb_end, coef, dz_full, acc, reinterpret_cast<char*>(workspace) + 256,
-                                    workspace_bytes - 256, st);
-  if (rc != B2_OK) {
-    if (rc == B2_ERR_UNSUPPORTED) set_error("b2_gae_loss_grad_sym_f32: workspace too small");
-    return rc;
-  }
-  float* dz_rows = dz_full + (size_t)row_begin * d;
-  switch (d) {
-    case 8: rc = launch_gae<8>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz_rows, acc, true, st); break;
-    case 16: rc = launch_gae<16>(z, ldz, lab_rowptr, lab_colidx, n, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz_rows, acc, true, st); break;
-    default:
-      set_error("b2_gae_loss_grad_sym_f32: embedding size %d unsupported (8, 16)", d);
-      return B2_ERR_UNSUPPORTED;
-  }
-  if (rc != B2_OK) return rc;
-  if (mu) {
-    int64_t blocks = ceil_div<int64_t>((int64_t)n_rows * d, 256);
-    if (blocks < 1) blocks = 1;
-    const int64_t cap = (int64_t)sm_count() * 16;
-    if (blocks > cap) blocks = cap;
-    gae_kld_kernel<<<(unsigned)blocks, 256, 0, st>>>(mu, logvar, ldm, n, n_rows, d, dmu, dlogvar, ldd, acc);
-    B2_CHECK_LAUNCH("gae_kld_kernel");
-  }
-  gae_finish_kernel<<<1, 1, 0, st>>>(acc, loss_out);
-  B2_CHECK_LAUNCH("gae_finish_kernel");
-  return B2_OK;
+  return gae_loss_grad("b2_gae_loss_grad_sym_f32", AllPairs{true, sb_begin, sb_end}, z, ldz, mu, logvar, ldm, lab_rowptr, lab_colidx,
+                       n, d, row_begin, n_rows, norm, pos_weight, use_pos_weight, dz_full, dmu, dlogvar, ldd, loss_out, workspace,
+                       workspace_bytes, as_stream(stream));
 }

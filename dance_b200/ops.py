@@ -320,42 +320,46 @@ def mse_sum_loss_grad(recon, target, ltmg_regu=None, regu_strength=0.0, relu_mas
     return loss_out, grad
 
 
-def gae_loss_grad(z, labels: CSR, norm: float, pos_weight: float, mu=None, logvar=None, use_pos_weight=True,
-                  dz=None, dmu=None, dlogvar=None, loss=None, row_begin: int = 0, n_rows: Optional[int] = None):
-    """Matrix-free Graph-AE loss: returns (loss[1], dz, dmu, dlogvar).
-
-    ``dmu``/``dlogvar`` may be column slices of one packed [n, 2d] buffer (shared leading dimension).
-    """
+def _gae_prepare(what, z, labels: CSR, n_rows, mu, logvar, dmu, dlogvar, loss):
+    """Checks and buffers both decoder calls share; returns (n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, workspace)."""
     _chk(z, torch.float32, "z", 2)
     n, d = z.shape
     n_rows = n if n_rows is None else n_rows
     if labels.shape[0] != n_rows or labels.shape[1] != n:
-        raise B2Error(f"gae_loss_grad: labels must be [{n_rows}, {n}] (rows of this shard x all columns), got {tuple(labels.shape)}")
-    if dz is None:
-        dz = torch.empty((n_rows, d), dtype=torch.float32, device=z.device)
-    else:
-        _chk(dz, torch.float32, "dz", 2)
-        if tuple(dz.shape) != (n_rows, d) or not dz.is_contiguous():
-            raise B2Error(f"gae_loss_grad: dz must be a contiguous [{n_rows}, {d}] buffer, got {tuple(dz.shape)} strides {dz.stride()}")
+        raise B2Error(f"{what}: labels must be [{n_rows}, {n}] (rows of this shard x all columns), got {tuple(labels.shape)}")
     ldm = ldd = 0
     if mu is not None:
         _chk(mu, torch.float32, "mu", 2)
         _chk(logvar, torch.float32, "logvar", 2)
         ldm = _rowmajor(mu, "mu")
         if _rowmajor(logvar, "logvar") != ldm:
-            raise B2Error("gae_loss_grad: mu and logvar must share a leading dimension")
+            raise B2Error(f"{what}: mu and logvar must share a leading dimension")
         if dmu is None:
             dmu = torch.empty((n_rows, d), dtype=torch.float32, device=z.device)
             dlogvar = torch.empty((n_rows, d), dtype=torch.float32, device=z.device)
         ldd = _rowmajor(dmu, "dmu")
         if _rowmajor(dlogvar, "dlogvar") != ldd:
-            raise B2Error("gae_loss_grad: dmu and dlogvar must share a leading dimension")
+            raise B2Error(f"{what}: dmu and dlogvar must share a leading dimension")
     if loss is None:
         loss = torch.empty(1, dtype=torch.float32, device=z.device)
-    ws = _workspace(lib().b2_gae_loss_workspace_bytes(n, d), z.device)
-    check(lib().b2_gae_loss_grad_f32(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, _p(labels.rowptr),
-                                     _p(labels.colidx), n, d, row_begin, n_rows, float(norm), float(pos_weight),
-                                     int(use_pos_weight),
+    return n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, _workspace(lib().b2_gae_loss_workspace_bytes(n, d), z.device)
+
+
+def gae_loss_grad(z, labels: CSR, norm: float, pos_weight: float, mu=None, logvar=None, use_pos_weight=True,
+                  dz=None, dmu=None, dlogvar=None, loss=None, row_begin: int = 0, n_rows: Optional[int] = None):
+    """Matrix-free Graph-AE loss: returns (loss[1], dz, dmu, dlogvar).
+
+    ``dmu``/``dlogvar`` may be column slices of one packed [n, 2d] buffer (shared leading dimension).
+    """
+    n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, ws = _gae_prepare("gae_loss_grad", z, labels, n_rows, mu, logvar, dmu, dlogvar, loss)
+    if dz is None:
+        dz = torch.empty((n_rows, d), dtype=torch.float32, device=z.device)
+    else:
+        _chk(dz, torch.float32, "dz", 2)
+        if tuple(dz.shape) != (n_rows, d) or not dz.is_contiguous():
+            raise B2Error(f"gae_loss_grad: dz must be a contiguous [{n_rows}, {d}] buffer, got {tuple(dz.shape)} strides {dz.stride()}")
+    check(lib().b2_gae_loss_grad_f32(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, _p(labels.rowptr), _p(labels.colidx), n, d,
+                                     row_begin, n_rows, float(norm), float(pos_weight), int(use_pos_weight),
                                      _p(dz), _p(dmu), _p(dlogvar), ldd, _p(loss), _p(ws), ws.numel(), _stream()),
           "b2_gae_loss_grad_f32")
     return loss, dz, dmu, dlogvar
@@ -372,32 +376,13 @@ def gae_loss_grad_sym(z, labels: CSR, norm: float, pos_weight: float, sb_begin: 
     """Pair-sharded matrix-free Graph-AE loss (multi-GPU form of :func:`gae_loss_grad`): this rank evaluates super-blocks
     ``[sb_begin, sb_end)`` of the unordered block-pair schedule and the label / KLD terms of its rows.  Returns
     ``(loss_share[1], dz_full[n, d], dmu, dlogvar)``; all-reduce ``dz_full`` and ``loss_share`` over ranks."""
-    _chk(z, torch.float32, "z", 2)
-    n, d = z.shape
-    n_rows = n if n_rows is None else n_rows
-    if labels.shape[0] != n_rows or labels.shape[1] != n:
-        raise B2Error(f"gae_loss_grad_sym: labels must be [{n_rows}, {n}], got {tuple(labels.shape)}")
+    n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, ws = _gae_prepare("gae_loss_grad_sym", z, labels, n_rows, mu, logvar, dmu, dlogvar,
+                                                                  loss)
     if dz_full is None:
         dz_full = torch.empty((n, d), dtype=torch.float32, device=z.device)
     _chk(dz_full, torch.float32, "dz_full", 2)
     if tuple(dz_full.shape) != (n, d) or not dz_full.is_contiguous():
         raise B2Error(f"gae_loss_grad_sym: dz_full must be a contiguous [{n}, {d}] buffer")
-    ldm = ldd = 0
-    if mu is not None:
-        _chk(mu, torch.float32, "mu", 2)
-        _chk(logvar, torch.float32, "logvar", 2)
-        ldm = _rowmajor(mu, "mu")
-        if _rowmajor(logvar, "logvar") != ldm:
-            raise B2Error("gae_loss_grad_sym: mu and logvar must share a leading dimension")
-        if dmu is None:
-            dmu = torch.empty((n_rows, d), dtype=torch.float32, device=z.device)
-            dlogvar = torch.empty((n_rows, d), dtype=torch.float32, device=z.device)
-        ldd = _rowmajor(dmu, "dmu")
-        if _rowmajor(dlogvar, "dlogvar") != ldd:
-            raise B2Error("gae_loss_grad_sym: dmu and dlogvar must share a leading dimension")
-    if loss is None:
-        loss = torch.empty(1, dtype=torch.float32, device=z.device)
-    ws = _workspace(lib().b2_gae_loss_workspace_bytes(n, d), z.device)
     check(lib().b2_gae_loss_grad_sym_f32(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, _p(labels.rowptr), _p(labels.colidx), n, d,
                                          sb_begin, sb_end, row_begin, n_rows, float(norm), float(pos_weight), int(use_pos_weight),
                                          _p(dz_full), _p(dmu), _p(dlogvar), ldd, _p(loss), _p(ws), ws.numel(), _stream()),

@@ -171,7 +171,8 @@ int b2_mse_sum_loss_grad_f32(const float* recon, const float* target, const floa
  *   shard's additive share of the loss (constants use the global n).
  *   mu/logvar may be NULL (plain GAE: cost only).
  *   When use_pos_weight == 0 computes loss_function (scgnn2.py:618-619):
- *   plain mean BCE (GAT branch), norm ignored. */
+ *   plain mean BCE (GAT branch), norm ignored.
+ *   d ∈ {8, 16, 32, 64}; any other d returns B2_ERR_UNSUPPORTED. */
 size_t b2_gae_loss_workspace_bytes(int32_t n, int32_t d);
 int b2_gae_loss_grad_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
                          const int32_t* lab_rowptr, const int32_t* lab_colidx,

@@ -386,8 +386,9 @@ def _dense_gae_reference(z, L_dense, norm, pw, mu=None, lv=None):
 
 
 def test_gae_loss_tensor_core_single_column_range(cuda):
-    """The tensor-core decoder at 150 row blocks (more than one wave of SMs: each CTA sweeps ALL columns and the epilogue adds into
-    dz without atomics).  Checked against the fp64 closed form evaluated in row chunks, full and row-sharded."""
+    """The tensor-core decoder at 150 row blocks, more than one wave of SMs.  The call over all rows runs the triangle, which adds
+    into dz atomically; the row shards run the full sweep, where a CTA of the long shard sweeps ALL columns and adds without
+    atomics.  Checked against the fp64 closed form evaluated in row chunks, full and row-sharded."""
     from dance_b200 import ops
     n, d, k = 19_200, 16, 7
     gen = torch.Generator(device=cuda).manual_seed(11)
@@ -413,8 +414,8 @@ def test_gae_loss_tensor_core_single_column_range(cuda):
 
 @pytest.mark.parametrize("n,d", [(128, 16), (100, 16), (256, 16), (300, 16), (384, 8), (1000, 16), (1537, 16), (1664, 8), (2048, 16), (2049, 16)])
 def test_gae_symmetric_decoder_small_graphs(cuda, n, d):
-    """The tensor-core decoder forced onto small graphs: 1, 2, 3, 8, 13, 16, 17 row blocks (odd / even counts, a ragged last
-    block) against the fp64 closed form and against the CUDA-core kernel."""
+    """The triangle (the call over all rows, forced onto the tensor cores) on small graphs: 1, 2, 3, 8, 13, 16, 17 row blocks, a
+    ragged last block and a ragged last 64-column tile, against the fp64 closed form and against the CUDA-core kernel."""
     from dance_b200 import ops
     gen = torch.Generator(device=cuda).manual_seed(n * 31 + d)
     z = (torch.randn(n, d, device=cuda, generator=gen) * 0.6).contiguous()
@@ -442,9 +443,9 @@ def test_gae_symmetric_decoder_small_graphs(cuda, n, d):
 
 @pytest.mark.parametrize("n,splits", [(1537, 2), (2049, 3), (2049, 5), (8200, 2), (8200, 3), (8200, 8)])
 def test_gae_symmetric_decoder_step_splits(cuda, n, splits):
-    """A super-block's J sweep cut into `splits` step ranges, one CTA each (what fills whole waves of SMs under sharding): the same
-    loss and gradient as the unsplit sweep and as the fp64 closed form — including parts of one or two steps, parts that start in
-    the middle of an accumulation segment, and more parts than some super-blocks have steps."""
+    """The triangle's J sweep of each row block (its tiles from the diagonal block on) cut into `splits` step ranges, one CTA each:
+    the same loss and gradient as the unsplit sweep and as the fp64 closed form — including parts of one or two tiles, and more
+    parts than the last row blocks have tiles."""
     from dance_b200 import ops
     gen = torch.Generator(device=cuda).manual_seed(n + splits)
     z = (torch.randn(n, 16, device=cuda, generator=gen) * 0.5).contiguous()
@@ -523,6 +524,58 @@ def test_gae_symmetric_decoder_pair_sharded(cuda, n, parts):
     rows = torch.arange(0, n, 37, device=cuda)
     _, ref_rows = gae_reference_rows(z, A.rowptr, A.colidx, norm, pw, rows)
     assert rel_err(dz_sum[rows], ref_rows) < 2e-5
+
+
+@pytest.mark.parametrize("with_mu", [False, True])
+@pytest.mark.parametrize("form,launches", [("rows-tc", 4), ("rows-cuda", 3), ("sym", 4), ("sym-empty", 3)])
+def test_gae_launches_per_call(cuda, form, launches, with_mu):
+    """Kernels one decoder call launches: the all-pairs part (tensor cores: the split of z and the sweep; an empty super-block
+    range: the split only; CUDA cores: one kernel), the label terms, KLD when mu / logvar are given, and the finish."""
+    from dance_b200 import ops
+    n, d = 300, 16
+    gen = torch.Generator(device=cuda).manual_seed(3)
+    z = (torch.randn(n, d, device=cuda, generator=gen) * 0.5).contiguous()
+    mu, lv = (torch.randn(n, d, device=cuda, generator=gen), torch.randn(n, d, device=cuda, generator=gen)) if with_mu else (None, None)
+    A = ops.knn_graph_build(torch.randint(0, n, (n, 5), device=cuda, dtype=torch.int32, generator=gen))
+    L = ops.CSR(A.rowptr, A.colidx, None, A.shape)
+    nsb = ops.gae_sym_super_blocks(n)
+    ops.set_path("gae", "cuda" if form == "rows-cuda" else "tc")
+    try:
+        ops.reset_counters()
+        if form.startswith("rows"):
+            ops.gae_loss_grad(z, L, 0.5, 20.0, mu, lv)
+        else:
+            sb = (0, nsb) if form == "sym" else (nsb, nsb)
+            ops.gae_loss_grad_sym(z, L, 0.5, 20.0, *sb, mu, lv)
+        got = ops.counters()["launches"]
+    finally:
+        ops.set_path("gae", "auto")
+    assert got == launches + with_mu
+
+
+@pytest.mark.parametrize("path", ["auto", "tc"])
+def test_gae_loss_no_rows(cuda, path):
+    """The row form with n_rows = 0 (a row shard of no rows, labels [0, n]): nothing to sweep, the loss share is 0 and no row of
+    dz, dmu or dlogvar is written.  Called through the C-ABI, which refuses null pointers: torch gives an empty tensor none, so the
+    row buffers point into a guard buffer that must stay as it is."""
+    from dance_b200 import _lib, ops
+    n, d, r = 300, 16, 120
+    lib = _lib.lib()
+    z = torch.randn(n, d, device=cuda)
+    rowptr = torch.zeros(1, dtype=torch.int32, device=cuda)
+    colidx = torch.zeros(1, dtype=torch.int32, device=cuda)
+    guard = torch.full((4, d), 5.0, device=cuda)
+    loss = torch.full((1,), 7.0, device=cuda)
+    ws = torch.empty(lib.b2_gae_loss_workspace_bytes(n, d), dtype=torch.uint8, device=cuda)
+    g = guard.data_ptr()
+    ops.set_path("gae", path)
+    try:
+        status = lib.b2_gae_loss_grad_f32(z.data_ptr(), d, g, g, d, rowptr.data_ptr(), colidx.data_ptr(), n, d, r, 0, 0.5, 20.0, 1,
+                                          g, g, g, d, loss.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream())
+    finally:
+        ops.set_path("gae", "auto")
+    assert status == 0
+    assert loss.item() == 0.0 and torch.all(guard == 5.0)
 
 
 @pytest.mark.parametrize("n,d", [(3000, 16), (2500, 16), (4133, 8), (2304, 32)])

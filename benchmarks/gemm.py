@@ -2,18 +2,21 @@
 precision: ms per call, achieved TFLOP/s from 2·M·N·K, and that rate as a share of the H100 SXM data-sheet dense peak of the
 type (989 TFLOP/s bf16, 495 tf32, 495/3 for tf32x3's three products).  The precisions are timed alternately, several rounds,
 with CUDA events around `--iters` back-to-back calls; the reported ms is the median over rounds.  The first line names the
-card and its power limit, read in the same run.
+card and its power limit, read in the same run.  `--dump-outputs DIR` also writes each shape's C per precision as
+DIR/<shape>.<precision>.npy, so that two builds can be compared element by element.
 
-    python benchmarks/gemm.py [--iters 20] [--rounds 5]
+    python benchmarks/gemm.py [--iters 20] [--rounds 5] [--dump-outputs DIR]
 """
 from __future__ import annotations
 
 import argparse
 import json
+import re
 import subprocess
 import sys
 from pathlib import Path
 
+import numpy as np
 import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
@@ -45,6 +48,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write C of every shape and precision here as .npy")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("benchmarks/gemm.py needs a CUDA device")
@@ -80,6 +84,13 @@ def main():
                               "ms": round(ms, 4), "ms_min": round(t[0], 4), "ms_max": round(t[-1], 4),
                               "tflops": round(tflops, 1), "share_of_peak": round(tflops / PEAK[p], 3), "peak_tflops": round(PEAK[p], 1),
                               "split_k_workspace_bytes": ws[p]}), flush=True)
+        if args.dump_outputs:
+            out = Path(args.dump_outputs)
+            out.mkdir(parents=True, exist_ok=True)
+            slug = re.sub(r"[^0-9A-Za-z]+", "_", name).strip("_")
+            for p in PRECISIONS:
+                ops.gemm(A, B, transA=tA, transB=tB, out=C, precision=p)
+                np.save(out / f"{slug}.{p}.npy", C.cpu().numpy())
         del A, B, C
         torch.cuda.empty_cache()
 

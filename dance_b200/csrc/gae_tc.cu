@@ -268,7 +268,10 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   fence_proxy_async();
   asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
 
-  const int wg = tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
+  // The triangle broadcasts wg from lane 0 so that ptxas knows it is warp-uniform: the shared-memory descriptors of the
+  // warpgroup's Gᵀ and Z_Iᵀ then live in uniform registers instead of taking consumer registers and an R2UR per wgmma.  The
+  // full sweep has no per-warpgroup operand but Z_I and already issues few R2UR (26 for 108 HGMMAs at DP = 16).
+  const int wg = TRI ? __shfl_sync(0xffffffffu, tid >> 7, 0) : tid >> 7, warp = (tid >> 5) & 3, lane = tid & 31;
   const int ra = row0 + wg * 64 + warp * 16 + (lane >> 2);       // rows of this thread: ra, ra + 8
   const bool live_a = ra < row_end, live_b = ra + 8 < row_end;
   const uint32_t ai_hi = smem_u32(zi_hi) + wg * 64 * 128, ai_lo = smem_u32(zi_lo) + wg * 64 * 128;
@@ -301,8 +304,9 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   //     dZ batch queues behind it instead of waiting for it to finish.
   //   Triangle at DP = 8 (OVERLAP): S alternates between two accumulators, so the dZ batch of tile i − 1 (A = the previous S
   //     and L) and the S batch of tile i go out back to back and the turn passes on once both are committed; the tensor pipe
-  //     does not drain within a turn.  wait<1> then retires dZ while S still runs.  At DP = 16 and 32 the second accumulator
-  //     makes ptxas spill in the consumer loop, so those keep one.
+  //     does not drain within a turn.  wait<1> then retires dZ while S still runs.  At DP = 32 the second accumulator makes
+  //     ptxas spill in the consumer loop.  At DP = 16 it fits with one [hi·hi | hi·lo] accumulator but measured slower than
+  //     one S accumulator (DESIGN §4.1), so DP = 16 and 32 keep one.
   constexpr bool OVERLAP = TRI && DP <= 8;
   float S[JW / 2], L[JW / 2];   // S: accumulator of S, then the hi part of G; L: the lo part of G
   auto take_turn = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(2 + wg), "n"(CONSUMERS) : "memory"); };

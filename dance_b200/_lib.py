@@ -12,7 +12,7 @@ from pathlib import Path
 _LIB_PATH = Path(__file__).resolve().parent / "lib" / "libdance_b200.so"
 _lib = None
 
-c_i32, c_i64, c_f32, c_vp, c_sz = C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_size_t
+c_i32, c_i64, c_f32, c_vp, c_sz, c_u32 = C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_size_t, C.c_uint32
 
 # name -> (restype, argtypes); mirrors include/dance_b200.h declaration by declaration
 _SIGNATURES = {
@@ -82,6 +82,16 @@ _SIGNATURES = {
     "b2_gat_combine_fwd_f32": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i32, c_i32, c_i32, C.c_int, C.c_int, c_vp, c_i64, c_vp]),
     "b2_gat_combine_bwd_f32": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_i32, C.c_int, C.c_int, c_vp, c_i64, c_vp, c_i64,
                                          c_vp]),
+    "b2_gat_combine_fwd_identity_f32": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_vp, c_i32, c_i32, c_i32, C.c_int, C.c_int, c_vp, c_i64,
+                                                  c_vp]),
+    "b2_gat_combine_bwd_identity_f32": (C.c_int, [c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_i32, C.c_int, C.c_int, c_vp, c_i64, c_vp,
+                                                  c_i64, c_vp, c_i64, c_vp]),
+    "b2_dropout_f32": (C.c_int, [c_vp, c_i64, c_i64, c_i32, c_f32, c_u32, c_u32, c_vp, c_i64, c_vp]),
+    "b2_gat_aggregate_fwd_drop_f32": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_i32, C.c_int, c_f32, C.c_int,
+                                                c_vp, c_vp, c_i64, c_vp, c_f32, c_u32, c_u32, c_vp]),
+    "b2_gat_aggregate_bwd_drop_f32": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64,
+                                                c_i32, c_i32, c_i32, C.c_int, c_f32, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp,
+                                                c_vp, c_f32, c_u32, c_u32, c_vp]),
     "b2_cellgene_graph_workspace_bytes": (c_sz, [c_i32, c_i32]),
     "b2_cellgene_graph_count": (C.c_int, [c_vp, c_i64, c_i32, c_i32, C.POINTER(c_i64), c_vp, c_sz, c_vp]),
     "b2_cellgene_graph_fill": (C.c_int, [c_vp, c_i64, c_i32, c_i32, C.c_int, c_i64, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]),

@@ -75,6 +75,21 @@ __device__ __forceinline__ void stg_stream_f4(float4* p, const float4& v) {
                "f"(v.z), "f"(v.w));
 }
 
+// Counter-based uniform draw in (0, 1) of element (row, col) of stream `stream` under `seed`: no state, so a backward pass
+// regenerates the forward's draws.  Used by CellwiseMaskData (prep.cu, streams 1 and 2) and by dropout (key = stream).
+__device__ __forceinline__ uint32_t hash32(uint32_t x) {
+  x ^= x >> 16; x *= 0x7FEB352Du; x ^= x >> 15; x *= 0x846CA68Bu; x ^= x >> 16;
+  return x;
+}
+__device__ __forceinline__ float uniform01(uint32_t seed, uint32_t stream, uint32_t row, uint32_t col) {
+  const uint32_t h = hash32(hash32(row + seed * 0x9E3779B1u + stream * 0x85EBCA77u) ^ hash32(col + stream * 0xC2B2AE3Du + 0x27D4EB2Fu));
+  return ((float)(h >> 8) + 0.5f) * (1.f / 16777216.f);
+}
+// Dropout keep bit of element (r, c) under (seed, key): Bernoulli(1 - p); p = 0 keeps everything, p = 1 nothing.
+__device__ __forceinline__ bool dropout_keep(uint32_t seed, uint32_t key, uint32_t r, uint32_t c, float p) {
+  return uniform01(seed, key, r, c) >= p;
+}
+
 __device__ __forceinline__ float apply_act(float v, int act) {
   switch (act) {
     case B2_ACT_RELU: return fmaxf(v, 0.f);

@@ -8,6 +8,11 @@
 //   STAGATE GATConv.forward/message  stagate.py:61-125 (sigmoid scores, PyG per-target softmax)
 // The E×NH×F "lifted" temporaries of the reference are never materialised: each target row streams its
 // in-edges once (twice when the attention coefficients are kept for the backward pass).
+//
+// Attention dropout (GATLayer's third dropout site, scgnn2.py:1029: α' = drop(α) after the softmax) is a compile-time
+// parameter of the aggregate and of both backward sweeps (DROP = false is the plain GAT).  The keep bit of (edge, head) is
+// dropout_keep(seed, key, p, h) with p the edge's position in the target CSR: nothing is stored, the backward regenerates
+// it, and alpha_out keeps the UNDROPPED α.  Per 32 edges each lane draws one edge's bits, shared by ballot / shuffle.
 #include "common.cuh"
 
 #include <math_constants.h>
@@ -55,6 +60,19 @@ __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
 
 __global__ void set_neg_inf_kernel(float* p) { *p = -CUDART_INF_F; }
 
+// Attention-dropout parameters: keep with probability 1 - p, kept coefficients scaled by `scale` = 1 / (1 - p).
+struct AttnDrop {
+  float p, scale;
+  uint32_t seed, key;
+};
+
+// keep bits of edge `pos` for heads 0..nh-1 (nh <= 32), bit h = head h
+__device__ __forceinline__ uint32_t edge_keep_bits(const AttnDrop& dr, int32_t pos, int32_t nh) {
+  uint32_t kb = 0;
+  for (int h = 0; h < nh; ++h) kb |= (uint32_t)dropout_keep(dr.seed, dr.key, (uint32_t)pos, (uint32_t)h, dr.p) << h;
+  return kb;
+}
+
 // scores_per_edge.max() over every edge and head (scgnn2.py:1076)
 __global__ void __launch_bounds__(256)
 gat_edge_max_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
@@ -77,12 +95,14 @@ gat_edge_max_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restric
 
 // Forward aggregate.  One warp per target row; lanes stride over the NH·F row of H.
 //   p_e,h = exp(act(s_src[u,h] + s_trg[v,h]) - shift_h) ; α = p / (Σp + 1e-16) ; out[v] = Σ α H[u]
+// DROP: out[v] = Σ keep_e α_e scale H[u]; a dropped edge is not gathered.
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 gat_aggregate_fwd_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
                          const float* __restrict__ H, int64_t ldh, const float* __restrict__ s_src,
                          const float* __restrict__ s_trg, int32_t n, int32_t nh, int32_t F, int act, float slope,
                          int shift_mode, const float* __restrict__ gmax, float* __restrict__ out, int64_t ldo,
-                         float* __restrict__ alpha_out) {
+                         float* __restrict__ alpha_out, AttnDrop dr) {
   constexpr int MAXV = 16;  // NH*F <= 32*16 = 512 floats per row
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -110,22 +130,30 @@ gat_aggregate_fwd_kernel(const int32_t* __restrict__ rowptr, const int32_t* __re
         }
         float den = 0.f;
         const int t0 = h * tper, t1 = t0 + tper;
+        uint32_t kmask = 0;  // DROP: bit j = keep bit of edge (p - s) rounded down to 32, + j
         for (int32_t p = s; p < e; ++p) {
+          if constexpr (DROP) {
+            if (((p - s) & 31) == 0)
+              kmask = __ballot_sync(0xffffffffu, p + lane < e && dropout_keep(dr.seed, dr.key, (uint32_t)(p + lane), (uint32_t)h, dr.p));
+          }
           const int32_t u = colidx[p];
           const float pe = expf(score_act_f(s_src[(int64_t)u * nh + h] + st, act, slope) - sh);
           den += pe;
+          if (DROP && !((kmask >> ((p - s) & 31)) & 1u)) continue;
           const float* hu = H + (int64_t)u * ldh + lane;
 #pragma unroll
           for (int t = 0; t < MAXV; ++t)
             if (t >= t0 && t < t1) acc[t] = fmaf(pe, hu[32 * t], acc[t]);
         }
-        const float inv = 1.f / (den + 1e-16f);
+        const float inv = DROP ? dr.scale / (den + 1e-16f) : 1.f / (den + 1e-16f);
 #pragma unroll
         for (int t = 0; t < MAXV; ++t)
           if (t >= t0 && t < t1) out[v * ldo + lane + 32 * t] = acc[t] * inv;
-        if (alpha_out)
+        if (alpha_out) {
+          const float ainv = DROP ? 1.f / (den + 1e-16f) : inv;   // α is stored undropped
           for (int32_t p = s + lane; p < e; p += 32)
-            alpha_out[(int64_t)p * nh + h] = expf(score_act_f(s_src[(int64_t)colidx[p] * nh + h] + st, act, slope) - sh) * inv;
+            alpha_out[(int64_t)p * nh + h] = expf(score_act_f(s_src[(int64_t)colidx[p] * nh + h] + st, act, slope) - sh) * ainv;
+        }
       }
     }
     return;
@@ -149,7 +177,13 @@ gat_aggregate_fwd_kernel(const int32_t* __restrict__ rowptr, const int32_t* __re
         }
       }
     }
+    uint32_t kb = 0;  // DROP: lane j holds the keep bits (one per head) of edge (p - s) rounded down to 32, + j
     for (int32_t p = s; p < e; ++p) {
+      uint32_t bits = 0;
+      if constexpr (DROP) {
+        if (((p - s) & 31) == 0) kb = p + lane < e ? edge_keep_bits(dr, p + lane, nh) : 0u;
+        bits = __shfl_sync(0xffffffffu, kb, (p - s) & 31);
+      }
       const int32_t u = colidx[p];
 #pragma unroll
       for (int t = 0; t < MAXV; ++t) {
@@ -158,14 +192,14 @@ gat_aggregate_fwd_kernel(const int32_t* __restrict__ rowptr, const int32_t* __re
           const int h = c / F;
           const float pe = expf(score_act_f(s_src[(int64_t)u * nh + h] + s_trg[v * nh + h], act, slope) - shift[t]);
           den[t] += pe;
-          acc[t] = fmaf(pe, H[(int64_t)u * ldh + c], acc[t]);
+          if (!DROP || ((bits >> h) & 1u)) acc[t] = fmaf(pe, H[(int64_t)u * ldh + c], acc[t]);
         }
       }
     }
 #pragma unroll
     for (int t = 0; t < MAXV; ++t) {
       const int c = lane + 32 * t;
-      if (c < W) out[v * ldo + c] = acc[t] / (den[t] + 1e-16f);
+      if (c < W) out[v * ldo + c] = DROP ? acc[t] / (den[t] + 1e-16f) * dr.scale : acc[t] / (den[t] + 1e-16f);
     }
     if (alpha_out) {
       // attention coefficients per (edge, head) for the backward pass: lanes own heads
@@ -192,6 +226,8 @@ gat_aggregate_fwd_kernel(const int32_t* __restrict__ rowptr, const int32_t* __re
 // With a global shift c (gmax != NULL) the softmax is shift-invariant only up to the +1e-16 of the denominator:
 // ∂α_e/∂c = -α_e ε/(S+ε) with S = Σ_e exp(score - c), so ∂L/∂c = -Σ_{v,h} (Σ α dα) ε/(S+ε).  That sum goes to
 // shift_acc[0] and the number of (edge, head) scores equal to c to shift_acc[1]; gat_bwd_shift_kernel routes it.
+// DROP: the dot is the gradient of the dropped coefficient α' = keep α scale, so dα = keep scale <dOut[v], H[u]>.
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 gat_bwd_target_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx,
                       const float* __restrict__ H, int64_t ldh, const float* __restrict__ s_src,
@@ -199,7 +235,7 @@ gat_bwd_target_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restr
                       const float* __restrict__ dOut, int64_t lddo, const float* __restrict__ H2, int64_t ldh2,
                       const float* __restrict__ dOut2, int64_t lddo2, int32_t n, int32_t nh, int32_t F, int act,
                       float slope, const float* __restrict__ gmax, float* __restrict__ dpre_edge, float* __restrict__ ds_trg,
-                      float* __restrict__ shift_acc) {
+                      float* __restrict__ shift_acc, AttnDrop dr) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -209,13 +245,21 @@ gat_bwd_target_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restr
     const int32_t s = rowptr[v], e = rowptr[v + 1];
     for (int h = 0; h < nh; ++h) {
       float t = 0.f;
+      uint32_t kmask = 0;
       for (int32_t p = s; p < e; ++p) {
         const int32_t u = colidx[p];
         float d = 0.f;
-        for (int f = lane; f < F; f += 32) d = fmaf(dOut[v * lddo + h * F + f], H[(int64_t)u * ldh + h * F + f], d);
-        if (H2)   // tied attention: the same α also weights a second layer's messages (stagate.py:197)
-          for (int f = lane; f < F; f += 32) d = fmaf(dOut2[v * lddo2 + h * F + f], H2[(int64_t)u * ldh2 + h * F + f], d);
-        d = warp_sum(d);
+        if constexpr (DROP) {
+          if (((p - s) & 31) == 0)
+            kmask = __ballot_sync(0xffffffffu, p + lane < e && dropout_keep(dr.seed, dr.key, (uint32_t)(p + lane), (uint32_t)h, dr.p));
+        }
+        if (!DROP || ((kmask >> ((p - s) & 31)) & 1u)) {
+          for (int f = lane; f < F; f += 32) d = fmaf(dOut[v * lddo + h * F + f], H[(int64_t)u * ldh + h * F + f], d);
+          if (H2)   // tied attention: the same α also weights a second layer's messages (stagate.py:197)
+            for (int f = lane; f < F; f += 32) d = fmaf(dOut2[v * lddo2 + h * F + f], H2[(int64_t)u * ldh2 + h * F + f], d);
+          d = warp_sum(d);
+          if constexpr (DROP) d *= dr.scale;
+        }
         if (lane == 0) dpre_edge[(int64_t)p * nh + h] = d;          // kept for the second sweep (same lane reads it back)
         t = fmaf(alpha[(int64_t)p * nh + h], d, t);
       }
@@ -278,14 +322,15 @@ gat_bwd_shift_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restri
 }
 
 // Backward, part 2 (by source, on the transposed CSR; t_perm maps each entry to its position in the
-// target CSR): dH[u] = Σ_out-edges α dOut[v] ; ds_src[u,h] = Σ dpre.
+// target CSR): dH[u] = Σ_out-edges α dOut[v] ; ds_src[u,h] = Σ dpre.  DROP: α' = keep α scale in place of α.
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 gat_bwd_source_kernel(const int32_t* __restrict__ t_rowptr, const int32_t* __restrict__ t_colidx,
                       const int32_t* __restrict__ t_perm, const float* __restrict__ alpha,
                       const float* __restrict__ dpre_edge, const float* __restrict__ dOut, int64_t lddo,
                       const float* __restrict__ dOut2, int64_t lddo2, int32_t n, int32_t nh, int32_t F,
                       float* __restrict__ dH, int64_t lddh, float* __restrict__ dH2, int64_t lddh2,
-                      float* __restrict__ ds_src) {
+                      float* __restrict__ ds_src, AttnDrop dr) {
   constexpr int MAXV = 16;
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -297,14 +342,24 @@ gat_bwd_source_kernel(const int32_t* __restrict__ t_rowptr, const int32_t* __res
 #pragma unroll
     for (int t = 0; t < MAXV; ++t) { acc[t] = 0.f; acc2[t] = 0.f; }
     float ssrc = 0.f;  // lanes < nh accumulate ds_src for their head
+    uint32_t kb = 0;  // DROP: lane j holds the keep bits of out-edge (q - s) rounded down to 32, + j
     for (int32_t q = s; q < e; ++q) {
+      uint32_t bits = 0;
+      if constexpr (DROP) {
+        if (((q - s) & 31) == 0) kb = q + lane < e ? edge_keep_bits(dr, t_perm[q + lane], nh) : 0u;
+        bits = __shfl_sync(0xffffffffu, kb, (q - s) & 31);
+      }
       const int32_t v = t_colidx[q];
       const int32_t p = t_perm[q];
 #pragma unroll
       for (int t = 0; t < MAXV; ++t) {
         const int c = lane + 32 * t;
         if (c < W) {
-          const float a = alpha[(int64_t)p * nh + c / F];
+          if constexpr (DROP) {
+            const int h = c / F;
+            if (!((bits >> h) & 1u)) continue;
+          }
+          const float a = DROP ? alpha[(int64_t)p * nh + c / F] * dr.scale : alpha[(int64_t)p * nh + c / F];
           acc[t] = fmaf(a, dOut[(int64_t)v * lddo + c], acc[t]);
           if (dOut2) acc2[t] = fmaf(a, dOut2[(int64_t)v * lddo2 + c], acc2[t]);
         }
@@ -362,6 +417,8 @@ gat_bwd_scores_kernel(const float* __restrict__ H, int64_t ldh, const float* __r
 }
 
 // skip / concat-or-mean / bias / activation  (scgnn2.py:1189-1215)
+// IDENTITY: skip is [n, F], added to every head (the FIN == FOUT branch, scgnn2.py:1167-1171)
+template <bool IDENTITY>
 __global__ void __launch_bounds__(256)
 gat_combine_fwd_kernel(const float* __restrict__ agg, int64_t lda, const float* __restrict__ skip, int64_t lds,
                        const float* __restrict__ bias, int32_t n, int32_t nh, int32_t F, int concat, int act,
@@ -373,15 +430,22 @@ gat_combine_fwd_kernel(const float* __restrict__ agg, int64_t lda, const float* 
     const int c = (int)(t % OW);
     float v;
     if (concat) {
-      v = agg[i * lda + c] + (skip ? skip[i * lds + c] : 0.f);
+      v = agg[i * lda + c] + (skip ? skip[i * lds + (IDENTITY ? c % F : c)] : 0.f);
     } else {
       v = 0.f;
-      for (int h = 0; h < nh; ++h) v += agg[i * lda + h * F + c] + (skip ? skip[i * lds + h * F + c] : 0.f);
+      for (int h = 0; h < nh; ++h) v += agg[i * lda + h * F + c] + (skip ? skip[i * lds + (IDENTITY ? c : h * F + c)] : 0.f);
       v = v / (float)nh;   // mean over heads
     }
     if (bias) v += bias[c];
     out[i * ldo + c] = apply_act(v, act);
   }
+}
+
+__device__ __forceinline__ float combine_act_bwd(float g, const float* __restrict__ o, int act) {
+  if (act == B2_ACT_ELU) { const float v = *o; g *= (v > 0.f ? 1.f : v + 1.f); }
+  else if (act == B2_ACT_RELU) { g = *o > 0.f ? g : 0.f; }
+  else if (act == B2_ACT_TANH) { const float v = *o; g *= (1.f - v * v); }
+  return g;
 }
 
 // d(pre-combine)[n, nh*F] and d(pre-activation)[n, OW] (the latter feeds the bias gradient)
@@ -394,13 +458,39 @@ gat_combine_bwd_kernel(const float* __restrict__ dout, int64_t lddo, const float
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t i = t / OW;
     const int c = (int)(t % OW);
-    float g = dout[i * lddo + c];
-    if (act == B2_ACT_ELU) { const float o = out[i * ldo + c]; g *= (o > 0.f ? 1.f : o + 1.f); }
-    else if (act == B2_ACT_RELU) { g = out[i * ldo + c] > 0.f ? g : 0.f; }
-    else if (act == B2_ACT_TANH) { const float o = out[i * ldo + c]; g *= (1.f - o * o); }
+    const float g = combine_act_bwd(dout[i * lddo + c], out + i * ldo + c, act);
     if (dact) dact[i * ldact + c] = g;
     if (concat) dpre[i * ldp + c] = g;
     else for (int h = 0; h < nh; ++h) dpre[i * ldp + h * F + c] = g / (float)nh;
+  }
+}
+
+// The same with an identity skip: additionally dskip[n, F] = Σ_h dpre[n, h·F:(h+1)·F], the skip's share of d(input).
+// One thread per (row, feature) walks the heads.
+__global__ void __launch_bounds__(256)
+gat_combine_bwd_identity_kernel(const float* __restrict__ dout, int64_t lddo, const float* __restrict__ out, int64_t ldo,
+                                int32_t n, int32_t nh, int32_t F, int concat, int act, float* __restrict__ dpre, int64_t ldp,
+                                float* __restrict__ dact, int64_t ldact, float* __restrict__ dskip, int64_t ldsk) {
+  const int64_t total = (int64_t)n * F;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t i = t / F;
+    const int f = (int)(t % F);
+    float sum = 0.f;
+    if (concat) {
+      for (int h = 0; h < nh; ++h) {
+        const int c = h * F + f;
+        const float g = combine_act_bwd(dout[i * lddo + c], out + i * ldo + c, act);
+        if (dact) dact[i * ldact + c] = g;
+        dpre[i * ldp + c] = g;
+        sum += g;
+      }
+    } else {
+      const float g = combine_act_bwd(dout[i * lddo + f], out + i * ldo + f, act);
+      if (dact) dact[i * ldact + f] = g;
+      const float gh = g / (float)nh;
+      for (int h = 0; h < nh; ++h) { dpre[i * ldp + h * F + f] = gh; sum += gh; }
+    }
+    dskip[i * ldsk + f] = sum;
   }
 }
 
@@ -456,10 +546,32 @@ extern "C" int b2_gat_aggregate_fwd_f32(const int32_t* rowptr, const int32_t* co
   B2_REQUIRE(shift_mode == 1 || gmax_dev, "b2_gat_aggregate_fwd_f32: global shift needs gmax_dev");
   if (n == 0) return B2_OK;
   B2_REQUIRE(rowptr && colidx && H && s_src && s_trg && out, "b2_gat_aggregate_fwd_f32: null pointer");
-  gat_aggregate_fwd_kernel<<<warp_rows_grid(n), 256, 0, as_stream(stream)>>>(rowptr, colidx, H, ldh, s_src, s_trg, n, nheads, F,
-                                                                           score_act, slope, shift_mode, gmax_dev, out, ldo,
-                                                                           alpha_out);
+  gat_aggregate_fwd_kernel<false><<<warp_rows_grid(n), 256, 0, as_stream(stream)>>>(rowptr, colidx, H, ldh, s_src, s_trg, n, nheads, F,
+                                                                                  score_act, slope, shift_mode, gmax_dev, out, ldo,
+                                                                                  alpha_out, AttnDrop{});
   B2_CHECK_LAUNCH("gat_aggregate_fwd_kernel");
+  return B2_OK;
+}
+
+static bool drop_prob_ok(float p) { return p >= 0.f && p <= 1.f; }   // false for NaN
+static AttnDrop make_drop(float p, uint32_t seed, uint32_t key) { return AttnDrop{p, p < 1.f ? 1.f / (1.f - p) : 0.f, seed, key}; }
+
+extern "C" int b2_gat_aggregate_fwd_drop_f32(const int32_t* rowptr, const int32_t* colidx, const float* H, int64_t ldh,
+                                             const float* s_src, const float* s_trg, int32_t n, int32_t nheads, int32_t F,
+                                             int score_act, float slope, int shift_mode, const float* gmax_dev, float* out,
+                                             int64_t ldo, float* alpha_out, float drop_p, uint32_t seed, uint32_t key,
+                                             void* stream) {
+  B2_REQUIRE(n >= 0 && nheads > 0 && nheads <= 32 && F > 0 && (int64_t)nheads * F <= 512 && ldh >= (int64_t)nheads * F &&
+                 ldo >= (int64_t)nheads * F,
+             "b2_gat_aggregate_fwd_drop_f32: nheads must be <= 32, nheads*F <= 512 and leading dimensions >= nheads*F");
+  B2_REQUIRE(drop_prob_ok(drop_p), "b2_gat_aggregate_fwd_drop_f32: drop_p must be in [0, 1]");
+  B2_REQUIRE(shift_mode == 1 || gmax_dev, "b2_gat_aggregate_fwd_drop_f32: global shift needs gmax_dev");
+  if (n == 0) return B2_OK;
+  B2_REQUIRE(rowptr && colidx && H && s_src && s_trg && out, "b2_gat_aggregate_fwd_drop_f32: null pointer");
+  gat_aggregate_fwd_kernel<true><<<warp_rows_grid(n), 256, 0, as_stream(stream)>>>(rowptr, colidx, H, ldh, s_src, s_trg, n, nheads, F,
+                                                                                 score_act, slope, shift_mode, gmax_dev, out, ldo,
+                                                                                 alpha_out, make_drop(drop_p, seed, key));
+  B2_CHECK_LAUNCH("gat_aggregate_fwd_kernel<drop>");
   return B2_OK;
 }
 
@@ -470,7 +582,7 @@ static int gat_aggregate_bwd_impl(const int32_t* rowptr, const int32_t* colidx, 
                                   const float* dOut2, int64_t lddo2, int32_t n, int32_t nheads, int32_t F, int score_act,
                                   float slope, const float* gmax_dev, float* dH, int64_t lddh, float* dH2, int64_t lddh2,
                                   float* da_src, float* da_trg, float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws,
-                                  float* shift_ws, void* stream) {
+                                  float* shift_ws, const AttnDrop* drop, void* stream) {
   B2_REQUIRE(n >= 0 && nheads > 0 && nheads <= 32 && F > 0 && (int64_t)nheads * F <= 512, "b2_gat_aggregate_bwd_f32: bad shape");
   B2_REQUIRE(a_src && a_trg && da_src && da_trg, "b2_gat_aggregate_bwd_f32: null pointer");
   B2_REQUIRE(!gmax_dev || shift_ws, "b2_gat_aggregate_bwd_f32: a global shift (gmax_dev) needs shift_ws");
@@ -483,17 +595,28 @@ static int gat_aggregate_bwd_impl(const int32_t* rowptr, const int32_t* colidx, 
                  ds_trg_ws && dpre_edge_ws,
              "b2_gat_aggregate_bwd_f32: null pointer");
   if (gmax_dev) B2_CHECK_CUDA(cudaMemsetAsync(shift_ws, 0, sizeof(float) * 2, st));
-  gat_bwd_target_kernel<<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, H, ldh, s_src, s_trg, alpha, dOut, lddo, H2, ldh2, dOut2,
-                                                          lddo2, n, nheads, F, score_act, slope, gmax_dev, dpre_edge_ws, ds_trg_ws,
-                                                          shift_ws);
+  if (drop)
+    gat_bwd_target_kernel<true><<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, H, ldh, s_src, s_trg, alpha, dOut, lddo, H2, ldh2,
+                                                                  dOut2, lddo2, n, nheads, F, score_act, slope, gmax_dev, dpre_edge_ws,
+                                                                  ds_trg_ws, shift_ws, *drop);
+  else
+    gat_bwd_target_kernel<false><<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, H, ldh, s_src, s_trg, alpha, dOut, lddo, H2, ldh2,
+                                                                   dOut2, lddo2, n, nheads, F, score_act, slope, gmax_dev, dpre_edge_ws,
+                                                                   ds_trg_ws, shift_ws, AttnDrop{});
   B2_CHECK_LAUNCH("gat_bwd_target_kernel");
   if (gmax_dev) {
     gat_bwd_shift_kernel<<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, s_src, s_trg, n, nheads, score_act, slope, gmax_dev,
                                                            shift_ws, dpre_edge_ws, ds_trg_ws);
     B2_CHECK_LAUNCH("gat_bwd_shift_kernel");
   }
-  gat_bwd_source_kernel<<<warp_rows_grid(n), 256, 0, st>>>(t_rowptr, t_colidx, t_perm, alpha, dpre_edge_ws, dOut, lddo,
-                                                          dH2 ? dOut2 : nullptr, lddo2, n, nheads, F, dH, lddh, dH2, lddh2, ds_src_ws);
+  if (drop)
+    gat_bwd_source_kernel<true><<<warp_rows_grid(n), 256, 0, st>>>(t_rowptr, t_colidx, t_perm, alpha, dpre_edge_ws, dOut, lddo,
+                                                                  dH2 ? dOut2 : nullptr, lddo2, n, nheads, F, dH, lddh, dH2, lddh2,
+                                                                  ds_src_ws, *drop);
+  else
+    gat_bwd_source_kernel<false><<<warp_rows_grid(n), 256, 0, st>>>(t_rowptr, t_colidx, t_perm, alpha, dpre_edge_ws, dOut, lddo,
+                                                                   dH2 ? dOut2 : nullptr, lddo2, n, nheads, F, dH, lddh, dH2, lddh2,
+                                                                   ds_src_ws, AttnDrop{});
   B2_CHECK_LAUNCH("gat_bwd_source_kernel");
   int splits = ceil_div(sm_count() * 2, ceil_div(W, 32));
   const int max_splits = n / 256 > 0 ? n / 256 : 1;
@@ -514,7 +637,21 @@ extern "C" int b2_gat_aggregate_bwd_f32(const int32_t* rowptr, const int32_t* co
                                         float* shift_ws, void* stream) {
   return gat_aggregate_bwd_impl(rowptr, colidx, t_rowptr, t_colidx, t_perm, H, ldh, a_src, a_trg, s_src, s_trg, alpha, dOut, lddo,
                                 nullptr, 0, nullptr, 0, n, nheads, F, score_act, slope, gmax_dev, dH, lddh, nullptr, 0, da_src,
-                                da_trg, ds_src_ws, ds_trg_ws, dpre_edge_ws, shift_ws, stream);
+                                da_trg, ds_src_ws, ds_trg_ws, dpre_edge_ws, shift_ws, nullptr, stream);
+}
+
+extern "C" int b2_gat_aggregate_bwd_drop_f32(const int32_t* rowptr, const int32_t* colidx, const int32_t* t_rowptr,
+                                             const int32_t* t_colidx, const int32_t* t_perm, const float* H, int64_t ldh,
+                                             const float* a_src, const float* a_trg, const float* s_src, const float* s_trg,
+                                             const float* alpha, const float* dOut, int64_t lddo, int32_t n, int32_t nheads,
+                                             int32_t F, int score_act, float slope, const float* gmax_dev, float* dH, int64_t lddh,
+                                             float* da_src, float* da_trg, float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws,
+                                             float* shift_ws, float drop_p, uint32_t seed, uint32_t key, void* stream) {
+  B2_REQUIRE(drop_prob_ok(drop_p), "b2_gat_aggregate_bwd_drop_f32: drop_p must be in [0, 1]");
+  const AttnDrop drop = make_drop(drop_p, seed, key);
+  return gat_aggregate_bwd_impl(rowptr, colidx, t_rowptr, t_colidx, t_perm, H, ldh, a_src, a_trg, s_src, s_trg, alpha, dOut, lddo,
+                                nullptr, 0, nullptr, 0, n, nheads, F, score_act, slope, gmax_dev, dH, lddh, nullptr, 0, da_src,
+                                da_trg, ds_src_ws, ds_trg_ws, dpre_edge_ws, shift_ws, &drop, stream);
 }
 
 extern "C" int b2_gat_aggregate_bwd_tied_f32(const int32_t* rowptr, const int32_t* colidx, const int32_t* t_rowptr,
@@ -528,7 +665,7 @@ extern "C" int b2_gat_aggregate_bwd_tied_f32(const int32_t* rowptr, const int32_
   B2_REQUIRE(n == 0 || (H2 && dOut2), "b2_gat_aggregate_bwd_tied_f32: the second layer's H2 / dOut2 are required (dH2 may be NULL)");
   return gat_aggregate_bwd_impl(rowptr, colidx, t_rowptr, t_colidx, t_perm, H, ldh, a_src, a_trg, s_src, s_trg, alpha, dOut, lddo,
                                 H2, ldh2, dOut2, lddo2, n, nheads, F, score_act, slope, gmax_dev, dH, lddh, dH2, lddh2, da_src,
-                                da_trg, ds_src_ws, ds_trg_ws, dpre_edge_ws, shift_ws, stream);
+                                da_trg, ds_src_ws, ds_trg_ws, dpre_edge_ws, shift_ws, nullptr, stream);
 }
 
 extern "C" int b2_gat_combine_fwd_f32(const float* agg, int64_t ldagg, const float* skip, int64_t ldskip, const float* bias,
@@ -537,9 +674,21 @@ extern "C" int b2_gat_combine_fwd_f32(const float* agg, int64_t ldagg, const flo
   B2_REQUIRE(n >= 0 && nheads > 0 && F > 0, "b2_gat_combine_fwd_f32: bad arguments");
   if (n == 0) return B2_OK;
   B2_REQUIRE(agg && out, "b2_gat_combine_fwd_f32: null pointer");
-  gat_combine_fwd_kernel<<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
+  gat_combine_fwd_kernel<false><<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
       agg, ldagg, skip, ldskip, bias, n, nheads, F, concat, act, out, ldo);
   B2_CHECK_LAUNCH("gat_combine_fwd_kernel");
+  return B2_OK;
+}
+
+extern "C" int b2_gat_combine_fwd_identity_f32(const float* agg, int64_t ldagg, const float* x, int64_t ldx, const float* bias,
+                                               int32_t n, int32_t nheads, int32_t F, int concat, int act, float* out, int64_t ldo,
+                                               void* stream) {
+  B2_REQUIRE(n >= 0 && nheads > 0 && F > 0 && ldx >= F, "b2_gat_combine_fwd_identity_f32: bad arguments");
+  if (n == 0) return B2_OK;
+  B2_REQUIRE(agg && x && out, "b2_gat_combine_fwd_identity_f32: null pointer");
+  gat_combine_fwd_kernel<true><<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
+      agg, ldagg, x, ldx, bias, n, nheads, F, concat, act, out, ldo);
+  B2_CHECK_LAUNCH("gat_combine_fwd_kernel<identity>");
   return B2_OK;
 }
 
@@ -552,5 +701,17 @@ extern "C" int b2_gat_combine_bwd_f32(const float* dout, int64_t lddo, const flo
   gat_combine_bwd_kernel<<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
       dout, lddo, out, ldo, n, nheads, F, concat, act, dpre, ldp, dact, ldact);
   B2_CHECK_LAUNCH("gat_combine_bwd_kernel");
+  return B2_OK;
+}
+
+extern "C" int b2_gat_combine_bwd_identity_f32(const float* dout, int64_t lddo, const float* out, int64_t ldo, int32_t n,
+                                               int32_t nheads, int32_t F, int concat, int act, float* dpre, int64_t ldp, float* dact,
+                                               int64_t ldact, float* dx_skip, int64_t ldx, void* stream) {
+  B2_REQUIRE(n >= 0 && nheads > 0 && F > 0 && ldx >= F, "b2_gat_combine_bwd_identity_f32: bad arguments");
+  if (n == 0) return B2_OK;
+  B2_REQUIRE(dout && out && dpre && dx_skip, "b2_gat_combine_bwd_identity_f32: null pointer");
+  gat_combine_bwd_identity_kernel<<<ew_blocks((int64_t)n * F), 256, 0, as_stream(stream)>>>(dout, lddo, out, ldo, n, nheads, F, concat,
+                                                                                           act, dpre, ldp, dact, ldact, dx_skip, ldx);
+  B2_CHECK_LAUNCH("gat_combine_bwd_identity_kernel");
   return B2_OK;
 }

@@ -66,14 +66,7 @@ subset_kernel(const float* __restrict__ X, int64_t ldx, const int64_t* __restric
 }
 
 // ---- CellwiseMaskData -------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t hash32(uint32_t x) {
-  x ^= x >> 16; x *= 0x7FEB352Du; x ^= x >> 15; x *= 0x846CA68Bu; x ^= x >> 16;
-  return x;
-}
-__device__ __forceinline__ float uniform01(uint32_t seed, uint32_t stream, uint32_t row, uint32_t col) {
-  const uint32_t h = hash32(hash32(row + seed * 0x9E3779B1u + stream * 0x85EBCA77u) ^ hash32(col + stream * 0xC2B2AE3Du + 0x27D4EB2Fu));
-  return ((float)(h >> 8) + 0.5f) * (1.f / 16777216.f);
-}
+// uniform01 (common.cuh) with streams 1 and 2
 
 // One block per cell.  Positive entries get the Efraimidis–Spirakis key log(u)/w (w = exp(−x/20) for distr "exp", 1 for
 // "uniform"): the n_masked LARGEST keys are a weighted sample without replacement with probabilities ∝ w — the distribution of

@@ -9,6 +9,8 @@ Reference being replaced:
   * Feature_AE + train_handler + loss_function_graph   scgnn2.py:338-370, 1217-1328
   * Graph_AE (GCN branch) + graph_AE_handler loop + gae_loss_function
                                                        scgnn2.py:373-412, 479-502, 555-615
+  * Graph_AE (GAT branch, with GATLayer's dropout and identity skips)
+                                                       scgnn2.py:376-378, 883-1215, 575-593
 """
 from __future__ import annotations
 
@@ -345,19 +347,27 @@ class GATEngine:
 
     Per layer the attention projection and the skip projection read the same input, so they are stored
     packed ``[linear_proj ; skip_proj]`` and evaluated by ONE GEMM; ``state_dict`` splits them back into the
-    reference's keys (``gat.gat_net.{l}.linear_proj.weight`` …).
+    reference's keys (``gat.gat_net.{l}.linear_proj.weight`` …).  A layer whose input width equals its per-head output
+    width adds its raw input to every head instead (scgnn2.py:1167-1171): it runs the projection half of the GEMM only, and
+    ``skip_proj`` — kept for the state_dict, as in the reference — gets an exactly zero gradient, so Adam never moves it.
+
+    ``dropout`` is GATLayer's ``nn.Dropout(p)`` in training steps, at its three sites (scgnn2.py:1005, 1010, 1029): the layer
+    input, the projection ``H`` and the attention coefficients.  The masks are counter-based draws under ``seed`` with one key
+    per (training step, layer, site) — :meth:`drop_key` — and the backward regenerates them (see :func:`ops.dropout`).
     """
 
+    SITES = ("input", "proj", "attn")
+
     def __init__(self, dim: int, hid: int = 64, embedding_size: int = 16, heads: int = 2, device="cuda", lr: float = 1e-2,
-                 precision: Optional[str] = None, seed: Optional[int] = None):
+                 precision: Optional[str] = None, seed: Optional[int] = None, *, dropout: float = 0.0):
         self.device, self.lr, self.precision, self.nh = torch.device(device), lr, precision, heads
+        self.dropout = ops._drop_prob(dropout)
+        # seed of the dropout draws; without a seed (and with dropout), one from torch's default generator
+        self.drop_seed = int(seed) & 0xFFFFFFFF if seed is not None else (int(torch.randint(0, 2**31, (1, )).item()) if self.dropout else 0)
+        self.step = 0        # training steps taken: part of every dropout key
         self.layers = [dict(fin=dim, F=hid, concat=True, act="elu"), dict(fin=hid * heads, F=embedding_size, concat=False, act=None)]
         for L in self.layers:
-            if L["fin"] == L["F"]:
-                # GATLayer adds the RAW input to every head when FIN == FOUT and leaves skip_proj unused / untrained
-                # (scgnn2.py:1163-1171); this engine always evaluates the packed projection+skip GEMM
-                raise NotImplementedError(f"GAT layer with equal input and per-head output width ({L['fin']}) uses an identity skip "
-                                          "connection in the reference; that branch is not built — choose gat_hid_embed != input width")
+            L["identity"] = L["fin"] == L["F"]
         shapes = []
         for l, L in enumerate(self.layers):
             W = heads * L["F"]
@@ -411,49 +421,84 @@ class GATEngine:
             out.update(self._split(self.params.g, l))
         return out
 
-    def forward(self, x: torch.Tensor, T: CSR, keep: bool = False):
-        """GAT.forward on the target-indexed CSR ``T`` (row v = sources of v's in-edges); returns the node embedding."""
+    def drop_key(self, layer: int, site: str, step: Optional[int] = None) -> int:
+        """Key of the dropout draw at ``site`` ("input" | "proj" | "attn") of ``layer`` in training step ``step`` (default: the
+        step :meth:`train_step` runs next).  ``ops.dropout(ones, p, eng.drop_seed, key)`` reproduces the mask; for "attn" over
+        [nnz, heads], row p is the edge at position p of the target CSR."""
+        s = self.step if step is None else step
+        return (s * len(self.layers) + layer) * len(self.SITES) + self.SITES.index(site)
+
+    def _drop_kw(self, l: int, site: str) -> dict:
+        return dict(dropout=self.dropout, seed=self.drop_seed, key=self.drop_key(l, site))
+
+    def forward(self, x: torch.Tensor, T: CSR, keep: bool = False, training: bool = False):
+        """GAT.forward on the target-indexed CSR ``T`` (row v = sources of v's in-edges); returns the node embedding.
+        ``training``: apply the layers' dropout (train() mode) with the keys of the current step."""
         P, pr, nh = self.params.p, self.precision, self.nh
+        drop = training and self.dropout > 0
         h = x
         for l, L in enumerate(self.layers):
             W = nh * L["F"]
-            hs = ops.gemm(h, P[f"l{l}.projskip"], transB=True, precision=pr)         # [n, 2W]: projection | skip projection
-            H, skip = hs[:, :W], hs[:, W:]
+            if drop:
+                h = ops.dropout(h, self.dropout, self.drop_seed, self.drop_key(l, "input"))   # out of place: ELU backward reads `out`
+            if L["identity"]:
+                hs = ops.gemm(h, P[f"l{l}.projskip"][:W], transB=True, precision=pr)   # [n, W]: projection; the skip is h itself
+                H, skip = hs, h
+            else:
+                hs = ops.gemm(h, P[f"l{l}.projskip"], transB=True, precision=pr)       # [n, 2W]: projection | skip projection
+                H, skip = hs[:, :W], hs[:, W:]
+            if drop:
+                ops.dropout(H, self.dropout, self.drop_seed, self.drop_key(l, "proj"), out=H)
             s_src, s_trg = ops.gat_scores(H, P[f"l{l}.a_src"], P[f"l{l}.a_trg"], nh)
-            agg, alpha, gmax = ops.gat_aggregate_fwd(T, H, s_src, s_trg, nh, "leakyrelu", 0.2, "global", keep_alpha=keep)
-            out = ops.gat_combine_fwd(agg, skip, P[f"l{l}.bias"], nh, L["concat"], L["act"])
+            agg, alpha, gmax = ops.gat_aggregate_fwd(T, H, s_src, s_trg, nh, "leakyrelu", 0.2, "global", keep_alpha=keep,
+                                                     **(self._drop_kw(l, "attn") if drop else {}))
+            out = ops.gat_combine_fwd(agg, skip, P[f"l{l}.bias"], nh, L["concat"], L["act"], identity=L["identity"])
             if keep:
-                self._cache[l] = dict(x=h, hs=hs, s_src=s_src, s_trg=s_trg, alpha=alpha, gmax=gmax, out=out)
+                self._cache[l] = dict(x=h, hs=hs, s_src=s_src, s_trg=s_trg, alpha=alpha, gmax=gmax, out=out, drop=drop)
             h = out
         return h
 
     def train_step(self, x: torch.Tensor, T: CSR, Tt: CSR, t_perm: torch.Tensor, labels: CSR):
-        """One epoch of graph_AE_handler with use_GAT=True (scgnn2.py:575-593): forward, loss_function
-        (plain mean BCE on z zᵀ, scgnn2.py:618-619), backward, Adam."""
+        """One epoch of graph_AE_handler with use_GAT=True (scgnn2.py:575-593): forward (train mode), loss_function
+        (plain mean BCE on z zᵀ, scgnn2.py:618-619), backward, Adam.  Returns the embedding of this (dropped-out) forward."""
         P, G, pr, nh = self.params.p, self.params.g, self.precision, self.nh
-        z = self.forward(x, T, keep=True)
+        z = self.forward(x, T, keep=True, training=True)
         _, dz, _, _ = ops.gae_loss_grad(z, labels, 1.0, 1.0, use_pos_weight=False, loss=self.loss)
         dout = dz
         for l in reversed(range(len(self.layers))):
             L, c = self.layers[l], self._cache[l]
             W, F = nh * L["F"], L["F"]
-            dhs = torch.empty_like(c["hs"])                                           # [n, 2W]: d projection | d skip
-            dH, dskip = dhs[:, :W], dhs[:, W:]
-            n = dout.shape[0]
-            dact = torch.empty_like(c["out"])
-            ops.check(ops.lib().b2_gat_combine_bwd_f32(ops._p(dout), ops._rowmajor(dout, "dout"), ops._p(c["out"]),
-                                                       ops._rowmajor(c["out"], "out"), n, nh, F, int(L["concat"]), ops.ACT[L["act"]],
-                                                       ops._p(dskip), ops._rowmajor(dskip, "dskip"), ops._p(dact),
-                                                       ops._rowmajor(dact, "dact"), ops._stream()), "b2_gat_combine_bwd_f32")
+            drop, ident = c["drop"], L["identity"]
+            if ident:
+                dskip, dact, dx = ops.gat_combine_bwd(dout, c["out"], nh, F, L["concat"], L["act"], identity=True)
+            else:
+                dhs = torch.empty_like(c["hs"])                                       # [n, 2W]: d projection | d skip
+                dH, dskip = dhs[:, :W], dhs[:, W:]
+                _, dact = ops.gat_combine_bwd(dout, c["out"], nh, F, L["concat"], L["act"], dpre=dskip)
             ops.colsum(dact, out=G[f"l{l}.bias"])
             H = c["hs"][:, :W]
             dHm, da_src, da_trg = ops.gat_aggregate_bwd(T, Tt, t_perm, H, P[f"l{l}.a_src"], P[f"l{l}.a_trg"], c["s_src"], c["s_trg"],
-                                                        c["alpha"], dskip, nh, gmax=c["gmax"])
-            dH.copy_(dHm)
+                                                        c["alpha"], dskip, nh, gmax=c["gmax"],
+                                                        **(self._drop_kw(l, "attn") if drop else {}))
+            if ident:
+                dH = dHm
+            else:
+                dH.copy_(dHm)
+            if drop:
+                ops.dropout(dH, self.dropout, self.drop_seed, self.drop_key(l, "proj"), out=dH)
             G[f"l{l}.a_src"].copy_(da_src)
             G[f"l{l}.a_trg"].copy_(da_trg)
-            ops.gemm(dhs, c["x"], transA=True, out=G[f"l{l}.projskip"], precision=pr)
-            if l > 0:
-                dout = ops.gemm(dhs, P[f"l{l}.projskip"], precision=pr)
+            if ident:
+                # skip_proj's half of the gradient stays zero (FlatParams starts it at zero and nothing writes it)
+                ops.gemm(dH, c["x"], transA=True, out=G[f"l{l}.projskip"][:W], precision=pr)
+                if l > 0:
+                    dout = ops.gemm(dH, P[f"l{l}.projskip"][:W], out=dx, accumulate=True, precision=pr)
+            else:
+                ops.gemm(dhs, c["x"], transA=True, out=G[f"l{l}.projskip"], precision=pr)
+                if l > 0:
+                    dout = ops.gemm(dhs, P[f"l{l}.projskip"], precision=pr)
+            if l > 0 and drop:
+                ops.dropout(dout, self.dropout, self.drop_seed, self.drop_key(l, "input"), out=dout)
         self.params.adam_step(self.lr)
+        self.step += 1
         return z

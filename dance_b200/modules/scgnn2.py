@@ -136,8 +136,9 @@ def build_knn_graph(x_embed: torch.Tensor, neighborhood_factor):
 def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int = 4096):
     """Graph autoencoder stage, GCN branch (scgnn2.py:530-600): returns (embed, recon_graph, edgeList, adj)."""
     logger.info("Starting Graph AE")
-    if args.graph_AE_use_GAT and args.graph_AE_GAT_dropout:
-        raise NotImplementedError("graph_AE_GAT_dropout > 0 is not built (the example default is 0)")
+    gat_dropout = float(getattr(args, "graph_AE_GAT_dropout", 0) or 0)
+    if args.graph_AE_use_GAT and not 0.0 <= gat_dropout <= 1.0:          # nn.Dropout's check (Graph_AE → GATLayer, scgnn2.py:375-378)
+        raise ValueError(f"dropout probability has to be between 0 and 1, but got {gat_dropout}")
     if args.graph_AE_concat_prev_embed and param["epoch_num"] > 0:
         raise NotImplementedError("graph_AE_concat_prev_embed is not built")
     if args.graph_AE_retain_weights:
@@ -192,8 +193,9 @@ def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int
         src_csr = ops.CSR(torch.arange(0, n * k + 1, k, dtype=torch.int32, device=dev), knn_idx.reshape(-1).contiguous(), None, (n, n))
         T, _ = ops.csr_transpose(src_csr)
         Tt, t_perm = ops.csr_transpose(T)
+        # train() mode: every epoch is a dropped-out forward, and the returned embedding is the last one (scgnn2.py:578-597)
         geng = GATEngine(xe.shape[1], args.gat_hid_embed, args.graph_AE_embedding_size, args.gat_multi_heads, device=dev,
-                         lr=args.graph_AE_learning_rate, precision=param.get("precision"), seed=param.get("seed"))
+                         lr=args.graph_AE_learning_rate, precision=param.get("precision"), seed=param.get("seed"), dropout=gat_dropout)
         z = None
         for epoch in range(args.graph_AE_epoch):
             z = geng.train_step(xin, T, Tt, t_perm, labels)                         # loss_function: plain BCE (scgnn2.py:581)

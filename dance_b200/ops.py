@@ -495,6 +495,33 @@ def _head_width(W: int, nheads: int, what: str) -> int:
     return W // nheads
 
 
+def _drop_prob(p) -> float:
+    """nn.Dropout's check: a probability outside [0, 1] is a ValueError."""
+    p = float(p)
+    if not 0.0 <= p <= 1.0:
+        raise ValueError(f"dropout probability has to be between 0 and 1, but got {p}")
+    return p
+
+
+def dropout(x, p: float, seed: int, key: int, out=None):
+    """Inverted dropout of a 2-D (strided) matrix: ``out[r, c] = x[r, c] / (1 - p)`` where keep(seed, key, r, c), else 0.
+
+    The keep bit is a counter-based draw (independent Bernoulli(1 - p) per element; see include/dance_b200.h), so calling this
+    again with the same (seed, key) applies the same mask — which is how a backward pass drops its gradient.  ``out`` may be
+    ``x`` (in place).  Over an [nnz, nheads] tensor with a GAT layer's attention key it materialises that layer's attention
+    mask (scaled): entry (p, h) is the keep bit of the edge at CSR position p and head h."""
+    _chk(x, torch.float32, "x", 2)
+    p = _drop_prob(p)
+    if out is None:
+        out = torch.empty(x.shape, dtype=torch.float32, device=x.device)
+    _chk(out, torch.float32, "out", 2)
+    if tuple(out.shape) != tuple(x.shape):
+        raise B2Error(f"dropout: out has shape {tuple(out.shape)}, expected {tuple(x.shape)}")
+    check(lib().b2_dropout_f32(_p(x), _rowmajor(x, "x"), x.shape[0], x.shape[1], p, int(seed) & 0xFFFFFFFF, int(key) & 0xFFFFFFFF,
+                               _p(out), _rowmajor(out, "out"), _stream()), "b2_dropout_f32")
+    return out
+
+
 def gat_scores(H, a_src, a_trg, nheads: int):
     """s_src[n,h] = <H[n,h,:], a_src[h,:]> (scgnn2.py:1016-1017)."""
     _chk(H, torch.float32, "H", 2)
@@ -508,11 +535,15 @@ def gat_scores(H, a_src, a_trg, nheads: int):
 
 
 def gat_aggregate_fwd(T: CSR, H, s_src, s_trg, nheads: int, score_act="leakyrelu", slope=0.2, shift="global",
-                      out=None, keep_alpha=True):
+                      out=None, keep_alpha=True, dropout: float = 0.0, seed: Optional[int] = None, key: int = 0):
     """Fused edge softmax + aggregate on the target-indexed CSR ``T``; returns (out, alpha, gmax).
 
     ``gmax`` [1] is the global shift (``shift="global"``; -inf for a graph without edges) and is what
-    :func:`gat_aggregate_bwd` needs to differentiate through it."""
+    :func:`gat_aggregate_bwd` needs to differentiate through it.
+
+    ``seed`` given: attention dropout (scgnn2.py:1029) — ``out[v] = Σ drop(α)_e H[u]`` with the keep bit of (edge at CSR
+    position p, head h) drawn as :func:`dropout` draws element (p, h) under (seed, key).  ``alpha`` stays undropped; pass
+    the same (dropout, seed, key) to :func:`gat_aggregate_bwd`."""
     n, W = H.shape
     F = _head_width(W, nheads, "gat_aggregate_fwd")
     if out is None:
@@ -524,18 +555,26 @@ def gat_aggregate_fwd(T: CSR, H, s_src, s_trg, nheads: int, score_act="leakyrelu
         check(lib().b2_gat_edge_max_f32(_p(T.rowptr), colidx, _p(s_src), _p(s_trg), n, nheads, act, slope, _p(gmax),
                                         _stream()), "b2_gat_edge_max_f32")
     alpha = torch.empty((T.nnz, nheads), dtype=torch.float32, device=H.device) if keep_alpha else None
-    check(lib().b2_gat_aggregate_fwd_f32(_p(T.rowptr), colidx, _p(H), _rowmajor(H, "H"), _p(s_src), _p(s_trg), n, nheads,
-                                         F, act, slope, sm, _p(gmax), _p(out), _rowmajor(out, "out"), _p(alpha) if T.nnz else None,
-                                         _stream()), "b2_gat_aggregate_fwd_f32")
+    head = (_p(T.rowptr), colidx, _p(H), _rowmajor(H, "H"), _p(s_src), _p(s_trg), n, nheads, F, act, slope, sm, _p(gmax), _p(out),
+            _rowmajor(out, "out"), _p(alpha) if T.nnz else None)
+    if seed is not None:
+        check(lib().b2_gat_aggregate_fwd_drop_f32(*head, _drop_prob(dropout), int(seed) & 0xFFFFFFFF, int(key) & 0xFFFFFFFF,
+                                                  _stream()), "b2_gat_aggregate_fwd_drop_f32")
+    elif dropout:
+        raise ValueError("gat_aggregate_fwd: attention dropout needs a seed")
+    else:
+        check(lib().b2_gat_aggregate_fwd_f32(*head, _stream()), "b2_gat_aggregate_fwd_f32")
     return out, alpha, gmax
 
 
 def gat_aggregate_bwd(T: CSR, Tt: CSR, t_perm, H, a_src, a_trg, s_src, s_trg, alpha, dOut, nheads: int,
-                      score_act="leakyrelu", slope=0.2, H2=None, dOut2=None, want_dH2=True, gmax=None):
+                      score_act="leakyrelu", slope=0.2, H2=None, dOut2=None, want_dH2=True, gmax=None, dropout: float = 0.0,
+                      seed: Optional[int] = None, key: int = 0):
     """Returns (dH, da_src, da_trg), or (dH, da_src, da_trg, dH2 | None) with a tied second layer (H2, dOut2).
 
     ``gmax``: the forward's global shift (third result of :func:`gat_aggregate_fwd` with ``shift="global"``), whose
-    gradient the backward then includes, as the reference does not detach its max; None for ``shift="segment"``."""
+    gradient the backward then includes, as the reference does not detach its max; None for ``shift="segment"``.
+    ``dropout`` / ``seed`` / ``key``: the forward's attention dropout (not with a tied layer); ``alpha`` is the undropped α."""
     n, W = H.shape
     F = _head_width(W, nheads, "gat_aggregate_bwd")
     dev = H.device
@@ -550,34 +589,62 @@ def gat_aggregate_bwd(T: CSR, Tt: CSR, t_perm, H, a_src, a_trg, s_src, s_trg, al
     edge = (lambda t: _p(t)) if T.nnz else (lambda t: _p(T.rowptr))
     head = (_p(T.rowptr), edge(T.colidx), _p(Tt.rowptr), edge(Tt.colidx), edge(t_perm), _p(H), _rowmajor(H, "H"), _p(a_src),
             _p(a_trg), _p(s_src), _p(s_trg), edge(alpha), _p(dOut), _rowmajor(dOut, "dOut"))
+    if seed is None and dropout:
+        raise ValueError("gat_aggregate_bwd: attention dropout needs a seed")
     if H2 is not None:
+        if seed is not None:
+            raise B2Error("gat_aggregate_bwd: the tied (STAGATE) backward has no attention dropout")
         dH2 = torch.empty((n, W), dtype=torch.float32, device=dev) if want_dH2 else None
         check(lib().b2_gat_aggregate_bwd_tied_f32(*head, _p(H2), _rowmajor(H2, "H2"), _p(dOut2), _rowmajor(dOut2, "dOut2"), n, nheads,
                                                   F, SCORE_ACT[score_act], slope, _p(gmax), _p(dH), _rowmajor(dH, "dH"), _p(dH2),
                                                   _rowmajor(dH2, "dH2") if want_dH2 else 0, _p(da_src), _p(da_trg), _p(ds_s), _p(ds_t),
                                                   _p(dpre), _p(shift_ws), _stream()), "b2_gat_aggregate_bwd_tied_f32")
         return dH, da_src, da_trg, dH2
-    check(lib().b2_gat_aggregate_bwd_f32(*head, n, nheads, F, SCORE_ACT[score_act], slope, _p(gmax), _p(dH), _rowmajor(dH, "dH"),
-                                         _p(da_src), _p(da_trg), _p(ds_s), _p(ds_t), _p(dpre), _p(shift_ws), _stream()),
-          "b2_gat_aggregate_bwd_f32")
+    tail = (n, nheads, F, SCORE_ACT[score_act], slope, _p(gmax), _p(dH), _rowmajor(dH, "dH"), _p(da_src), _p(da_trg), _p(ds_s),
+            _p(ds_t), _p(dpre), _p(shift_ws))
+    if seed is not None:
+        check(lib().b2_gat_aggregate_bwd_drop_f32(*head, *tail, _drop_prob(dropout), int(seed) & 0xFFFFFFFF, int(key) & 0xFFFFFFFF,
+                                                  _stream()), "b2_gat_aggregate_bwd_drop_f32")
+    else:
+        check(lib().b2_gat_aggregate_bwd_f32(*head, *tail, _stream()), "b2_gat_aggregate_bwd_f32")
     return dH, da_src, da_trg
 
 
-def gat_combine_fwd(agg, skip, bias, nheads: int, concat: bool, act=None):
+def gat_combine_fwd(agg, skip, bias, nheads: int, concat: bool, act=None, identity: bool = False):
+    """``identity``: ``skip`` is the layer's raw input [n, F], added to every head (GATLayer with FIN == FOUT,
+    scgnn2.py:1167-1171); otherwise ``skip`` is [n, nheads*F] or None."""
     n, W = agg.shape
     F = _head_width(W, nheads, "gat_combine_fwd")
     out = torch.empty((n, W if concat else F), dtype=torch.float32, device=agg.device)
+    if identity:
+        _chk(skip, torch.float32, "skip", 2)
+        if tuple(skip.shape) != (n, F):
+            raise B2Error(f"gat_combine_fwd: an identity skip must have shape {(n, F)}, got {tuple(skip.shape)}")
+        check(lib().b2_gat_combine_fwd_identity_f32(_p(agg), _rowmajor(agg, "agg"), _p(skip), _rowmajor(skip, "skip"), _p(bias), n, nheads,
+                                                    F, int(concat), ACT[act], _p(out), _rowmajor(out, "out"), _stream()),
+              "b2_gat_combine_fwd_identity_f32")
+        return out
     check(lib().b2_gat_combine_fwd_f32(_p(agg), _rowmajor(agg, "agg"), _p(skip), _rowmajor(skip, "skip") if skip is not None else 0,
                                        _p(bias), n, nheads, F, int(concat), ACT[act], _p(out), _rowmajor(out, "out"), _stream()),
           "b2_gat_combine_fwd_f32")
     return out
 
 
-def gat_combine_bwd(dout, out, nheads: int, F: int, concat: bool, act=None):
-    """Returns (dpre [n, nheads*F], dact [n, out width])."""
+def gat_combine_bwd(dout, out, nheads: int, F: int, concat: bool, act=None, identity: bool = False, dpre=None, dx_skip=None):
+    """Returns (dpre [n, nheads*F], dact [n, out width]); with ``identity`` also dx_skip [n, F] = Σ_h dpre[:, h·F:(h+1)·F],
+    the identity skip's gradient of the layer input.  ``dpre`` / ``dx_skip``: optional (strided) output buffers."""
     n = dout.shape[0]
-    dpre = torch.empty((n, nheads * F), dtype=torch.float32, device=dout.device)
+    if dpre is None:
+        dpre = torch.empty((n, nheads * F), dtype=torch.float32, device=dout.device)
     dact = torch.empty_like(out)
+    if identity:
+        if dx_skip is None:
+            dx_skip = torch.empty((n, F), dtype=torch.float32, device=dout.device)
+        check(lib().b2_gat_combine_bwd_identity_f32(_p(dout), _rowmajor(dout, "dout"), _p(out), _rowmajor(out, "out"), n, nheads, F,
+                                                    int(concat), ACT[act], _p(dpre), _rowmajor(dpre, "dpre"), _p(dact),
+                                                    _rowmajor(dact, "dact"), _p(dx_skip), _rowmajor(dx_skip, "dx_skip"), _stream()),
+              "b2_gat_combine_bwd_identity_f32")
+        return dpre, dact, dx_skip
     check(lib().b2_gat_combine_bwd_f32(_p(dout), _rowmajor(dout, "dout"), _p(out), _rowmajor(out, "out"), n, nheads, F,
                                        int(concat), ACT[act], _p(dpre), _rowmajor(dpre, "dpre"), _p(dact), _rowmajor(dact, "dact"),
                                        _stream()), "b2_gat_combine_bwd_f32")

@@ -324,6 +324,43 @@ int b2_gat_combine_fwd_f32(const float* agg, int64_t ldagg, const float* skip, i
 int b2_gat_combine_bwd_f32(const float* dout, int64_t lddo, const float* out, int64_t ldo,
                            int32_t n, int32_t nheads, int32_t F, int concat, int act,
                            float* dpre, int64_t ldp, float* dact, int64_t ldact, void* stream);
+/* Identity skip (GATLayer with FIN == FOUT, scgnn2.py:1167-1171: the raw input x [n, F] is added to every head):
+ *   forward as b2_gat_combine_fwd_f32 with skip[n, h*F + f] = x[n, f];
+ *   backward as b2_gat_combine_bwd_f32, plus dx_skip[n, F] = Σ_h dpre[n, h*F:(h+1)*F] (overwritten). */
+int b2_gat_combine_fwd_identity_f32(const float* agg, int64_t ldagg, const float* x, int64_t ldx, const float* bias,
+                                    int32_t n, int32_t nheads, int32_t F, int concat, int act,
+                                    float* out, int64_t ldo, void* stream);
+int b2_gat_combine_bwd_identity_f32(const float* dout, int64_t lddo, const float* out, int64_t ldo,
+                                    int32_t n, int32_t nheads, int32_t F, int concat, int act,
+                                    float* dpre, int64_t ldp, float* dact, int64_t ldact,
+                                    float* dx_skip, int64_t ldx, void* stream);
+
+/* Dropout (scGNN GATLayer, scgnn2.py:1005 / :1010 / :1029: one nn.Dropout(p) at the input, the projection and the
+ * attention coefficients).  Keep bits are counter-based, keep(seed, key, r, c) = uniform01(seed, key, r, c) >= p with the
+ * hash of CellwiseMaskData: the masks follow torch's distribution (independent Bernoulli(1 - p), kept values scaled by
+ * 1 / (1 - p), p = 1 gives zeros) but are not torch's masks.  The backward regenerates them from the same (seed, key).
+ *   b2_dropout_f32 : y[r, c] = keep(r, c) ? x[r, c] / (1 - p) : 0 over a strided [rows, cols] matrix; y may be x.
+ *   b2_gat_aggregate_fwd_drop_f32 / _bwd_drop_f32 : the aggregate and its backward with α' = drop(α) on (edge, head),
+ *     r = the edge's position in the target CSR, c = the head; alpha_out stays the UNDROPPED α, which is what the
+ *     backward takes.  nheads <= 32.  drop_p = 0 gives the results of the plain entry points bit for bit.
+ *   0 <= p <= 1, otherwise an error. */
+int b2_dropout_f32(const float* x, int64_t ldx, int64_t rows, int32_t cols, float p, uint32_t seed, uint32_t key,
+                   float* y, int64_t ldy, void* stream);
+int b2_gat_aggregate_fwd_drop_f32(const int32_t* rowptr, const int32_t* colidx,
+                                  const float* H, int64_t ldh, const float* s_src, const float* s_trg,
+                                  int32_t n, int32_t nheads, int32_t F,
+                                  int score_act, float slope, int shift_mode, const float* gmax_dev,
+                                  float* out, int64_t ldo, float* alpha_out,
+                                  float drop_p, uint32_t seed, uint32_t key, void* stream);
+int b2_gat_aggregate_bwd_drop_f32(const int32_t* rowptr, const int32_t* colidx,
+                                  const int32_t* t_rowptr, const int32_t* t_colidx, const int32_t* t_perm,
+                                  const float* H, int64_t ldh, const float* a_src, const float* a_trg,
+                                  const float* s_src, const float* s_trg, const float* alpha,
+                                  const float* dOut, int64_t lddo, int32_t n, int32_t nheads, int32_t F,
+                                  int score_act, float slope, const float* gmax_dev,
+                                  float* dH, int64_t lddh, float* da_src, float* da_trg,
+                                  float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws, float* shift_ws,
+                                  float drop_p, uint32_t seed, uint32_t key, void* stream);
 
 /* ------------------------------------------------------------------------
  * NeighborGraph connectivities (transforms/graph/neighbor_graph.py:50-57 → scanpy.pp.neighbors(method="umap") →

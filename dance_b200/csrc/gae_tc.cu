@@ -16,12 +16,15 @@
 //                          tile above it counts its loss twice and also yields dZ_J += Gᵀ · Z_I: G goes to shared memory as
 //                          hi / lo planes of Gᵀ (K-major in i, the A operand) and Z_Iᵀ is the B operand.  Both dZ products
 //                          issue their three products as two: hi·hi and hi·lo as one m64n(2·DP)k8 against a B operand laid
-//                          out [hi | lo], and lo·hi.  The tile's dZ_J leaves through red.global.add.
+//                          out [hi | lo], and lo·hi.  dZ_J runs on a fourth warpgroup of its own (below).
 //
 // Schedule: each product is issued as one batch of wgmmas with one commit and one wait, which needs S, both halves of G and
 // the dZ accumulators live in registers at once; the producer warpgroup gives its registers to the consumers (setmaxnreg) to
 // make room.  The two consumer warpgroups run out of phase ("ping-pong"): while one does σ / softplus on the SFU, the other's
 // products run on the tensor cores.  Tiles with no masked logit take an elementwise loop without the per-logit mask.
+// Triangle: the consumers' turns hold S and dZ_I only.  A dZ_J warpgroup takes each consumer warpgroup's Gᵀ through an
+// mbarrier pair (Gᵀ full / Gᵀ empty), issues both halves of a tile's dZ_J (K = warpgroup 0's rows, then warpgroup 1's) into
+// the same accumulators in turn, adds the halves in fp32 and sends the tile's sum to dz with one set of red.global.add.
 //
 // Register fragment trick: the accumulator of S gives a thread columns (2t, 2t+1) of each 8-column block, the tf32 A fragment
 // wants columns (t, t+4).  The sum over j does not care about order, so the 8 columns of each block are fed to the second
@@ -46,9 +49,17 @@ using namespace tc;
 constexpr int BT = 128;                 // rows per block / workspace tile
 constexpr int CONSUMERS = 256;          // two warpgroups
 constexpr int THREADS = CONSUMERS + 128; // + producer warpgroup
+constexpr int TRI_THREADS = THREADS + 128; // triangle: + dZ_J warpgroup
 // Register split (setmaxnreg): the consumers hold S, both halves of G and the dZ accumulators while a dZ batch is in flight.
-// 128 · 40 + 256 · 232 = 64 512 of the 65 536 registers of an SM.
+// Full sweep: 128 · 40 + 256 · 232 = 64 512 of the 65 536 registers of an SM.
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+// Triangle: producer 24, dZ_J warpgroup DJ (its accumulators and the tile's fp32 sum), consumers (no dZ_J accumulators).
+template <int DP>
+struct TriRegs {
+  static constexpr int PRODUCER = 24, DJ = DP <= 16 ? 80 : 96, CONSUMER = DP <= 16 ? 200 : 192;
+};
+static_assert(128 * (TriRegs<16>::PRODUCER + TriRegs<16>::DJ + 2 * TriRegs<16>::CONSUMER) <= 65536 &&
+              128 * (TriRegs<32>::PRODUCER + TriRegs<32>::DJ + 2 * TriRegs<32>::CONSUMER) <= 65536, "triangle registers");
 constexpr int STAGES = 3;
 constexpr int MAX_D = 32;
 constexpr uint32_t ZS_BYTES = BT * 128; // one plane of a tile for S (K-major, 128-byte rows)
@@ -69,7 +80,7 @@ struct Tiles {
   static constexpr uint32_t ZIT = TRI ? zt_bytes<DP>() : 0;       // one plane of Z_Iᵀ
   static constexpr uint32_t GT = TRI ? 64 * 64 * 4 : 0;           // one plane of a warpgroup's Gᵀ: 64 j x 64 i, 2 atoms
   static constexpr uint32_t RING = ZS_PLANES * ZS_BYTES + 2 * ZIT + 4 * GT;
-  static constexpr size_t SMEM = RING + STAGES * STAGE + 16 * STAGES + 1024;
+  static constexpr size_t SMEM = RING + STAGES * STAGE + 16 * STAGES + (TRI ? 32 : 0) + 1024;   // + Gᵀ full / empty x 2
 };
 static_assert(Tiles<MAX_D, false>::SMEM <= MAX_SMEM && Tiles<MAX_D, true>::SMEM <= MAX_SMEM, "decoder shared memory");
 
@@ -172,6 +183,16 @@ __device__ __forceinline__ float sigmoid_softplus(float (&S)[V], float (&L)[V], 
   return relu + LN2 * (lg + lg2_approx(prod));
 }
 
+// Triangle: sum of a tile's merged dZ accumulators for output element v: columns c (hi·hi) and c + DP (hi·lo) sit DP / 2
+// elements apart, s holds lo·hi
+template <int NBM, int DP>
+__device__ __forceinline__ float merged(const float (&acc)[NBM][DP], const float (&s)[DP / 2], int v) {
+  float t = s[v];
+#pragma unroll
+  for (int b = 0; b < NBM; ++b) t += acc[b][v] + acc[b][v + DP / 2];
+  return t;
+}
+
 // The sweep of one work unit; TRI selects the triangle (see header).
 template <int DP, bool TRI>
 __device__ __forceinline__ void decoder_sweep(const Params& p) {
@@ -187,6 +208,8 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   constexpr int NB = DP <= 16 ? 4 : 2;             // full sweep: hi·hi accumulators
   constexpr int NBM = DP <= 16 ? 2 : 1;            // triangle: [hi·hi | hi·lo] accumulators
   const uint32_t full_bar = smem_u32(ring + STAGES * T::STAGE), empty_bar = full_bar + 8 * STAGES;
+  // triangle: per consumer warpgroup, "its Gᵀ is written" (4 warp arrivals) and "its Gᵀ may be overwritten" (4 dZ_J warps)
+  const uint32_t gt_full = empty_bar + 8 * STAGES, gt_empty = gt_full + 16;
 
   // ---- work unit ----
   int row0, row_end, dz_row0, jt0, jt1;
@@ -210,18 +233,92 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   if (jt0 >= jt1) return;
   const int nt = jt1 - jt0;
   const int diag_end = (row0 + BT) / JW;                 // triangle: tiles below this one are the diagonal block's
+  const int handed0 = max(jt0, diag_end) - jt0;          // triangle: tiles handed0 .. nt − 1 yield dZ_J
 
   const int tid = threadIdx.x;
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar + 8 * s, 1); mbar_init(empty_bar + 8 * s, CONSUMERS / 32); }
+    if constexpr (TRI) {
+      for (int w = 0; w < 2; ++w) { mbar_init(gt_full + 8 * w, 4); mbar_init(gt_empty + 8 * w, 4); }
+    }
     fence_barrier_init();
   }
   __syncthreads();
 
+  if constexpr (TRI) {
+    if (tid >= THREADS) {
+      // ===================== dZ_J warpgroup =====================
+      // dZ_J += Gᵀ · Z_I of every tile above the diagonal block, both consumer warpgroups' halves (K = their 64 rows i) in
+      // turn into the same accumulators as one warpgroup's used to, each half summed into an fp32 total; the tile's total
+      // then goes to dz with one set of reductions.  A consumer's Gᵀ planes are handed over through gt_full / gt_empty.
+      asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TriRegs<DP>::DJ));
+      if (handed0 >= nt) return;
+      const int t = tid - THREADS, warp = t >> 5, lane = t & 31;
+      // Z_Iᵀ (B of dZ_J), per consumer warpgroup 2 atoms of [DP hi rows | DP lo rows] x 32 i in the gt_pos order; rows past the
+      // range are zero
+      for (int e = t; e < BT * DP; e += 128) {
+        const int r = e / DP, k = e % DP;
+        const int row = row0 + r;
+        const float v = (row < row_end && k < p.d) ? p.z[(int64_t)row * p.ldz + k] : 0.f;
+        const float h = tf32_trunc(v);
+        const int q = gt_pos(r & 63);
+        const uint32_t ot = (uint32_t)(r >> 6) * (4 * ATOM) + (uint32_t)(q >> 5) * (2 * ATOM) + sw128_offset32((uint32_t)k, (uint32_t)(q & 31));
+        *reinterpret_cast<float*>(zit + ot) = h;
+        *reinterpret_cast<float*>(zit + ot + ATOM) = v - h;
+      }
+      fence_proxy_async();
+      asm volatile("bar.sync 4, 128;" ::: "memory");
+      const bool vec = (p.d & 1) == 0 && (reinterpret_cast<uintptr_t>(p.dz) & 7) == 0;
+      const float c2 = 2.f * p.coef;
+      float djm[NBM][DP], djs[DP / 2], djt[DP / 2];
+      for (int i = handed0; i < nt; ++i) {
+        const uint32_t parity = (uint32_t)((i - handed0) & 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          mbar_wait(gt_full + 8 * h, parity);
+          const uint32_t ag_hi = smem_u32(zit + 2 * T::ZIT + h * 2 * T::GT), ag_lo = ag_hi + T::GT;
+          const uint32_t bi = smem_u32(zit) + h * (4 * ATOM);
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < 64 / 8; ++kk) {
+            const uint32_t oa = (uint32_t)(kk >> 2) * (64 * 128) + (uint32_t)(kk & 3) * 32;
+            const uint32_t ob = (uint32_t)(kk >> 2) * (2 * ATOM) + (uint32_t)(kk & 3) * 32;
+            mma_ss<DP>(djs, wgmma_desc_sw128(ag_lo + oa), wgmma_desc_sw128(bi + ob), kk > 0);
+            mma_ss<2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + oa), wgmma_desc_sw128(bi + ob), kk >= NBM);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(djs);
+#pragma unroll
+          for (int b = 0; b < NBM; ++b) reg_fence(djm[b]);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(gt_empty + 8 * h);     // this warpgroup's Gᵀ is read
+#pragma unroll
+          for (int v = 0; v < DP / 2; ++v) djt[v] = (h ? djt[v] : 0.f) + merged(djm, djs, v);
+        }
+        const int ja = (jt0 + i) * JW + warp * 16 + (lane >> 2);
+#pragma unroll
+        for (int v = 0; v < DP / 2; v += 2) {
+          const int row = ja + 8 * ((v >> 1) & 1);
+          const int col = 8 * (v >> 2) + 2 * (lane & 3);
+          if (row >= p.n || col >= p.d) continue;
+          float* dst = p.dz + (int64_t)row * p.d + col;
+          if (vec) {
+            atomicAdd(reinterpret_cast<float2*>(dst), make_float2(c2 * djt[v], c2 * djt[v + 1]));
+          } else {
+            atomicAdd(dst, c2 * djt[v]);
+            if (col + 1 < p.d) atomicAdd(dst + 1, c2 * djt[v + 1]);
+          }
+        }
+      }
+      return;
+    }
+  }
+
   if (tid >= CONSUMERS) {
     // ===================== producer warpgroup =====================
     // One thread issues the copies; the warpgroup exists so that it can hand its registers to the consumers.
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TRI ? TriRegs<DP>::PRODUCER : PRODUCER_REGS));
     if (tid == CONSUMERS) {
       for (int i = 0; i < nt; ++i) {
         const int s = i % STAGES;
@@ -247,9 +344,8 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   }
 
   // ===================== consumers =====================
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
-  // Z_I planes from z (rows past the range are zero: their logits are masked below); the triangle also builds Z_Iᵀ, per
-  // warpgroup 2 atoms of [DP hi rows | DP lo rows] x 32 i in the gt_pos order
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(TRI ? TriRegs<DP>::CONSUMER : CONSUMER_REGS));
+  // Z_I planes from z (rows past the range are zero: their logits are masked below)
   for (int e = tid; e < BT * DP; e += CONSUMERS) {
     const int r = e / DP, k = e % DP;
     const int row = row0 + r;
@@ -258,12 +354,6 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
     const uint32_t o = sw128_offset32((uint32_t)r, (uint32_t)k);
     *reinterpret_cast<float*>(zi_hi + o) = h;
     *reinterpret_cast<float*>(zi_lo + o) = v - h;
-    if constexpr (TRI) {
-      const int q = gt_pos(r & 63);
-      const uint32_t ot = (uint32_t)(r >> 6) * (4 * ATOM) + (uint32_t)(q >> 5) * (2 * ATOM) + sw128_offset32((uint32_t)k, (uint32_t)(q & 31));
-      *reinterpret_cast<float*>(zit + ot) = h;
-      *reinterpret_cast<float*>(zit + ot + ATOM) = v - h;
-    }
   }
   fence_proxy_async();
   asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");
@@ -276,10 +366,9 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   const bool live_a = ra < row_end, live_b = ra + 8 < row_end;
   const uint32_t ai_hi = smem_u32(zi_hi) + wg * 64 * 128, ai_lo = smem_u32(zi_lo) + wg * 64 * 128;
   const bool full_rows = row0 + BT <= row_end;                   // no dead rows in this block: only the last J tile is masked
-  // triangle: this warpgroup's Gᵀ planes (A of dZ_J) and Z_Iᵀ (B of dZ_J)
+  // triangle: this warpgroup's Gᵀ planes (A of dZ_J)
   uint8_t* gt_hi = zit + 2 * T::ZIT + wg * 2 * T::GT;
   uint8_t* gt_lo = gt_hi + T::GT;
-  const uint32_t bi = smem_u32(zit) + wg * (4 * ATOM);
   const float c2 = 2.f * p.coef;
 
   // The accumulation inside the tensor core truncates, and the hi·hi product carries almost all of dZ: over a whole J sweep one
@@ -287,9 +376,9 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   // several accumulators (at most 4 k-steps each for DP ≤ 16, 8 at DP = 32), the cross terms into one more, and the tile's sum
   // joins an fp32 total with round-to-nearest adds.  The full sweep issues the three products at N = DP (NB accumulators for
   // hi·hi).  The triangle has twice the dZ products per logit and issues fewer, wider ones: hi·hi and hi·lo as one N = 2·DP
-  // product against [hi | lo] of the B operand (NBM accumulators), lo·hi alone; the same for dZ_J.
+  // product against [hi | lo] of the B operand (NBM accumulators), lo·hi alone; the same for dZ_J (dZ_J warpgroup).
   float dzb[TRI ? 1 : NB][DP / 2], dzs[DP / 2], dzt[DP / 2];
-  float dzm[TRI ? NBM : 1][DP], djm[TRI ? NBM : 1][DP], djs[DP / 2];
+  float dzm[TRI ? NBM : 1][DP];
 #pragma unroll
   for (int v = 0; v < DP / 2; ++v) dzt[v] = 0.f;
   double loss = 0.0;
@@ -298,16 +387,15 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   // S product of the next one, each issued as one batch with one commit (named barrier 2 + wg means "wg may issue"), and the
   // warpgroup works through σ / softplus of its S while the other one's products run.  Warpgroup 0 takes the first turn.  Each
   // warpgroup takes nt + 1 turns and passes nt of them on; warpgroup 0 passes its last one as well, so that every bar.arrive
-  // meets one bar.sync.  The bar.sync of a turn also orders this warpgroup's Gᵀ stores before the dZ_J product that reads them.
+  // meets one bar.sync.  In the triangle a turn holds dZ_I only: dZ_J of the tile runs on the dZ_J warpgroup, which takes each
+  // warpgroup's Gᵀ through gt_full and gives it back through gt_empty once its wgmmas have retired.
   //   Full sweep: the dZ batch is waited for before S is issued into the same registers, and the turn passes on once S is done.
-  //   Triangle at DP = 16 and 32: the same, but the turn passes on as soon as S is committed, so that the other warpgroup's
-  //     dZ batch queues behind it instead of waiting for it to finish.
-  //   Triangle at DP = 8 (OVERLAP): S alternates between two accumulators, so the dZ batch of tile i − 1 (A = the previous S
-  //     and L) and the S batch of tile i go out back to back and the turn passes on once both are committed; the tensor pipe
-  //     does not drain within a turn.  wait<1> then retires dZ while S still runs.  At DP = 32 the second accumulator makes
-  //     ptxas spill in the consumer loop.  At DP = 16 it fits with one [hi·hi | hi·lo] accumulator but measured slower than
-  //     one S accumulator (DESIGN §4.1), so DP = 16 and 32 keep one.
-  constexpr bool OVERLAP = TRI && DP <= 8;
+  //   Triangle (OVERLAP): S alternates between two accumulators, so the dZ_I batch of tile i − 1 (A = the previous S and L) and
+  //     the S batch of tile i go out back to back and the turn passes on once both are committed; the tensor pipe does not
+  //     drain within a turn, and the other warpgroup's batches queue behind them.  wait<1> then retires dZ_I while S still
+  //     runs.  With dZ_J on its own warpgroup the second accumulator fits at every DP without spills, and it measured faster
+  //     than one S accumulator at DP = 16 and 32 as well (DESIGN §4.1).
+  constexpr bool OVERLAP = TRI;
   float S[JW / 2], L[JW / 2];   // S: accumulator of S, then the hi part of G; L: the lo part of G
   auto take_turn = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(2 + wg), "n"(CONSUMERS) : "memory"); };
   auto pass_turn = [&]() { asm volatile("bar.arrive %0, %1;" ::"r"(3 - wg), "n"(CONSUMERS) : "memory"); };
@@ -327,9 +415,8 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
     }
     wgmma_commit();
   };
-  // dZ_I += G · Z_J of tile i with A = (S, L) from the registers, and in the triangle dZ_J += Gᵀ · Z_I (on the diagonal block
-  // it is computed and dropped); one batch, committed (the caller waits, then dz_fence).  Full sweep: 3·16 products; triangle:
-  // 2·8 + 2·8.
+  // dZ_I += G · Z_J of tile i with A = (S, L) from the registers; one batch, committed (the caller waits, then dz_fence).
+  // Full sweep: 3·16 products; triangle: 2·8.
   auto issue_dz = [&](int i, float (&S)[JW / 2]) {
     const uint32_t bt_hi = smem_u32(ring + (i % STAGES) * T::STAGE) + 2 * T::JS, bt_lo = bt_hi + T::JT;
     wgmma_fence();
@@ -351,37 +438,19 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
         mma_rs<DP>(dzb[kb % NB], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NB);
       }
     }
-    if constexpr (TRI) {
-      const uint32_t ag_hi = smem_u32(gt_hi), ag_lo = smem_u32(gt_lo);
-#pragma unroll
-      for (int kk = 0; kk < 64 / 8; ++kk) {
-        const uint32_t oa = (uint32_t)(kk >> 2) * (64 * 128) + (uint32_t)(kk & 3) * 32;
-        const uint32_t ob = (uint32_t)(kk >> 2) * (2 * ATOM) + (uint32_t)(kk & 3) * 32;
-        mma_ss<DP>(djs, wgmma_desc_sw128(ag_lo + oa), wgmma_desc_sw128(bi + ob), kk > 0);
-        mma_ss<2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + oa), wgmma_desc_sw128(bi + ob), kk >= NBM);
-      }
-    }
     wgmma_commit();
   };
   auto dz_fence = [&]() {
     reg_fence(dzs);
     if constexpr (TRI) {
 #pragma unroll
-      for (int b = 0; b < NBM; ++b) { reg_fence(dzm[b]); reg_fence(djm[b]); }
-      reg_fence(djs);
+      for (int b = 0; b < NBM; ++b) reg_fence(dzm[b]);
     } else {
 #pragma unroll
       for (int b = 0; b < NB; ++b) reg_fence(dzb[b]);
     }
   };
-  // sum of a tile's merged accumulators for output element v: columns c (hi·hi) and c + DP (hi·lo) sit DP / 2 elements apart
-  auto merged = [&](const float (&acc)[TRI ? NBM : 1][DP], const float (&s)[DP / 2], int v) {
-    float t = s[v];
-#pragma unroll
-    for (int b = 0; b < NBM; ++b) t += acc[b][v] + acc[b][v + DP / 2];
-    return t;
-  };
-  // the tile's dZ_I joins the fp32 total, its dZ_J (above the diagonal block) goes to dz, and its stage goes back to the producer
+  // the tile's dZ_I joins the fp32 total and its stage goes back to the producer
   auto retire_dz = [&](int i) {
 #pragma unroll
     for (int v = 0; v < DP / 2; ++v) {
@@ -394,49 +463,37 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
         dzt[v] += t;
       }
     }
-    if constexpr (TRI) {
-      if (jt0 + i >= diag_end) {
-        const int ja = (jt0 + i) * JW + warp * 16 + (lane >> 2);
-        const bool vec = (p.d & 1) == 0 && (reinterpret_cast<uintptr_t>(p.dz) & 7) == 0;
-#pragma unroll
-        for (int v = 0; v < DP / 2; v += 2) {
-          const int row = ja + 8 * ((v >> 1) & 1);
-          const int col = 8 * (v >> 2) + 2 * (lane & 3);
-          const float x = merged(djm, djs, v), y = merged(djm, djs, v + 1);
-          if (row >= p.n || col >= p.d) continue;
-          float* dst = p.dz + (int64_t)row * p.d + col;
-          if (vec) {
-            atomicAdd(reinterpret_cast<float2*>(dst), make_float2(c2 * x, c2 * y));
-          } else {
-            atomicAdd(dst, c2 * x);
-            if (col + 1 < p.d) atomicAdd(dst + 1, c2 * y);
-          }
-        }
-      }
-    }
     __syncwarp();
     if (lane == 0) mbar_arrive(empty_bar + 8 * (i % STAGES));
   };
-  // σ / softplus of tile i on the registers once its S is done; the triangle then writes Gᵀ for dZ_J
+  // σ / softplus of tile i on the registers once its S is done; above the diagonal block the triangle then writes Gᵀ for the
+  // dZ_J warpgroup, once that warpgroup has read the previous one
   auto elementwise = [&](int i, float (&S)[JW / 2]) {
     const int jbase = (jt0 + i) * JW + 2 * (lane & 3);
     const float l = full_rows && (jt0 + i + 1) * JW <= p.n ? sigmoid_softplus<false>(S, L, jbase, p.n, live_a, live_b)
                                                            : sigmoid_softplus<true>(S, L, jbase, p.n, live_a, live_b);
     if constexpr (TRI) {
-      loss += (jt0 + i >= diag_end ? 2.0 : 1.0) * (double)l;   // a tile above the diagonal block stands for its mirror too
-      // column jj of G is row jj of Gᵀ; the thread's rows r, r + 8 sit at K positions gt_pos(r), gt_pos(r) + 1
-      const uint32_t k = (uint32_t)gt_pos(warp * 16 + (lane >> 2));
-      const uint32_t base = (k >> 5) * (64 * 128);
+      if (i >= handed0) {
+        loss += 2.0 * (double)l;   // a tile above the diagonal block stands for its mirror too
+        mbar_wait(gt_empty + 8 * wg, (uint32_t)(((i - handed0) & 1) ^ 1));
+        // column jj of G is row jj of Gᵀ; the thread's rows r, r + 8 sit at K positions gt_pos(r), gt_pos(r) + 1
+        const uint32_t k = (uint32_t)gt_pos(warp * 16 + (lane >> 2));
+        const uint32_t base = (k >> 5) * (64 * 128);
 #pragma unroll
-      for (int c = 0; c < JW / 8; ++c) {
+        for (int c = 0; c < JW / 8; ++c) {
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const uint32_t o = base + sw128_offset32((uint32_t)(8 * c + 2 * (lane & 3) + e), k & 31);
-          sts_v2(smem_u32(gt_hi) + o, S[4 * c + e], S[4 * c + 2 + e]);
-          sts_v2(smem_u32(gt_lo) + o, L[4 * c + e], L[4 * c + 2 + e]);
+          for (int e = 0; e < 2; ++e) {
+            const uint32_t o = base + sw128_offset32((uint32_t)(8 * c + 2 * (lane & 3) + e), k & 31);
+            sts_v2(smem_u32(gt_hi) + o, S[4 * c + e], S[4 * c + 2 + e]);
+            sts_v2(smem_u32(gt_lo) + o, L[4 * c + e], L[4 * c + 2 + e]);
+          }
         }
+        fence_proxy_async();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(gt_full + 8 * wg);
+      } else {
+        loss += (double)l;
       }
-      fence_proxy_async();
     } else {
       loss += (double)l;
     }
@@ -486,26 +543,20 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
       wgmma_wait<0>();
       dz_fence();
     };
-    // The triangle passes the turn on as soon as S is committed, so that the other warpgroup's dZ batch queues behind it; the
-    // full sweep once S is done.
-    auto start_s = [&](int i) {
-      issue_s(i, S);
-      if constexpr (TRI) pass_turn();
-    };
-    // wait for S of tile i, then σ / softplus
+    // wait for S of tile i, pass the turn on, then σ / softplus
     auto finish_s = [&](int i) {
       wgmma_wait<0>();
       reg_fence(S);
-      if constexpr (!TRI) pass_turn();
+      pass_turn();
       elementwise(i, S);
     };
     if (wg == 1) take_turn();
-    start_s(0);
+    issue_s(0, S);
     finish_s(0);
     for (int i = 1; i < nt; ++i) {
       take_turn();
       run_dz(i - 1);
-      start_s(i);          // S runs while the previous tile's dZ is summed
+      issue_s(i, S);       // S runs while the previous tile's dZ is summed
       retire_dz(i - 1);
       finish_s(i);
     }
@@ -539,7 +590,7 @@ gae_allpairs_tc_kernel(const __grid_constant__ Params p) {
 }
 
 template <int DP>
-__global__ void __launch_bounds__(THREADS, 1)
+__global__ void __launch_bounds__(TRI_THREADS, 1)
 gae_tri_tc_kernel(const __grid_constant__ Params p) {
   decoder_sweep<DP, true>(p);
 }
@@ -568,7 +619,7 @@ static int launch_sweep(const Params& p, int units, cudaStream_t st) {
     B2_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_set = true;
   }
-  kernel<<<dim3((unsigned)units, (unsigned)splits), THREADS, smem, st>>>(p);
+  kernel<<<dim3((unsigned)units, (unsigned)splits), TRI ? TRI_THREADS : THREADS, smem, st>>>(p);
   B2_CHECK_LAUNCH(TRI ? "gae_tri_tc_kernel" : "gae_allpairs_tc_kernel");
   return B2_OK;
 }

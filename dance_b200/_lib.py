@@ -43,6 +43,7 @@ _SIGNATURES = {
     "b2_kmeans_workspace_bytes": (c_sz, [c_i32, c_i32]),
     "b2_kmeans_step_f32": (C.c_int, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i32, c_vp, C.c_int, c_vp, c_vp, c_sz, c_vp]),
     "b2_graph_regu_weights_f32": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp]),
+    "b2_graph_regu_weights_weighted_f32": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "b2_celltype_loss_grad_f32": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, C.c_int, c_vp, c_vp, c_vp, c_vp]),
     "b2_l1_grad_add_f32": (C.c_int, [c_vp, c_vp, c_i64, c_f32, c_vp, c_vp]),
     "b2_louvain_csr_host": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_vp, C.POINTER(c_i32), C.POINTER(C.c_double), C.c_int, C.c_double]),
@@ -57,9 +58,14 @@ _SIGNATURES = {
     "b2_gae_loss_workspace_bytes": (c_sz, [c_i32, c_i32]),
     "b2_gae_loss_grad_f32": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_f32, c_f32, C.c_int,
                                        c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_sz, c_vp]),
+    "b2_gae_loss_grad_weighted_f32": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32,
+                                                c_i32, c_f32, c_f32, C.c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_sz, c_vp]),
     "b2_gae_sym_super_blocks": (C.c_int, [c_i32]),
     "b2_gae_loss_grad_sym_f32": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_i32, c_i32, c_i32, c_i32, c_f32, c_f32,
                                            C.c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_sz, c_vp]),
+    "b2_gae_loss_grad_sym_weighted_f32": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32,
+                                                    c_i32, c_i32, c_i32, c_i32, c_f32, c_f32, C.c_int, c_vp, c_vp, c_vp, c_i64, c_vp, c_vp,
+                                                    c_sz, c_vp]),
     "b2_adam_step_f32": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i32, c_vp]),
     "b2_relu_bwd_f32": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_vp]),
     "b2_reparam_fwd_f32": (C.c_int, [c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_i64, c_i64, c_i32, c_vp]),
@@ -69,6 +75,9 @@ _SIGNATURES = {
     "b2_pairwise_l2_dense_f32": (C.c_int, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp]),
     "b2_knn_graph_workspace_bytes": (c_sz, [c_i32, c_i32]),
     "b2_knn_graph_build": (C.c_int, [c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_i64, C.POINTER(c_i64), c_vp, c_sz, c_vp]),
+    "b2_knn_graph_weighted_workspace_bytes": (c_sz, [c_i32, c_i32]),
+    "b2_knn_graph_weighted_build": (C.c_int, [c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i64,
+                                              C.POINTER(c_i64), c_vp, c_sz, c_vp]),
     "b2_gat_scores_f32": (C.c_int, [c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "b2_gat_edge_max_f32": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, C.c_int, c_f32, c_vp, c_vp]),
     "b2_gat_aggregate_fwd_f32": (C.c_int, [c_vp, c_vp, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_i32, C.c_int, c_f32, C.c_int,

@@ -94,6 +94,34 @@ graph_regu_weights_kernel(const int32_t* __restrict__ rowptr, const int32_t* __r
   }
 }
 
+// The same weights for a weighted, directed adj (graph_AE_retain_weights returns W, scgnn2.py:659-670): adjdense[i, j] =
+// colsum_j / rowsum_i, so w_j = colsum_j · Σ_{i∈cluster(j)} 1/rowsum_i; a row with zero sum is masked (np.ma) and adds 0.
+// Diagonal entries are skipped as above.  Pass 1: rowsum_i in column order, colsum_j by fp64 atomics, Σ 1/rowsum per cluster.
+__global__ void __launch_bounds__(256)
+weighted_sums_kernel(const int32_t* __restrict__ rowptr, const int32_t* __restrict__ colidx, const double* __restrict__ vals,
+                     const int32_t* __restrict__ labels, int32_t n, int32_t n_clusters, double* __restrict__ colsum,
+                     double* __restrict__ sums) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    double r = 0.0;
+    for (int32_t q = rowptr[i]; q < rowptr[i + 1]; ++q) {
+      const int32_t j = colidx[q];
+      if (j == (int32_t)i) continue;
+      r += vals[q];
+      atomicAdd(colsum + j, vals[q]);
+    }
+    const int32_t c = labels[i];
+    if (r != 0.0 && c >= 0 && c < n_clusters) atomicAdd(sums + c, 1.0 / r);
+  }
+}
+__global__ void __launch_bounds__(256)
+weighted_regu_weights_kernel(const int32_t* __restrict__ labels, int32_t n, int32_t n_clusters, const double* __restrict__ colsum,
+                             const double* __restrict__ sums, float* __restrict__ w) {
+  for (int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (int64_t)gridDim.x * blockDim.x) {
+    const int32_t c = labels[j];
+    w[j] = (c >= 0 && c < n_clusters) ? (float)(colsum[j] * sums[c]) : 0.f;
+  }
+}
+
 // ---- loss_function_graph("Celltype") --------------------------------------------------------------------------------------
 // pass 1: acc[0] += Σ_j roww_j Σ_g (r−x)²,  acc[1] += Σ_{xd≠0} (xd − r)²      (fp64)
 __global__ void __launch_bounds__(256)
@@ -206,6 +234,22 @@ extern "C" int b2_graph_regu_weights_f32(const int32_t* rowptr, const int32_t* c
   B2_CHECK_LAUNCH("cluster_inv_degree_kernel");
   graph_regu_weights_kernel<<<grid_for(n, 1), 256, 0, st>>>(rowptr, colidx, labels, n, n_clusters, cluster_sums, w);
   B2_CHECK_LAUNCH("graph_regu_weights_kernel");
+  return B2_OK;
+}
+
+extern "C" int b2_graph_regu_weights_weighted_f32(const int32_t* rowptr, const int32_t* colidx, const double* vals, const int32_t* labels,
+                                                  int32_t n, int32_t n_clusters, double* scratch, float* w, void* stream) {
+  using namespace b2;
+  B2_REQUIRE(rowptr && colidx && vals && labels && w && scratch && n_clusters > 0, "b2_graph_regu_weights_weighted_f32: bad arguments");
+  if (n <= 0) return B2_OK;
+  cudaStream_t st = as_stream(stream);
+  double* colsum = scratch;
+  double* sums = scratch + n;
+  B2_CHECK_CUDA(cudaMemsetAsync(scratch, 0, sizeof(double) * ((size_t)n + n_clusters), st));
+  weighted_sums_kernel<<<grid_for(n, 1), 256, 0, st>>>(rowptr, colidx, vals, labels, n, n_clusters, colsum, sums);
+  B2_CHECK_LAUNCH("weighted_sums_kernel");
+  weighted_regu_weights_kernel<<<grid_for(n, 1), 256, 0, st>>>(labels, n, n_clusters, colsum, sums, w);
+  B2_CHECK_LAUNCH("weighted_regu_weights_kernel");
   return B2_OK;
 }
 

@@ -296,10 +296,11 @@ class GraphAEEngine:
         return b["z"], mu, logvar
 
     def train_step(self, x: torch.Tensor, adj: CSR, labels: CSR, norm: float, pos_weight: float, eps: torch.Tensor,
-                   adj_t: Optional[CSR] = None):
+                   adj_t: Optional[CSR] = None, labels_t: Optional[CSR] = None):
         """One epoch of the graph_AE_handler loop (scgnn2.py:575-593): forward, gae_loss_function,
         backward, Adam.  ``adj_t`` = Âᵀ for the backward SpMMs; defaults to Â itself (the
-        preprocess_graph output is symmetric, scgnn2.py:1196).  Loss is left in ``self.loss``
+        preprocess_graph output is symmetric, scgnn2.py:1196).  Real-valued labels (``labels.vals`` set, graph_AE_retain_weights)
+        come with ``labels_t``, the same rows of Lᵀ (see ops.gae_loss_grad).  Loss is left in ``self.loss``
         (under sharding: all-reduced, so every rank holds the global value)."""
         P, G, pr, e = self.params.p, self.params.g, self.precision, self.emb
         adj_t = adj_t or adj
@@ -320,12 +321,12 @@ class GraphAEEngine:
             sb0, sb1 = shard_bounds(ops.gae_sym_super_blocks(n_all), comm.world)[comm.rank]
             dzf = self._bufs.setdefault(("dz_full", n_all), torch.empty(n_all, e, dtype=torch.float32, device=self.device))
             ops.gae_loss_grad_sym(z_all, labels, norm, pos_weight, sb0, sb1, mu, logvar, True, dz_full=dzf, dmu=dmu, dlogvar=dlv,
-                                  loss=self.loss, row_begin=row_begin, n_rows=n_loc)
+                                  loss=self.loss, row_begin=row_begin, n_rows=n_loc, labels_t=labels_t)
             comm.allreduce_sum_(dzf)
             b["dz"].copy_(dzf[row_begin:row_begin + n_loc])
         else:
             ops.gae_loss_grad(z_all, labels, norm, pos_weight, mu, logvar, True, dz=b["dz"], dmu=dmu, dlogvar=dlv, loss=self.loss,
-                              row_begin=row_begin, n_rows=n_loc)
+                              row_begin=row_begin, n_rows=n_loc, labels_t=labels_t)
         ops.reparam_bwd(b["dz"], logvar, eps, dmu, dlv)                  # chain through z = mu + eps·exp(logvar)
         ops.spmm(adj_t, self._gather(b["dml"], "dml"), out=b["ds2"])     # d support2 = Âᵀ · d[mu|logvar]
         ops.gemm(b["h1"], b["ds2"], transA=True, out=G["gc23.weight"], precision=pr)
@@ -458,12 +459,13 @@ class GATEngine:
             h = out
         return h
 
-    def train_step(self, x: torch.Tensor, T: CSR, Tt: CSR, t_perm: torch.Tensor, labels: CSR):
+    def train_step(self, x: torch.Tensor, T: CSR, Tt: CSR, t_perm: torch.Tensor, labels: CSR, labels_t: Optional[CSR] = None):
         """One epoch of graph_AE_handler with use_GAT=True (scgnn2.py:575-593): forward (train mode), loss_function
-        (plain mean BCE on z zᵀ, scgnn2.py:618-619), backward, Adam.  Returns the embedding of this (dropped-out) forward."""
+        (plain mean BCE on z zᵀ, scgnn2.py:618-619), backward, Adam.  Soft labels (``labels.vals`` set, graph_AE_retain_weights)
+        come with ``labels_t``, Lᵀ.  Returns the embedding of this (dropped-out) forward."""
         P, G, pr, nh = self.params.p, self.params.g, self.precision, self.nh
         z = self.forward(x, T, keep=True, training=True)
-        _, dz, _, _ = ops.gae_loss_grad(z, labels, 1.0, 1.0, use_pos_weight=False, loss=self.loss)
+        _, dz, _, _ = ops.gae_loss_grad(z, labels, 1.0, 1.0, use_pos_weight=False, loss=self.loss, labels_t=labels_t)
         dout = dz
         for l in reversed(range(len(self.layers))):
             L, c = self.layers[l], self._cache[l]

@@ -123,14 +123,15 @@ def feature_AE_handler(X, TRS, args, param, model_state=None):
     return embed_host.numpy(), recon_host.numpy()[:, :nf], checkpoint
 
 
-def build_knn_graph(x_embed: torch.Tensor, neighborhood_factor):
+def build_knn_graph(x_embed: torch.Tensor, neighborhood_factor, retain_weights: bool = False):
     """feature2adj + preprocess_graph on device (scgnn2.py:650-689, 1191-1198).
-    Returns (Â as CSR with the A+I pattern, knn index [N,k] int32, knn fp64 distances)."""
+    Returns (Â as CSR with the A+I pattern, knn index [N,k] int32, knn fp64 distances); with ``retain_weights`` the first item
+    is the weighted, directed graph instead (``ops.WeightedGraph``, cell order)."""
     n = x_embed.shape[0]
     k_tmp = neighborhood_factor if neighborhood_factor > 1 else round(n * neighborhood_factor)
     k = int(k_tmp - 1 if k_tmp == n else k_tmp)
     idx, dist = ops.knn(x_embed, k, include_rank0=False)
-    return ops.knn_graph_build(idx), idx, dist
+    return (ops.knn_graph_weighted_build(idx, dist) if retain_weights else ops.knn_graph_build(idx)), idx, dist
 
 
 def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int = 4096):
@@ -141,8 +142,9 @@ def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int
         raise ValueError(f"dropout probability has to be between 0 and 1, but got {gat_dropout}")
     if args.graph_AE_concat_prev_embed and param["epoch_num"] > 0:
         raise NotImplementedError("graph_AE_concat_prev_embed is not built")
-    if args.graph_AE_retain_weights:
-        raise NotImplementedError("graph_AE_retain_weights permutes node order in the reference (App. B); not built")
+    # graph_AE_retain_weights: the weighted, directed kNN graph W = 1/(d + 1e-16) (scgnn2.py:659-670), built in cell order — the
+    # reference orders its nodes by first appearance in edgeList instead (INTEGRATION.md, behavioural differences)
+    retain = bool(args.graph_AE_retain_weights)
     dev = param["device"]
     pool = param.get("io_pool")
     if isinstance(X_embed, torch.Tensor) and X_embed.is_cuda:
@@ -160,13 +162,13 @@ def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int
     # ``param["graph_cache"]`` (extension): a dict that keeps the kNN graph of a previous call on the SAME embedding — the
     # reference rebuilds it on every call (feature2adj, scgnn2.py:555); bench.py uses it to time the training epochs alone.
     cache = param.get("graph_cache")
-    if cache is not None and cache.get("n") == xe.shape[0] and "A" in cache:
+    if cache is not None and cache.get("n") == xe.shape[0] and cache.get("retain_weights", False) == retain and "A" in cache:
         A, knn_idx, knn_dist = cache["A"], cache["knn_idx"], cache["knn_dist"]
     else:
-        A, knn_idx, knn_dist = build_knn_graph(xe, args.graph_AE_neighborhood_factor)
+        A, knn_idx, knn_dist = build_knn_graph(xe, args.graph_AE_neighborhood_factor, retain)
         if cache is not None:
             cache.clear()
-            cache.update(n=xe.shape[0], A=A, knn_idx=knn_idx, knn_dist=knn_dist)
+            cache.update(n=xe.shape[0], retain_weights=retain, A=A, knn_idx=knn_idx, knn_dist=knn_dist)
     n = xe.shape[0]
     # ``param["cell_order"] = "locality"`` (extension): the epochs run on a relabelled copy of the graph in which cells are grouped
     # by nearest embedding centroid (ops.locality_order) — the aggregate's gathers then stay L2-resident; outputs are un-permuted
@@ -177,15 +179,22 @@ def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int
             perm, inv, A_run = cache["perm"], cache["inv"], cache["A_run"]
         else:
             perm, inv = ops.locality_order(xe, n_anchors=int(param.get("cell_order_anchors", 64)))
-            A_run = ops.knn_graph_build(inv[knn_idx[perm].long()].to(torch.int32).contiguous())
+            idx_run = inv[knn_idx[perm].long()].to(torch.int32).contiguous()
+            # the kNN lists are relabelled with their distances, so the weighted graph is the same graph relabelled
+            A_run = ops.knn_graph_weighted_build(idx_run, knn_dist[perm].contiguous()) if retain else ops.knn_graph_build(idx_run)
             if cache is not None:
                 cache.update(perm=perm, inv=inv, A_run=A_run)
-    adj_sum = A.nnz - n                                                         # Σ adj_train (no diagonal)
+    if retain:
+        adj_sum = float(A.sum_w.item())                                         # ΣW = adj_train.sum(), fp64
+        adj_fwd, adj_bwd, labels, labels_t = A_run.adj, A_run.adj_t, A_run.labels, A_run.labels_t
+    else:
+        adj_sum = A.nnz - n                                                     # Σ adj_train (no diagonal)
+        labels = ops.CSR(A_run.rowptr, A_run.colidx, None, A_run.shape)         # A + I: pattern of Â, unit entries
+        adj_fwd, adj_bwd, labels_t = A_run, None, None
     pos_weight = float(n * n - adj_sum) / adj_sum                               # scgnn2.py:567
     norm = n * n / float((n * n - adj_sum) * 2)                                 # scgnn2.py:568-569
-    labels = ops.CSR(A_run.rowptr, A_run.colidx, None, A_run.shape)             # A + I: pattern of Â, unit entries
     xin = xin.contiguous() if perm is None else xin[perm].contiguous()
-    out_kw = dict(pool=pool, cache=cache, keep_dev=bool(param.get("keep_on_device")))
+    out_kw = dict(pool=pool, cache=cache, keep_dev=bool(param.get("keep_on_device")), retain=retain)
     if args.graph_AE_use_GAT:
         # edge_index = edgeList (i → its k neighbours), directed, no self loops (scgnn2.py:560-563); the kernels
         # index the graph by TARGET node, i.e. the transpose of the regular kNN-list CSR
@@ -198,7 +207,7 @@ def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int
                          lr=args.graph_AE_learning_rate, precision=param.get("precision"), seed=param.get("seed"), dropout=gat_dropout)
         z = None
         for epoch in range(args.graph_AE_epoch):
-            z = geng.train_step(xin, T, Tt, t_perm, labels)                         # loss_function: plain BCE (scgnn2.py:581)
+            z = geng.train_step(xin, T, Tt, t_perm, labels, labels_t)               # loss_function: plain BCE (scgnn2.py:581)
             if logger.isEnabledFor(logging.INFO):
                 logger.info(f"Epoch: {epoch+1}/{args.graph_AE_epoch}, Current loss: {geng.loss.item():.4f}")
         param["_graph_AE_engine"] = geng
@@ -211,7 +220,8 @@ def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int
     z = None
     for epoch in range(args.graph_AE_epoch):
         eps.normal_(generator=gen)                                              # torch.randn_like(std), scgnn2.py:397
-        z, _, _ = eng.train_step(xin, A_run, labels, norm, pos_weight, eps if perm is None else eps[perm].contiguous())
+        z, _, _ = eng.train_step(xin, adj_fwd, labels, norm, pos_weight, eps if perm is None else eps[perm].contiguous(), adj_t=adj_bwd,
+                                 labels_t=labels_t)
         if logger.isEnabledFor(logging.INFO):
             logger.info(f"Epoch: {epoch+1}/{args.graph_AE_epoch}, Current loss: {eng.loss.item():.4f}")
     param["_graph_AE_engine"] = eng
@@ -220,10 +230,32 @@ def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int
     return _graph_ae_outputs(z, n, knn_idx, knn_dist, A, dense_recon_max_cells, **out_kw)
 
 
-def _graph_ae_outputs(z, n, knn_idx, knn_dist, A, dense_recon_max_cells, pool=None, cache=None, keep_dev=False):
+def _weighted_adj(knn_idx, knn_dist, on_device: bool):
+    """``adj`` of feature2adj(retain_weights=True) (scgnn2.py:662-664, 670) in cell order: W[i, j] = 1/(d_ij + 1e-16) in fp64 with
+    any diagonal — a scipy CSR, or (``on_device``) a torch sparse CSR tensor on the device."""
+    n, k = knn_idx.shape
+    w = 1.0 / (knn_dist.reshape(-1).double() + 1e-16)
+    cols = knn_idx.reshape(-1).long()
+    order = torch.argsort(torch.arange(n, device=cols.device).repeat_interleave(k) * n + cols)   # sorted columns within each row
+    rowptr = torch.arange(0, n * k + 1, k, dtype=torch.int64, device=cols.device)
+    if on_device:
+        return torch.sparse_csr_tensor(rowptr, cols[order], w[order], (n, n))
+    import scipy.sparse as sp
+    return sp.csr_matrix((w[order].cpu().numpy(), cols[order].cpu().numpy(), rowptr.cpu().numpy()), shape=(n, n))
+
+
+def _graph_ae_outputs(z, n, knn_idx, knn_dist, A, dense_recon_max_cells, pool=None, cache=None, keep_dev=False, retain=False):
     """(graph_embed, recon_graph | None, edgeList, adj) like scgnn2.py:597-600.  ``edgeList`` is ([N·k, 2] int64 pairs, fp64
-    weights 1/(d+1e-16)) instead of a Python list of tuples; ``adj`` the 0/1 union-symmetrised adjacency without diagonal."""
+    weights 1/(d+1e-16)) instead of a Python list of tuples; ``adj`` the 0/1 union-symmetrised adjacency without diagonal, or with
+    ``retain`` the weighted, directed W (fp64, diagonal kept)."""
     if keep_dev:
+        if retain:
+            if cache is not None and "adj_dev" in cache:
+                return z, None, (knn_idx, knn_dist), cache["adj_dev"]
+            adj = _weighted_adj(knn_idx, knn_dist, on_device=True)
+            if cache is not None:
+                cache["adj_dev"] = adj
+            return z, None, (knn_idx, knn_dist), adj
         return z, None, (knn_idx, knn_dist), A
     embed_host = hostio.pinned_empty(pool, "graph_embed", tuple(z.shape))
     embed_host.copy_(z, non_blocking=True)
@@ -237,6 +269,12 @@ def _graph_ae_outputs(z, n, knn_idx, knn_dist, A, dense_recon_max_cells, pool=No
         edge_w = (1.0 / (knn_dist.reshape(-1).double() + 1e-16)).cpu().numpy()  # scgnn2.py:686
         edge_list = (edge_index, edge_w)
         import scipy.sparse as sp
+        if retain:
+            adj = _weighted_adj(knn_idx, knn_dist, on_device=False)
+            if cache is not None:
+                cache["edge_list"], cache["adj"] = edge_list, adj
+            torch.cuda.current_stream(z.device).synchronize()
+            return embed_host.numpy(), recon, edge_list, adj
         rp = A.rowptr.long()
         rows = torch.repeat_interleave(torch.arange(n, device=z.device), rp[1:] - rp[:-1])
         off = A.colidx.long() != rows                                           # drop the diagonal of A + I on the device
@@ -368,8 +406,25 @@ def graph_celltype_regu_handler(adj, cluster_labels, device=None):
     """scgnn2.py:716-724 without the two dense N×N matrices: returns what the Cluster-AE loss takes from them, per cell —
     (w_graph [N], w_celltype [N]) = their column sums inside the cell's cluster.  The reference's "normalised" adjacency is
     deg_j / deg_i (it multiplies np.matrix objects, see csrc/em.cu), so w_graph_j = deg_j · Σ_{i∈cluster(j)} 1/deg_i; the
-    same-cluster indicator is a true ndarray, row-normalised elementwise, whose column sums inside the cluster are 1."""
+    same-cluster indicator is a true ndarray, row-normalised elementwise, whose column sums inside the cluster are 1.
+    A weighted ``adj`` (graph_AE_retain_weights: W as scipy CSR, or a device ``torch.sparse_csr`` tensor) gives
+    w_graph_j = colsum_j · Σ_{i∈cluster(j)} 1/rowsum_i (``ops.graph_regu_weights_weighted``); a 0/1 scipy ``adj`` keeps the path
+    above."""
     lab = torch.as_tensor(np.asarray(cluster_labels), dtype=torch.int32)
+    if isinstance(adj, torch.Tensor) and adj.layout == torch.sparse_csr:        # weighted W on the device (retain_weights)
+        lab = lab.to(adj.device)
+        w_graph = ops.graph_regu_weights_weighted(adj.crow_indices().to(torch.int32), adj.col_indices().to(torch.int32),
+                                                  adj.values().double().contiguous(), lab)
+        return w_graph, torch.ones_like(w_graph)
+    if not isinstance(adj, ops.CSR) and not np.all(adj.data == 1):              # weighted scipy adjacency (retain_weights): W
+        m = adj.tocsr()
+        m.sort_indices()
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        lab = lab.to(dev)
+        w_graph = ops.graph_regu_weights_weighted(torch.from_numpy(m.indptr.astype(np.int32)).to(dev),
+                                                  torch.from_numpy(m.indices.astype(np.int32)).to(dev),
+                                                  torch.from_numpy(m.data.astype(np.float64)).to(dev), lab)
+        return w_graph, torch.ones_like(w_graph)
     if isinstance(adj, ops.CSR):
         A = adj
     else:                                                                       # scipy 0/1 adjacency without diagonal

@@ -7,7 +7,7 @@ falls back to torch kernels: a missing library or a non-CUDA tensor raises.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Tuple
+from typing import NamedTuple, Optional, Tuple
 
 import torch
 
@@ -320,13 +320,18 @@ def mse_sum_loss_grad(recon, target, ltmg_regu=None, regu_strength=0.0, relu_mas
     return loss_out, grad
 
 
-def _gae_prepare(what, z, labels: CSR, n_rows, mu, logvar, dmu, dlogvar, loss):
+def _gae_prepare(what, z, labels: CSR, n_rows, mu, logvar, dmu, dlogvar, loss, labels_t: Optional[CSR] = None):
     """Checks and buffers both decoder calls share; returns (n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, workspace)."""
     _chk(z, torch.float32, "z", 2)
     n, d = z.shape
     n_rows = n if n_rows is None else n_rows
     if labels.shape[0] != n_rows or labels.shape[1] != n:
         raise B2Error(f"{what}: labels must be [{n_rows}, {n}] (rows of this shard x all columns), got {tuple(labels.shape)}")
+    if labels.vals is not None:
+        if labels_t is None or labels_t.vals is None:
+            raise B2Error(f"{what}: real-valued labels need labels_t= (the same rows of Lᵀ, with values)")
+        if tuple(labels_t.shape) != tuple(labels.shape):
+            raise B2Error(f"{what}: labels_t must be [{n_rows}, {n}] like labels, got {tuple(labels_t.shape)}")
     ldm = ldd = 0
     if mu is not None:
         _chk(mu, torch.float32, "mu", 2)
@@ -345,23 +350,34 @@ def _gae_prepare(what, z, labels: CSR, n_rows, mu, logvar, dmu, dlogvar, loss):
     return n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, _workspace(lib().b2_gae_loss_workspace_bytes(n, d), z.device)
 
 
+def _label_args(labels: CSR, labels_t: Optional[CSR]):
+    """The label arguments of the decoder entry points: (rowptr, colidx) for unit labels, plus values and Lᵀ for real ones."""
+    if labels.vals is None:
+        return [_p(labels.rowptr), _p(labels.colidx)]
+    return [_p(labels.rowptr), _p(labels.colidx), _p(labels.vals), _p(labels_t.rowptr), _p(labels_t.colidx), _p(labels_t.vals)]
+
+
 def gae_loss_grad(z, labels: CSR, norm: float, pos_weight: float, mu=None, logvar=None, use_pos_weight=True,
-                  dz=None, dmu=None, dlogvar=None, loss=None, row_begin: int = 0, n_rows: Optional[int] = None):
+                  dz=None, dmu=None, dlogvar=None, loss=None, row_begin: int = 0, n_rows: Optional[int] = None,
+                  labels_t: Optional[CSR] = None):
     """Matrix-free Graph-AE loss: returns (loss[1], dz, dmu, dlogvar).
 
     ``dmu``/``dlogvar`` may be column slices of one packed [n, 2d] buffer (shared leading dimension).
+    ``labels.vals`` None: unit, symmetric labels.  Otherwise real-valued, possibly asymmetric labels (graph_AE_retain_weights), and
+    ``labels_t`` holds the same rows of Lᵀ with their values.
     """
-    n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, ws = _gae_prepare("gae_loss_grad", z, labels, n_rows, mu, logvar, dmu, dlogvar, loss)
+    n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, ws = _gae_prepare("gae_loss_grad", z, labels, n_rows, mu, logvar, dmu, dlogvar, loss,
+                                                                  labels_t)
     if dz is None:
         dz = torch.empty((n_rows, d), dtype=torch.float32, device=z.device)
     else:
         _chk(dz, torch.float32, "dz", 2)
         if tuple(dz.shape) != (n_rows, d) or not dz.is_contiguous():
             raise B2Error(f"gae_loss_grad: dz must be a contiguous [{n_rows}, {d}] buffer, got {tuple(dz.shape)} strides {dz.stride()}")
-    check(lib().b2_gae_loss_grad_f32(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, _p(labels.rowptr), _p(labels.colidx), n, d,
-                                     row_begin, n_rows, float(norm), float(pos_weight), int(use_pos_weight),
-                                     _p(dz), _p(dmu), _p(dlogvar), ldd, _p(loss), _p(ws), ws.numel(), _stream()),
-          "b2_gae_loss_grad_f32")
+    fn = "b2_gae_loss_grad_f32" if labels.vals is None else "b2_gae_loss_grad_weighted_f32"
+    check(getattr(lib(), fn)(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, *_label_args(labels, labels_t), n, d,
+                             row_begin, n_rows, float(norm), float(pos_weight), int(use_pos_weight),
+                             _p(dz), _p(dmu), _p(dlogvar), ldd, _p(loss), _p(ws), ws.numel(), _stream()), fn)
     return loss, dz, dmu, dlogvar
 
 
@@ -372,21 +388,22 @@ def gae_sym_super_blocks(n: int) -> int:
 
 def gae_loss_grad_sym(z, labels: CSR, norm: float, pos_weight: float, sb_begin: int, sb_end: int, mu=None, logvar=None,
                       use_pos_weight=True, dz_full=None, dmu=None, dlogvar=None, loss=None, row_begin: int = 0,
-                      n_rows: Optional[int] = None):
+                      n_rows: Optional[int] = None, labels_t: Optional[CSR] = None):
     """Pair-sharded matrix-free Graph-AE loss (multi-GPU form of :func:`gae_loss_grad`): this rank evaluates super-blocks
     ``[sb_begin, sb_end)`` of the unordered block-pair schedule and the label / KLD terms of its rows.  Returns
-    ``(loss_share[1], dz_full[n, d], dmu, dlogvar)``; all-reduce ``dz_full`` and ``loss_share`` over ranks."""
+    ``(loss_share[1], dz_full[n, d], dmu, dlogvar)``; all-reduce ``dz_full`` and ``loss_share`` over ranks.  Real-valued labels
+    (``labels.vals`` set) need ``labels_t`` as in :func:`gae_loss_grad`."""
     n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, ws = _gae_prepare("gae_loss_grad_sym", z, labels, n_rows, mu, logvar, dmu, dlogvar,
-                                                                  loss)
+                                                                  loss, labels_t)
     if dz_full is None:
         dz_full = torch.empty((n, d), dtype=torch.float32, device=z.device)
     _chk(dz_full, torch.float32, "dz_full", 2)
     if tuple(dz_full.shape) != (n, d) or not dz_full.is_contiguous():
         raise B2Error(f"gae_loss_grad_sym: dz_full must be a contiguous [{n}, {d}] buffer")
-    check(lib().b2_gae_loss_grad_sym_f32(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, _p(labels.rowptr), _p(labels.colidx), n, d,
-                                         sb_begin, sb_end, row_begin, n_rows, float(norm), float(pos_weight), int(use_pos_weight),
-                                         _p(dz_full), _p(dmu), _p(dlogvar), ldd, _p(loss), _p(ws), ws.numel(), _stream()),
-          "b2_gae_loss_grad_sym_f32")
+    fn = "b2_gae_loss_grad_sym_f32" if labels.vals is None else "b2_gae_loss_grad_sym_weighted_f32"
+    check(getattr(lib(), fn)(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, *_label_args(labels, labels_t), n, d,
+                             sb_begin, sb_end, row_begin, n_rows, float(norm), float(pos_weight), int(use_pos_weight),
+                             _p(dz_full), _p(dmu), _p(dlogvar), ldd, _p(loss), _p(ws), ws.numel(), _stream()), fn)
     return loss, dz_full, dmu, dlogvar
 
 
@@ -469,6 +486,43 @@ def knn_graph_build(knn_idx: torch.Tensor) -> CSR:
                                    ws.numel(), _stream()), "b2_knn_graph_build")
     m = nnz.value
     return CSR(rowptr, colidx[:m].clone(), vals[:m].clone(), (n, n))
+
+
+class WeightedGraph(NamedTuple):
+    """The weighted, directed kNN graph of ``graph_AE_retain_weights`` (see :func:`knn_graph_weighted_build`).  ``adj`` and
+    ``labels_t`` share the target-row index arrays, ``adj_t`` and ``labels`` the source-row ones."""
+    adj: CSR          # Â, rows = target: the forward aggregate
+    adj_t: CSR        # Âᵀ, rows = source: the backward aggregate
+    labels: CSR       # L = adj_train + I with its fp32 values, rows = source
+    labels_t: CSR     # Lᵀ with its values, rows = target
+    sum_w: torch.Tensor   # ΣW = adj_train.sum(), device fp64 [1]
+
+
+def knn_graph_weighted_build(knn_idx: torch.Tensor, knn_dist: torch.Tensor) -> WeightedGraph:
+    """feature2adj(retain_weights=True) + preprocess_graph (scgnn2.py:659-670, 1191-1198) from the kNN lists: W = 1/(d + 1e-16),
+    directed, in cell order; Â = ((adj_train + I)·Dm)ᵀ·Dm with Dm = diag(rowsum^-1/2), evaluated in fp64, stored in fp32."""
+    _chk(knn_idx, torch.int32, "knn_idx", 2)
+    _chk(knn_dist, torch.float64, "knn_dist", 2)
+    if not (knn_idx.is_contiguous() and knn_dist.is_contiguous()) or knn_idx.shape != knn_dist.shape:
+        raise B2Error("knn_graph_weighted_build: knn_idx and knn_dist must be contiguous and of one shape")
+    n, k = knn_idx.shape
+    cap = n * (k + 1)
+    dev = knn_idx.device
+    i32 = lambda m: torch.empty(m, dtype=torch.int32, device=dev)
+    f32 = lambda m: torch.empty(m, dtype=torch.float32, device=dev)
+    rowptr, colidx, y, norm_t = i32(n + 1), i32(cap), f32(cap), f32(cap)
+    t_rowptr, t_colidx, t_y, norm = i32(n + 1), i32(cap), f32(cap), f32(cap)
+    sum_w = torch.empty(1, dtype=torch.float64, device=dev)
+    nnz = C.c_int64(0)
+    ws = _workspace(lib().b2_knn_graph_weighted_workspace_bytes(n, k), dev)
+    check(lib().b2_knn_graph_weighted_build(_p(knn_idx), _p(knn_dist), n, k, _p(rowptr), _p(colidx), _p(y), _p(norm_t), _p(t_rowptr),
+                                            _p(t_colidx), _p(t_y), _p(norm), _p(sum_w), cap, C.byref(nnz), _p(ws), ws.numel(),
+                                            _stream()), "b2_knn_graph_weighted_build")
+    m = nnz.value
+    if m < cap:
+        colidx, y, norm_t, t_colidx, t_y, norm = (t[:m].clone() for t in (colidx, y, norm_t, t_colidx, t_y, norm))
+    return WeightedGraph(CSR(t_rowptr, t_colidx, norm, (n, n)), CSR(rowptr, colidx, norm_t, (n, n)), CSR(rowptr, colidx, y, (n, n)),
+                         CSR(t_rowptr, t_colidx, t_y, (n, n)), sum_w)
 
 
 def normalize_total_log1p_(X: torch.Tensor, target_sum: Optional[float] = None, max_fraction: float = 1.0,
@@ -1019,6 +1073,27 @@ def graph_regu_weights(A: CSR, labels: torch.Tensor, n_clusters: Optional[int] =
     sums = torch.empty(max(n_clusters, 1), dtype=torch.float64, device=labels.device)
     check(lib().b2_graph_regu_weights_f32(_p(A.rowptr), _p(A.colidx), _p(labels), n, int(n_clusters), _p(sums), _p(w), _stream()),
           "b2_graph_regu_weights_f32")
+    return w
+
+
+def graph_regu_weights_weighted(rowptr: torch.Tensor, colidx: torch.Tensor, vals: torch.Tensor, labels: torch.Tensor,
+                                n_clusters: Optional[int] = None) -> torch.Tensor:
+    """:func:`graph_regu_weights` for a weighted, directed adjacency (CSR with fp64 ``vals``, the ``adj`` of
+    graph_AE_retain_weights): w_j = colsum_j · Σ_{i ∈ cluster(j)} 1/rowsum_i (see b2_graph_regu_weights_weighted_f32)."""
+    _chk(labels, torch.int32, "labels", 1)
+    _chk(rowptr, torch.int32, "rowptr", 1)
+    _chk(colidx, torch.int32, "colidx", 1)
+    _chk(vals, torch.float64, "vals", 1)
+    n = rowptr.numel() - 1
+    if labels.numel() != n or vals.numel() != colidx.numel():
+        raise B2Error(f"graph_regu_weights_weighted: {n} rows but {labels.numel()} labels, or values and columns differ in length")
+    if n_clusters is None:
+        n_clusters = int(labels.max().item()) + 1 if n else 1
+    w = torch.empty(n, dtype=torch.float32, device=labels.device)
+    scratch = torch.empty(n + max(n_clusters, 1), dtype=torch.float64, device=labels.device)
+    check(lib().b2_graph_regu_weights_weighted_f32(_p(rowptr), _p(colidx) if colidx.numel() else _p(rowptr),
+                                                   _p(vals) if vals.numel() else _p(scratch), _p(labels), n, int(n_clusters),
+                                                   _p(scratch), _p(w), _stream()), "b2_graph_regu_weights_weighted_f32")
     return w
 
 

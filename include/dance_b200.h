@@ -180,6 +180,18 @@ int b2_gae_loss_grad_f32(const float* z, int64_t ldz, const float* mu, const flo
                          float norm, float pos_weight, int use_pos_weight,
                          float* dz, float* dmu, float* dlogvar, int64_t ldd, float* loss_out,
                          void* workspace, size_t workspace_bytes, void* stream);
+/* b2_gae_loss_grad_f32 with real-valued, asymmetric labels y (graph_AE_retain_weights, scgnn2.py:555-569):
+ *   lab_*  : the local rows of L (entries (i, j), values y_ij, diagonal included);
+ *   labt_* : the local rows of Lᵀ (row i holds the j with (j, i) in L, values y_ji), n_rows+1 row pointers, global column ids.
+ * Per entry ℓ = (1−y)·softplus(x) + y²·pw·softplus(−x) (pos_weight = labels·pw); use_pos_weight = 0: ℓ = softplus(x) − y·x.
+ * Unit symmetric labels give b2_gae_loss_grad_f32.  The all-pairs part, the KLD and the workspace are those of that call. */
+int b2_gae_loss_grad_weighted_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
+                                  const int32_t* lab_rowptr, const int32_t* lab_colidx, const float* lab_vals,
+                                  const int32_t* labt_rowptr, const int32_t* labt_colidx, const float* labt_vals,
+                                  int32_t n, int32_t d, int32_t row_begin, int32_t n_rows,
+                                  float norm, float pos_weight, int use_pos_weight,
+                                  float* dz, float* dmu, float* dlogvar, int64_t ldd, float* loss_out,
+                                  void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * Optimiser: torch.optim.Adam semantics (scgnn2.py:301,573; default eps 1e-8,
@@ -245,6 +257,23 @@ int b2_knn_graph_build(const int32_t* knn_idx, int32_t n, int32_t k,
                        int32_t* rowptr /* n+1 */, int32_t* colidx /* cap */, float* vals_norm /* cap */,
                        int64_t capacity, int64_t* nnz_out_host,
                        void* workspace, size_t workspace_bytes, void* stream);
+
+/* Weighted, directed kNN graph: feature2adj(retain_weights=True) (scgnn2.py:659-670) + preprocess_graph (scgnn2.py:1191-1198).
+ *   knn_idx [n,k] int32 (distinct neighbours per row), knn_dist [n,k] fp64 → W[i,j] = 1/(d_ij + 1e-16) in fp64, directed, no
+ *   clamping (a zero distance gives 1e16).  adj_train = W without its diagonal (a row listing itself drops that slot).
+ *   L = adj_train + I with sorted columns, in two orientations of nnz entries each (capacity >= n·(k+1)):
+ *     rowptr/colidx  : rows = source i;  y = float32(L[i,j]) (the decoder labels),  norm_t = Âᵀ[i,j]
+ *     t_rowptr/...   : rows = target j;  t_y = float32(L[i,j]) at (j, i),            norm   = Â[j,i]
+ *   Â[i,j] = adj_[j,i]·r_i^-1/2·r_j^-1/2 with adj_ = adj_train + I and r = rowsum(adj_) (the out-weight + 1), the products in
+ *   fp64 in the reference's order ((adj_·Dm)ᵀ·Dm), cast to fp32.  (Lᵀ rows, norm) is the CSR of Â for the forward aggregate,
+ *   (L rows, norm_t) the CSR of Âᵀ for the backward.  sum_w: one device double, ΣW = adj_train.sum().  Synchronises the stream;
+ *   *nnz_out_host = nnz. */
+size_t b2_knn_graph_weighted_workspace_bytes(int32_t n, int32_t k);
+int b2_knn_graph_weighted_build(const int32_t* knn_idx, const double* knn_dist, int32_t n, int32_t k,
+                                int32_t* rowptr /* n+1 */, int32_t* colidx, float* y, float* norm_t,
+                                int32_t* t_rowptr /* n+1 */, int32_t* t_colidx, float* t_y, float* norm,
+                                double* sum_w, int64_t capacity, int64_t* nnz_out_host,
+                                void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * K9  normalize_total (+ optional log1p), in place on dense X [n,g]
@@ -526,6 +555,13 @@ int b2_gae_loss_grad_sym_f32(const float* z, int64_t ldz, const float* mu, const
                              int32_t sb_begin, int32_t sb_end, int32_t row_begin, int32_t n_rows, float norm, float pos_weight,
                              int use_pos_weight, float* dz_full, float* dmu, float* dlogvar, int64_t ldd, float* loss_out,
                              void* workspace, size_t workspace_bytes, void* stream);
+/* Pair-sharded form with real-valued, asymmetric labels (see b2_gae_loss_grad_weighted_f32). */
+int b2_gae_loss_grad_sym_weighted_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
+                                      const int32_t* lab_rowptr, const int32_t* lab_colidx, const float* lab_vals,
+                                      const int32_t* labt_rowptr, const int32_t* labt_colidx, const float* labt_vals,
+                                      int32_t n, int32_t d, int32_t sb_begin, int32_t sb_end, int32_t row_begin, int32_t n_rows,
+                                      float norm, float pos_weight, int use_pos_weight, float* dz_full, float* dmu, float* dlogvar,
+                                      int64_t ldd, float* loss_out, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * scGNN EM-iteration stages (SURVEY §8f row 3)
@@ -537,6 +573,9 @@ int b2_gae_loss_grad_sym_f32(const float* z, int64_t ldz, const float* mu, const
  *       `avg_mtx * x` is a MATRIX product and adjdense[i, j] = deg_j / deg_i (dense, rank one); the column sums inside j's cluster are
  *       w_j = deg_j * sum_{i in cluster(j)} 1/deg_i.  Pattern = A or A + I CSR (the diagonal is not counted); cluster_sums: n_clusters
  *       device doubles of scratch.
+ *   b2_graph_regu_weights_weighted_f32 : the same for a weighted, directed adj (graph_AE_retain_weights returns W): adjdense[i, j]
+ *       = colsum_j / rowsum_i, so w_j = colsum_j * sum_{i in cluster(j)} 1/rowsum_i; a row with zero sum adds 0.  vals: fp64 CSR
+ *       values; the diagonal is not counted.  scratch: n + n_clusters device doubles.
  *   b2_celltype_loss_grad_f32 : loss_function_graph(regularizer_type="Celltype"), scgnn2.py:1316-1326, with the dense
  *       `M @ mse` products folded into per-row weights: value = sum_j row_weight_j * sum_g (r-x)^2 + || (x_dropout - r)[x_dropout != 0] ||_2
  *       (callers pass row_weight = 0.3 + 0.3*w_graph + 0.1*w_celltype); grad = d value / d recon masked by recon > 0.
@@ -551,6 +590,8 @@ int b2_kmeans_step_f32(const float* X, int64_t ldx, int32_t n, int32_t d, float*
                        double* stats, void* workspace, size_t workspace_bytes, void* stream);
 int b2_graph_regu_weights_f32(const int32_t* rowptr, const int32_t* colidx, const int32_t* labels, int32_t n, int32_t n_clusters,
                               double* cluster_sums, float* w, void* stream);
+int b2_graph_regu_weights_weighted_f32(const int32_t* rowptr, const int32_t* colidx, const double* vals, const int32_t* labels, int32_t n,
+                                       int32_t n_clusters, double* scratch, float* w, void* stream);
 int b2_celltype_loss_grad_f32(const float* recon, const float* target, const float* x_dropout, const float* row_weight,
                               int64_t rows, int32_t cols, int32_t cols_orig, int relu_mask, float* grad, float* loss_out,
                               double* scratch2, void* stream);

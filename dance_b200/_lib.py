@@ -44,6 +44,13 @@ _SIGNATURES = {
     "b2_kmeans_step_f32": (C.c_int, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i32, c_vp, C.c_int, c_vp, c_vp, c_sz, c_vp]),
     "b2_graph_regu_weights_f32": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "b2_graph_regu_weights_weighted_f32": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp, c_vp]),
+    "b2_quantiles_workspace_bytes": (c_sz, []),
+    "b2_quantiles_f32": (C.c_int, [c_vp, c_i64, c_i64, c_i32, c_vp, c_i32, c_vp, c_vp, c_sz, c_vp]),
+    "b2_col_minmax_workspace_bytes": (c_sz, [c_i32]),
+    "b2_col_minmax_f32": (C.c_int, [c_vp, c_i64, c_i64, c_i32, c_vp, c_vp, c_vp, c_vp, c_sz, c_vp]),
+    "b2_concat_scaled_workspace_bytes": (c_sz, [c_i32]),
+    "b2_concat_scaled_f32": (C.c_int, [c_vp, c_i64, c_i32, c_vp, c_i64, c_i32, c_i64, c_vp, c_vp, c_f32, c_f32, C.c_int, c_vp, c_i64,
+                                       c_vp, c_sz, c_vp]),
     "b2_celltype_loss_grad_f32": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, C.c_int, c_vp, c_vp, c_vp, c_vp]),
     "b2_l1_grad_add_f32": (C.c_int, [c_vp, c_vp, c_i64, c_f32, c_vp, c_vp]),
     "b2_louvain_csr_host": (C.c_int, [c_vp, c_vp, c_vp, c_i32, c_vp, C.POINTER(c_i32), C.POINTER(C.c_double), C.c_int, C.c_double]),

@@ -54,21 +54,32 @@ def feature_AE_handler(X, TRS, args, param, model_state=None):
     batch_size = args.feature_AE_batch_size
     total_epoch = args.feature_AE_epoch[param["epoch_num"] > 0]
     p_drop = float(args.feature_AE_dropout_prob or 0.0)        # train_handler's masked_prob: F.dropout on the network input (scgnn2.py:1256)
-    if getattr(args, "feature_AE_concat_prev_embed", None) and param["epoch_num"] > 0:
-        raise NotImplementedError("feature_AE_concat_prev_embed is not built")
+    concat = getattr(args, "feature_AE_concat_prev_embed", None) if param["epoch_num"] > 0 else None
+    if concat and concat not in ("graph", "feature"):
+        # the reference logs and sets prev_embed = None, and np.concatenate then fails (scgnn2.py:291-293)
+        raise ValueError(f"feature_AE_concat_prev_embed must be 'graph' or 'feature', got {concat!r}")
     pool = param.get("io_pool")
     resident = isinstance(X, torch.Tensor) and X.is_cuda
     if resident:                                   # already in HBM (EM iterations hand device tensors from stage to stage)
         Xd, host = X.float().contiguous(), None
+    elif concat:                                   # the quantiles need all of X in HBM: no row streaming in the first epoch
+        Xd, host = hostio.as_host_tensor(X).to(dev), None
     else:
         host = hostio.as_host_tensor(X)
         Xd = torch.empty(host.shape, dtype=torch.float32, device=dev)
+    if concat:
+        # X ← [X | normalizer(graph_embed, base=X)] or [X | feature_embed] (scgnn2.py:286-294), in a row-padded buffer
+        prev = _on_device(param["graph_embed" if concat == "graph" else "feature_embed"], dev)
+        Xd = ops.concat_normalized(Xd, prev, base=Xd if concat == "graph" else None)
     n, dim = Xd.shape
     ltmg = None
     if TRS is not None and np.any(TRS):
         ltmg = torch.as_tensor(TRS, dtype=torch.float32).to(dev)
     eng = FeatureAEEngine(dim, device=dev, lr=args.feature_AE_learning_rate, precision=param.get("precision"), seed=param.get("seed"))
-    if param["epoch_num"] > 0 and model_state is not None:
+    if concat:
+        if param["epoch_num"] > 1:                 # epoch 1 starts the widened model from a fresh initialisation
+            eng.load_state_dict(model_state["model_concat"])
+    elif param["epoch_num"] > 0 and model_state is not None:
         eng.load_state_dict(model_state["model"])
     # regu_type=["LTMG", "noregu"][epoch_num > 0]   (scgnn2.py:314)
     regu = "noregu" if param["epoch_num"] > 0 else "LTMG"
@@ -99,8 +110,11 @@ def feature_AE_handler(X, TRS, args, param, model_state=None):
             if slot_busy[slot] is not None:               # the download of batch b-2's reconstruction has left this buffer set
                 main.wait_event(slot_busy[slot])
                 slot_busy[slot] = None
-            z, r = eng.train_step(Xd[b0:b1], None if ltmg is None else ltmg[b0:b1], args.feature_AE_regu_strength, regu, slot=slot,
-                                  x_input=eng.input_dropout(Xd[b0:b1], p_drop) if p_drop > 0.0 else None)
+            xb = Xd[b0:b1]
+            if not xb.is_contiguous():                    # the loss kernel takes a dense target: compact a batch of the row-padded
+                xb = xb.contiguous()                      # widened matrix
+            z, r = eng.train_step(xb, None if ltmg is None else ltmg[b0:b1], args.feature_AE_regu_strength, regu, slot=slot,
+                                  x_input=eng.input_dropout(xb, p_drop) if p_drop > 0.0 else None)
             if last:
                 z_all[b0:b1].copy_(z)
                 if keep_dev:
@@ -109,9 +123,13 @@ def feature_AE_handler(X, TRS, args, param, model_state=None):
                     slot_busy[slot] = down.copy(r, recon_host[b0:b1])
         if logger.isEnabledFor(logging.INFO):
             logger.info(f"Epoch: {epoch+1}/{total_epoch}, Average loss: {eng.loss_acc.item() / n:.4f}")
-    checkpoint = {"model": eng.state_dict(),
-                  "optimizer": {"step": eng.params.step, "exp_avg": eng.params.exp_avg.clone(),
-                                "exp_avg_sq": eng.params.exp_avg_sq.clone()}}
+    optimizer = {"step": eng.params.step, "exp_avg": eng.params.exp_avg.clone(), "exp_avg_sq": eng.params.exp_avg_sq.clone()}
+    if concat:
+        # the widened model is kept beside the G-wide pre-EM one, which the Cluster-AE keeps loading (scgnn2.py:323-329)
+        checkpoint = {"model_concat": eng.state_dict(), "optimizer_concat": optimizer, "model": model_state["model"],
+                      "optimizer": model_state["optimizer"]}
+    else:
+        checkpoint = {"model": eng.state_dict(), "optimizer": optimizer}
     param["_feature_AE_engine"] = eng
     nf = param["n_feature_orig"]
     if keep_dev:
@@ -121,6 +139,13 @@ def feature_AE_handler(X, TRS, args, param, model_state=None):
     down.synchronize()
     torch.cuda.current_stream(dev).synchronize()
     return embed_host.numpy(), recon_host.numpy()[:, :nf], checkpoint
+
+
+def _on_device(a, dev) -> torch.Tensor:
+    """An fp32 matrix in HBM: device tensors are used in place, host arrays copied."""
+    if isinstance(a, torch.Tensor) and a.is_cuda:
+        return a if a.dtype == torch.float32 else a.float()
+    return hostio.as_host_tensor(a).to(dev)
 
 
 def build_knn_graph(x_embed: torch.Tensor, neighborhood_factor, retain_weights: bool = False):
@@ -140,8 +165,6 @@ def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int
     gat_dropout = float(getattr(args, "graph_AE_GAT_dropout", 0) or 0)
     if args.graph_AE_use_GAT and not 0.0 <= gat_dropout <= 1.0:          # nn.Dropout's check (Graph_AE → GATLayer, scgnn2.py:375-378)
         raise ValueError(f"dropout probability has to be between 0 and 1, but got {gat_dropout}")
-    if args.graph_AE_concat_prev_embed and param["epoch_num"] > 0:
-        raise NotImplementedError("graph_AE_concat_prev_embed is not built")
     # graph_AE_retain_weights: the weighted, directed kNN graph W = 1/(d + 1e-16) (scgnn2.py:659-670), built in cell order — the
     # reference orders its nodes by first appearance in edgeList instead (INTEGRATION.md, behavioural differences)
     retain = bool(args.graph_AE_retain_weights)
@@ -153,6 +176,10 @@ def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int
         xh = hostio.as_host_tensor(X_embed)
         xe = torch.empty(xh.shape, dtype=torch.float32, device=dev)
         xe.copy_(xh, non_blocking=True)
+    if args.graph_AE_concat_prev_embed and param["epoch_num"] > 0:
+        # X_embed ← [X_embed | normalizer(graph_embed, base=X_embed)] (scgnn2.py:543-546): the kNN graph, normalize_embed and the
+        # model all take the widened matrix
+        xe = ops.concat_normalized(xe, _on_device(param["graph_embed"], dev), base=xe)
     if args.graph_AE_normalize_embed == "sum1":
         xin = xe / xe.sum(1, keepdim=True).clamp(min=1)                         # scgnn2.py:622-628
     elif args.graph_AE_normalize_embed == "binary":
@@ -162,13 +189,15 @@ def graph_AE_handler(X_embed, CCC_graph, args, param, dense_recon_max_cells: int
     # ``param["graph_cache"]`` (extension): a dict that keeps the kNN graph of a previous call on the SAME embedding — the
     # reference rebuilds it on every call (feature2adj, scgnn2.py:555); bench.py uses it to time the training epochs alone.
     cache = param.get("graph_cache")
-    if cache is not None and cache.get("n") == xe.shape[0] and cache.get("retain_weights", False) == retain and "A" in cache:
+    # Its key holds the input width, so a widened (concat_prev_embed) call never reuses the graph of a narrower one.
+    if (cache is not None and cache.get("n") == xe.shape[0] and cache.get("d") == xe.shape[1]
+            and cache.get("retain_weights", False) == retain and "A" in cache):
         A, knn_idx, knn_dist = cache["A"], cache["knn_idx"], cache["knn_dist"]
     else:
         A, knn_idx, knn_dist = build_knn_graph(xe, args.graph_AE_neighborhood_factor, retain)
         if cache is not None:
             cache.clear()
-            cache.update(n=xe.shape[0], retain_weights=retain, A=A, knn_idx=knn_idx, knn_dist=knn_dist)
+            cache.update(n=xe.shape[0], d=xe.shape[1], retain_weights=retain, A=A, knn_idx=knn_idx, knn_dist=knn_dist)
     n = xe.shape[0]
     # ``param["cell_order"] = "locality"`` (extension): the epochs run on a relabelled copy of the graph in which cells are grouped
     # by nearest embedding centroid (ops.locality_order) — the aggregate's gathers then stay L2-resident; outputs are un-permuted
@@ -335,14 +364,6 @@ def cluster_output_handler(listResult):
     return list(listResult), [np.nonzero(lab == c)[0].tolist() for c in range(len(set(lab.tolist())))]
 
 
-def _normalizer(X, base, axis=0):
-    from sklearn.preprocessing import minmax_scale
-    upper, lower = np.quantile(base, q=0.9), np.quantile(base, q=0.1)
-    if upper != lower:
-        return minmax_scale(X, feature_range=(lower, upper), axis=axis)
-    return minmax_scale(X, feature_range=(np.quantile(base, q=0), np.quantile(base, q=1)), axis=axis)
-
-
 def kmeans_fit_predict(embed, k: int, device, seed: int = 0, init_max_cells: int = 200_000):
     """``KMeans(n_clusters=k, n_init="auto", random_state=0).fit_predict(embed)`` (scgnn2.py:186): k-means++ seeding by
     sklearn's own routine on the host (on a fixed-seed subsample above ``init_max_cells`` cells), Lloyd iterations on the device."""
@@ -374,7 +395,11 @@ def clustering_handler(edgeList, args, param):
     if args.clustering_embed == "feature":
         embed = fe
     elif args.clustering_embed == "both":
-        embed = np.concatenate((to_np(ge), _normalizer(to_np(fe), base=to_np(ge), axis=0)), axis=1).astype(np.float32)
+        # [graph_embed | normalizer(feature_embed, base=graph_embed)] (scgnn2.py:155-157) on the device; host arrays come back as one
+        dev = param["device"]
+        embed = ops.concat_normalized(_on_device(ge, dev), _on_device(fe, dev), base=_on_device(ge, dev))
+        if not (isinstance(ge, torch.Tensor) or isinstance(fe, torch.Tensor)):
+            embed = embed.cpu().numpy()
     else:
         if args.clustering_embed != "graph":
             logger.error("clustering_embed argument not recognized, using graph embed")

@@ -1206,3 +1206,101 @@ def locality_order(X: torch.Tensor, n_anchors: int = 64, iters: int = 4, seed: i
     inv = torch.empty_like(perm)
     inv[perm] = torch.arange(n, device=X.device)
     return perm, inv
+
+
+# ---- scGNN's normalizer(X, base) and the concatenations that use it (scgnn2.py:155-157, 283-294, 543-546, 795-805) ------------
+def _quantiles_launch(base: torch.Tensor, qs, out: torch.Tensor) -> None:
+    """Enqueue b2_quantiles_f32 for one or two q: ``out`` (device doubles) receives the quantiles, min, max, #non-finite."""
+    _chk(base, torch.float32, "base", 2)
+    rows, cols = base.shape
+    if rows == 0 or cols == 0:
+        raise ValueError("quantiles: base is empty")
+    qh = (C.c_float * len(qs))(*[float(q) for q in qs])
+    nbytes = lib().b2_quantiles_workspace_bytes()
+    ws = _workspace(nbytes, base.device)
+    check(lib().b2_quantiles_f32(_p(base), _rowmajor(base, "base"), rows, cols, qh, len(qs), _p(out), _p(ws), ws.numel(), _stream()),
+          "b2_quantiles_f32")
+
+
+def quantiles(base: torch.Tensor, qs) -> "np.ndarray":
+    """``np.quantile(base, q)`` (method "linear") for every q of ``qs`` over ALL elements of the (row-padded) fp32 matrix ``base``,
+    bit for bit, as a float32 numpy array.  A zero comes back as +0.0 whatever its sign in ``base``.  Synchronises once per pair
+    of q; a non-finite element raises ``ValueError`` (numpy would return NaN)."""
+    import numpy as np
+    qs = [float(np.float32(q)) for q in np.atleast_1d(np.asarray(qs, dtype=np.float64))]
+    if not all(0.0 <= q <= 1.0 for q in qs):
+        raise ValueError("Quantiles must be in the range [0, 1]")
+    res = []
+    for j in range(0, len(qs), 2):
+        pair = qs[j:j + 2]
+        out = torch.empty(len(pair) + 3, dtype=torch.float64, device=base.device)
+        _quantiles_launch(base, pair, out)
+        vals = out.tolist()
+        if vals[-1] > 0:
+            raise ValueError(f"quantiles: base holds {int(vals[-1])} non-finite values")
+        res.extend(vals[:len(pair)])
+    return np.asarray(res, dtype=np.float32)
+
+
+def col_minmax(x: torch.Tensor, nonfinite: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Per-column (min, max) of a 2-D fp32 matrix ignoring NaN (np.nanmin / np.nanmax); ``nonfinite``: an optional device double
+    that receives the number of non-finite elements."""
+    _chk(x, torch.float32, "x", 2)
+    rows, cols = x.shape
+    cmin = torch.empty(cols, dtype=torch.float32, device=x.device)
+    cmax = torch.empty(cols, dtype=torch.float32, device=x.device)
+    ws = _workspace(lib().b2_col_minmax_workspace_bytes(cols), x.device)
+    check(lib().b2_col_minmax_f32(_p(x), _rowmajor(x, "x"), rows, cols, _p(cmin), _p(cmax), _p(nonfinite), _p(ws), ws.numel(),
+                                  _stream()), "b2_col_minmax_f32")
+    return cmin, cmax
+
+
+def _feature_range(base: torch.Tensor, upper: float, lower: float, bmin: float, bmax: float):
+    """normalizer's feature range (scgnn2.py:797-804): (q0.1, q0.9) of base, or (q0, q1) when those two are equal.  q1 is the
+    maximum (numpy's lerp adds a zero to it) and q0 the minimum plus (second smallest − minimum)·0 — the minimum unless that
+    difference overflows, which only a second selection can settle.  Raises like MinMaxScaler for an empty range."""
+    import numpy as np
+    f32 = np.float32
+    if f32(upper) != f32(lower):
+        lo, hi = f32(lower), f32(upper)
+    else:
+        hi = f32(bmax) + f32(0)
+        with np.errstate(over="ignore"):
+            spread = f32(bmax) - f32(bmin)
+        lo = f32(bmin) + f32(0) if np.isfinite(spread) else quantiles(base, [0.0])[0]
+    if lo >= hi:
+        raise ValueError(f"Minimum of desired feature range must be smaller than maximum. Got {(lo, hi)}.")
+    return float(lo), float(hi)
+
+
+def concat_normalized(left: torch.Tensor, right: torch.Tensor, base: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``[left | normalizer(right, base)]`` (scgnn2.py:795-805 then np.concatenate along columns), or ``[left | right]`` unscaled
+    when ``base`` is None.  normalizer = np.quantile(base, 0.9 / 0.1) (all elements of base, exact) and sklearn's
+    minmax_scale(right, feature_range, axis=0) in float32, bit for bit; a non-finite element of base or right raises
+    ``ValueError``, as does an empty feature range.  Returns an [N, a + e] view of an [N, pitch] buffer whose pitch is a + e
+    rounded up to a multiple of 4, so GEMMs and the kNN on it stay on their tensor-core paths.  With ``base`` it synchronises once."""
+    _chk(left, torch.float32, "left", 2)
+    _chk(right, torch.float32, "right", 2)
+    n, a = left.shape
+    e = right.shape[1]
+    if right.shape[0] != n:
+        raise B2Error(f"concat_normalized: left has {n} rows, right {right.shape[0]}")
+    pitch = (a + e + 3) // 4 * 4
+    out = torch.empty((n, pitch), dtype=torch.float32, device=left.device)
+    lo = hi = 0.0
+    cmin = cmax = None
+    if base is not None:
+        res = torch.empty(6, dtype=torch.float64, device=left.device)   # q0.9, q0.1, min, max, #non-finite base, #non-finite right
+        _quantiles_launch(base, (0.9, 0.1), res[0:5])
+        cmin, cmax = col_minmax(right, nonfinite=res[5:6])
+        upper, lower, bmin, bmax, bad_base, bad_right = res.tolist()
+        if bad_base > 0:
+            raise ValueError(f"normalizer: base holds {int(bad_base)} non-finite values")
+        if bad_right > 0:
+            raise ValueError(f"normalizer: the matrix to scale holds {int(bad_right)} non-finite values")
+        lo, hi = _feature_range(base, upper, lower, bmin, bmax)
+    ws = _workspace(lib().b2_concat_scaled_workspace_bytes(e), left.device)
+    check(lib().b2_concat_scaled_f32(_p(left), _rowmajor(left, "left"), a, _p(right), _rowmajor(right, "right"), e, n, _p(cmin),
+                                     _p(cmax), lo, hi, int(base is not None), _p(out), pitch, _p(ws), ws.numel(), _stream()),
+          "b2_concat_scaled_f32")
+    return out[:, :a + e]

@@ -600,6 +600,34 @@ int b2_louvain_csr_host(const int64_t* rowptr, const int32_t* colidx, const doub
                         int32_t* n_comm_out, double* modularity_out, int max_levels, double min_gain);
 
 /* ------------------------------------------------------------------------
+ * scGNN's normalizer(X, base) (scgnn2.py:795-805) and the concatenations that use it: *_concat_prev_embed
+ * (feature_AE_handler scgnn2.py:283-294, graph_AE_handler scgnn2.py:543-546) and clustering_embed = "both" (scgnn2.py:155-157).
+ *   b2_quantiles_f32     : np.quantile(base, qs[j]) over ALL rows*cols elements of the row-padded matrix base (method "linear",
+ *       q cast to float32 first, so the virtual index (n-1)*q is a float32 product; numpy's _get_indexes clamp and float32 _lerp).
+ *       Radix select on the order-preserving uint32 key (-0.0 keyed as +0.0): the order statistics of both quantiles come out of
+ *       the same three histogram passes over base (11 / 11 / 10 bits), with 64-bit counts.  nq in {1, 2}; qs is a HOST array.
+ *       out: nq + 3 DEVICE doubles, written on the stream: the nq quantiles, then min(base), max(base) and the number of
+ *       non-finite elements.  Nothing is synchronised; the caller reads out once.
+ *   b2_col_minmax_f32    : per-column min / max of x ignoring NaN (np.nanmin / nanmax, MinMaxScaler.partial_fit's data_min_ /
+ *       data_max_); an all-NaN column gives NaN.  nonfinite (nullable): one device double, the count of non-finite elements.
+ *   b2_concat_scaled_f32 : out[:, :a] = left; out[:, a:a+e] = right * scale_ + min_ (scale != 0) or right; out[:, a+e:ldo] = 0.
+ *       scale_ / min_ are MinMaxScaler's, in float32: scale_ = (hi - lo) / range (range = cmax - cmin, set to 1 below 10*eps),
+ *       min_ = lo - cmin * scale_; the transform is two separately rounded operations (x *= scale_; x += min_), never an FMA.
+ *       ldo must be a multiple of 4 (so the row-padded result keeps the GEMM / kNN on their tensor-core paths) and out 16-byte
+ *       aligned.  The workspace is used only when scale != 0.
+ * ---------------------------------------------------------------------- */
+size_t b2_quantiles_workspace_bytes(void);
+int b2_quantiles_f32(const float* base, int64_t ldb, int64_t rows, int32_t cols, const float* qs, int32_t nq, double* out,
+                     void* workspace, size_t workspace_bytes, void* stream);
+size_t b2_col_minmax_workspace_bytes(int32_t cols);
+int b2_col_minmax_f32(const float* x, int64_t ldx, int64_t rows, int32_t cols, float* cmin, float* cmax, double* nonfinite,
+                      void* workspace, size_t workspace_bytes, void* stream);
+size_t b2_concat_scaled_workspace_bytes(int32_t e);
+int b2_concat_scaled_f32(const float* left, int64_t ldl, int32_t a, const float* right, int64_t ldr, int32_t e, int64_t rows,
+                         const float* cmin, const float* cmax, float lo, float hi, int scale, float* out, int64_t ldo,
+                         void* workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------
  * Cell-sharded data parallelism inside the C-ABI (SURVEY §8(b)4, §8(e)): NCCL over NVLink, resolved with dlopen at run time
  * (b2_comm_available() == 0 when libnccl.so.2 cannot be loaded).  One communicator per process / GPU:
  *   rank 0: b2_comm_unique_id(id) → ship the 128 bytes to the other ranks by any channel → every rank: b2_comm_init_rank

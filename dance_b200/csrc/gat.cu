@@ -537,55 +537,41 @@ extern "C" int b2_gat_edge_max_f32(const int32_t* rowptr, const int32_t* colidx,
   return B2_OK;
 }
 
+static bool drop_prob_ok(float p) { return p >= 0.f && p <= 1.f; }   // false for NaN
+static AttnDrop make_drop(float p, uint32_t seed, uint32_t key) { return AttnDrop{p, p < 1.f ? 1.f / (1.f - p) : 0.f, seed, key}; }
+
 extern "C" int b2_gat_aggregate_fwd_f32(const int32_t* rowptr, const int32_t* colidx, const float* H, int64_t ldh,
                                         const float* s_src, const float* s_trg, int32_t n, int32_t nheads, int32_t F,
                                         int score_act, float slope, int shift_mode, const float* gmax_dev, float* out,
-                                        int64_t ldo, float* alpha_out, void* stream) {
+                                        int64_t ldo, float* alpha_out, float drop_p, uint32_t seed, uint32_t key, void* stream) {
   B2_REQUIRE(n >= 0 && nheads > 0 && F > 0 && (int64_t)nheads * F <= 512 && ldh >= (int64_t)nheads * F && ldo >= (int64_t)nheads * F,
              "b2_gat_aggregate_fwd_f32: nheads*F must be <= 512 and leading dimensions >= nheads*F");
+  B2_REQUIRE(drop_prob_ok(drop_p), "b2_gat_aggregate_fwd_f32: drop_p must be in [0, 1]");
+  B2_REQUIRE(drop_p == 0.f || nheads <= 32, "b2_gat_aggregate_fwd_f32: attention dropout needs nheads <= 32");
   B2_REQUIRE(shift_mode == 1 || gmax_dev, "b2_gat_aggregate_fwd_f32: global shift needs gmax_dev");
   if (n == 0) return B2_OK;
   B2_REQUIRE(rowptr && colidx && H && s_src && s_trg && out, "b2_gat_aggregate_fwd_f32: null pointer");
-  gat_aggregate_fwd_kernel<false><<<warp_rows_grid(n), 256, 0, as_stream(stream)>>>(rowptr, colidx, H, ldh, s_src, s_trg, n, nheads, F,
-                                                                                  score_act, slope, shift_mode, gmax_dev, out, ldo,
-                                                                                  alpha_out, AttnDrop{});
+  const auto kernel = drop_p > 0.f ? gat_aggregate_fwd_kernel<true> : gat_aggregate_fwd_kernel<false>;
+  kernel<<<warp_rows_grid(n), 256, 0, as_stream(stream)>>>(rowptr, colidx, H, ldh, s_src, s_trg, n, nheads, F, score_act, slope,
+                                                           shift_mode, gmax_dev, out, ldo, alpha_out, make_drop(drop_p, seed, key));
   B2_CHECK_LAUNCH("gat_aggregate_fwd_kernel");
   return B2_OK;
 }
 
-static bool drop_prob_ok(float p) { return p >= 0.f && p <= 1.f; }   // false for NaN
-static AttnDrop make_drop(float p, uint32_t seed, uint32_t key) { return AttnDrop{p, p < 1.f ? 1.f / (1.f - p) : 0.f, seed, key}; }
-
-extern "C" int b2_gat_aggregate_fwd_drop_f32(const int32_t* rowptr, const int32_t* colidx, const float* H, int64_t ldh,
-                                             const float* s_src, const float* s_trg, int32_t n, int32_t nheads, int32_t F,
-                                             int score_act, float slope, int shift_mode, const float* gmax_dev, float* out,
-                                             int64_t ldo, float* alpha_out, float drop_p, uint32_t seed, uint32_t key,
-                                             void* stream) {
-  B2_REQUIRE(n >= 0 && nheads > 0 && nheads <= 32 && F > 0 && (int64_t)nheads * F <= 512 && ldh >= (int64_t)nheads * F &&
-                 ldo >= (int64_t)nheads * F,
-             "b2_gat_aggregate_fwd_drop_f32: nheads must be <= 32, nheads*F <= 512 and leading dimensions >= nheads*F");
-  B2_REQUIRE(drop_prob_ok(drop_p), "b2_gat_aggregate_fwd_drop_f32: drop_p must be in [0, 1]");
-  B2_REQUIRE(shift_mode == 1 || gmax_dev, "b2_gat_aggregate_fwd_drop_f32: global shift needs gmax_dev");
-  if (n == 0) return B2_OK;
-  B2_REQUIRE(rowptr && colidx && H && s_src && s_trg && out, "b2_gat_aggregate_fwd_drop_f32: null pointer");
-  gat_aggregate_fwd_kernel<true><<<warp_rows_grid(n), 256, 0, as_stream(stream)>>>(rowptr, colidx, H, ldh, s_src, s_trg, n, nheads, F,
-                                                                                 score_act, slope, shift_mode, gmax_dev, out, ldo,
-                                                                                 alpha_out, make_drop(drop_p, seed, key));
-  B2_CHECK_LAUNCH("gat_aggregate_fwd_kernel<drop>");
-  return B2_OK;
-}
-
-static int gat_aggregate_bwd_impl(const int32_t* rowptr, const int32_t* colidx, const int32_t* t_rowptr,
-                                  const int32_t* t_colidx, const int32_t* t_perm, const float* H, int64_t ldh,
-                                  const float* a_src, const float* a_trg, const float* s_src, const float* s_trg,
-                                  const float* alpha, const float* dOut, int64_t lddo, const float* H2, int64_t ldh2,
-                                  const float* dOut2, int64_t lddo2, int32_t n, int32_t nheads, int32_t F, int score_act,
-                                  float slope, const float* gmax_dev, float* dH, int64_t lddh, float* dH2, int64_t lddh2,
-                                  float* da_src, float* da_trg, float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws,
-                                  float* shift_ws, const AttnDrop* drop, void* stream) {
+extern "C" int b2_gat_aggregate_bwd_f32(const int32_t* rowptr, const int32_t* colidx, const int32_t* t_rowptr,
+                                        const int32_t* t_colidx, const int32_t* t_perm, const float* H, int64_t ldh,
+                                        const float* a_src, const float* a_trg, const float* s_src, const float* s_trg,
+                                        const float* alpha, const float* dOut, int64_t lddo, const float* H2, int64_t ldh2,
+                                        const float* dOut2, int64_t lddo2, int32_t n, int32_t nheads, int32_t F, int score_act,
+                                        float slope, const float* gmax_dev, float* dH, int64_t lddh, float* dH2, int64_t lddh2,
+                                        float* da_src, float* da_trg, float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws,
+                                        float* shift_ws, float drop_p, uint32_t seed, uint32_t key, void* stream) {
   B2_REQUIRE(n >= 0 && nheads > 0 && nheads <= 32 && F > 0 && (int64_t)nheads * F <= 512, "b2_gat_aggregate_bwd_f32: bad shape");
   B2_REQUIRE(a_src && a_trg && da_src && da_trg, "b2_gat_aggregate_bwd_f32: null pointer");
   B2_REQUIRE(!gmax_dev || shift_ws, "b2_gat_aggregate_bwd_f32: a global shift (gmax_dev) needs shift_ws");
+  B2_REQUIRE(!H2 || dOut2, "b2_gat_aggregate_bwd_f32: a tied second layer (H2) needs its dOut2");
+  B2_REQUIRE(drop_prob_ok(drop_p), "b2_gat_aggregate_bwd_f32: drop_p must be in [0, 1]");
+  B2_REQUIRE(!H2 || drop_p == 0.f, "b2_gat_aggregate_bwd_f32: the tied backward has no attention dropout");
   cudaStream_t st = as_stream(stream);
   const int W = nheads * F;
   B2_CHECK_CUDA(cudaMemsetAsync(da_src, 0, sizeof(float) * W, st));
@@ -595,28 +581,19 @@ static int gat_aggregate_bwd_impl(const int32_t* rowptr, const int32_t* colidx, 
                  ds_trg_ws && dpre_edge_ws,
              "b2_gat_aggregate_bwd_f32: null pointer");
   if (gmax_dev) B2_CHECK_CUDA(cudaMemsetAsync(shift_ws, 0, sizeof(float) * 2, st));
-  if (drop)
-    gat_bwd_target_kernel<true><<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, H, ldh, s_src, s_trg, alpha, dOut, lddo, H2, ldh2,
-                                                                  dOut2, lddo2, n, nheads, F, score_act, slope, gmax_dev, dpre_edge_ws,
-                                                                  ds_trg_ws, shift_ws, *drop);
-  else
-    gat_bwd_target_kernel<false><<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, H, ldh, s_src, s_trg, alpha, dOut, lddo, H2, ldh2,
-                                                                   dOut2, lddo2, n, nheads, F, score_act, slope, gmax_dev, dpre_edge_ws,
-                                                                   ds_trg_ws, shift_ws, AttnDrop{});
+  const AttnDrop drop = make_drop(drop_p, seed, key);
+  const auto target_kernel = drop_p > 0.f ? gat_bwd_target_kernel<true> : gat_bwd_target_kernel<false>;
+  target_kernel<<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, H, ldh, s_src, s_trg, alpha, dOut, lddo, H2, ldh2, dOut2, lddo2, n,
+                                                   nheads, F, score_act, slope, gmax_dev, dpre_edge_ws, ds_trg_ws, shift_ws, drop);
   B2_CHECK_LAUNCH("gat_bwd_target_kernel");
   if (gmax_dev) {
     gat_bwd_shift_kernel<<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, s_src, s_trg, n, nheads, score_act, slope, gmax_dev,
                                                            shift_ws, dpre_edge_ws, ds_trg_ws);
     B2_CHECK_LAUNCH("gat_bwd_shift_kernel");
   }
-  if (drop)
-    gat_bwd_source_kernel<true><<<warp_rows_grid(n), 256, 0, st>>>(t_rowptr, t_colidx, t_perm, alpha, dpre_edge_ws, dOut, lddo,
-                                                                  dH2 ? dOut2 : nullptr, lddo2, n, nheads, F, dH, lddh, dH2, lddh2,
-                                                                  ds_src_ws, *drop);
-  else
-    gat_bwd_source_kernel<false><<<warp_rows_grid(n), 256, 0, st>>>(t_rowptr, t_colidx, t_perm, alpha, dpre_edge_ws, dOut, lddo,
-                                                                   dH2 ? dOut2 : nullptr, lddo2, n, nheads, F, dH, lddh, dH2, lddh2,
-                                                                   ds_src_ws, AttnDrop{});
+  const auto source_kernel = drop_p > 0.f ? gat_bwd_source_kernel<true> : gat_bwd_source_kernel<false>;
+  source_kernel<<<warp_rows_grid(n), 256, 0, st>>>(t_rowptr, t_colidx, t_perm, alpha, dpre_edge_ws, dOut, lddo, dH2 ? dOut2 : nullptr,
+                                                   lddo2, n, nheads, F, dH, lddh, dH2, lddh2, ds_src_ws, drop);
   B2_CHECK_LAUNCH("gat_bwd_source_kernel");
   int splits = ceil_div(sm_count() * 2, ceil_div(W, 32));
   const int max_splits = n / 256 > 0 ? n / 256 : 1;
@@ -628,90 +605,35 @@ static int gat_aggregate_bwd_impl(const int32_t* rowptr, const int32_t* colidx, 
   return B2_OK;
 }
 
-extern "C" int b2_gat_aggregate_bwd_f32(const int32_t* rowptr, const int32_t* colidx, const int32_t* t_rowptr,
-                                        const int32_t* t_colidx, const int32_t* t_perm, const float* H, int64_t ldh,
-                                        const float* a_src, const float* a_trg, const float* s_src, const float* s_trg,
-                                        const float* alpha, const float* dOut, int64_t lddo, int32_t n, int32_t nheads,
-                                        int32_t F, int score_act, float slope, const float* gmax_dev, float* dH, int64_t lddh,
-                                        float* da_src, float* da_trg, float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws,
-                                        float* shift_ws, void* stream) {
-  return gat_aggregate_bwd_impl(rowptr, colidx, t_rowptr, t_colidx, t_perm, H, ldh, a_src, a_trg, s_src, s_trg, alpha, dOut, lddo,
-                                nullptr, 0, nullptr, 0, n, nheads, F, score_act, slope, gmax_dev, dH, lddh, nullptr, 0, da_src,
-                                da_trg, ds_src_ws, ds_trg_ws, dpre_edge_ws, shift_ws, nullptr, stream);
-}
-
-extern "C" int b2_gat_aggregate_bwd_drop_f32(const int32_t* rowptr, const int32_t* colidx, const int32_t* t_rowptr,
-                                             const int32_t* t_colidx, const int32_t* t_perm, const float* H, int64_t ldh,
-                                             const float* a_src, const float* a_trg, const float* s_src, const float* s_trg,
-                                             const float* alpha, const float* dOut, int64_t lddo, int32_t n, int32_t nheads,
-                                             int32_t F, int score_act, float slope, const float* gmax_dev, float* dH, int64_t lddh,
-                                             float* da_src, float* da_trg, float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws,
-                                             float* shift_ws, float drop_p, uint32_t seed, uint32_t key, void* stream) {
-  B2_REQUIRE(drop_prob_ok(drop_p), "b2_gat_aggregate_bwd_drop_f32: drop_p must be in [0, 1]");
-  const AttnDrop drop = make_drop(drop_p, seed, key);
-  return gat_aggregate_bwd_impl(rowptr, colidx, t_rowptr, t_colidx, t_perm, H, ldh, a_src, a_trg, s_src, s_trg, alpha, dOut, lddo,
-                                nullptr, 0, nullptr, 0, n, nheads, F, score_act, slope, gmax_dev, dH, lddh, nullptr, 0, da_src,
-                                da_trg, ds_src_ws, ds_trg_ws, dpre_edge_ws, shift_ws, &drop, stream);
-}
-
-extern "C" int b2_gat_aggregate_bwd_tied_f32(const int32_t* rowptr, const int32_t* colidx, const int32_t* t_rowptr,
-                                             const int32_t* t_colidx, const int32_t* t_perm, const float* H, int64_t ldh,
-                                             const float* a_src, const float* a_trg, const float* s_src, const float* s_trg,
-                                             const float* alpha, const float* dOut, int64_t lddo, const float* H2, int64_t ldh2,
-                                             const float* dOut2, int64_t lddo2, int32_t n, int32_t nheads, int32_t F,
-                                             int score_act, float slope, const float* gmax_dev, float* dH, int64_t lddh,
-                                             float* dH2, int64_t lddh2, float* da_src, float* da_trg, float* ds_src_ws,
-                                             float* ds_trg_ws, float* dpre_edge_ws, float* shift_ws, void* stream) {
-  B2_REQUIRE(n == 0 || (H2 && dOut2), "b2_gat_aggregate_bwd_tied_f32: the second layer's H2 / dOut2 are required (dH2 may be NULL)");
-  return gat_aggregate_bwd_impl(rowptr, colidx, t_rowptr, t_colidx, t_perm, H, ldh, a_src, a_trg, s_src, s_trg, alpha, dOut, lddo,
-                                H2, ldh2, dOut2, lddo2, n, nheads, F, score_act, slope, gmax_dev, dH, lddh, dH2, lddh2, da_src,
-                                da_trg, ds_src_ws, ds_trg_ws, dpre_edge_ws, shift_ws, nullptr, stream);
-}
-
 extern "C" int b2_gat_combine_fwd_f32(const float* agg, int64_t ldagg, const float* skip, int64_t ldskip, const float* bias,
-                                      int32_t n, int32_t nheads, int32_t F, int concat, int act, float* out, int64_t ldo,
-                                      void* stream) {
+                                      int32_t n, int32_t nheads, int32_t F, int concat, int act, int identity_skip, float* out,
+                                      int64_t ldo, void* stream) {
   B2_REQUIRE(n >= 0 && nheads > 0 && F > 0, "b2_gat_combine_fwd_f32: bad arguments");
+  B2_REQUIRE(!identity_skip || ldskip >= F, "b2_gat_combine_fwd_f32: an identity skip needs ldskip >= F");
   if (n == 0) return B2_OK;
-  B2_REQUIRE(agg && out, "b2_gat_combine_fwd_f32: null pointer");
-  gat_combine_fwd_kernel<false><<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
-      agg, ldagg, skip, ldskip, bias, n, nheads, F, concat, act, out, ldo);
+  B2_REQUIRE(agg && out && (skip || !identity_skip), "b2_gat_combine_fwd_f32: null pointer");
+  const auto kernel = identity_skip ? gat_combine_fwd_kernel<true> : gat_combine_fwd_kernel<false>;
+  kernel<<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(agg, ldagg, skip, ldskip, bias, n, nheads, F,
+                                                                                         concat, act, out, ldo);
   B2_CHECK_LAUNCH("gat_combine_fwd_kernel");
-  return B2_OK;
-}
-
-extern "C" int b2_gat_combine_fwd_identity_f32(const float* agg, int64_t ldagg, const float* x, int64_t ldx, const float* bias,
-                                               int32_t n, int32_t nheads, int32_t F, int concat, int act, float* out, int64_t ldo,
-                                               void* stream) {
-  B2_REQUIRE(n >= 0 && nheads > 0 && F > 0 && ldx >= F, "b2_gat_combine_fwd_identity_f32: bad arguments");
-  if (n == 0) return B2_OK;
-  B2_REQUIRE(agg && x && out, "b2_gat_combine_fwd_identity_f32: null pointer");
-  gat_combine_fwd_kernel<true><<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
-      agg, ldagg, x, ldx, bias, n, nheads, F, concat, act, out, ldo);
-  B2_CHECK_LAUNCH("gat_combine_fwd_kernel<identity>");
   return B2_OK;
 }
 
 extern "C" int b2_gat_combine_bwd_f32(const float* dout, int64_t lddo, const float* out, int64_t ldo, int32_t n,
                                       int32_t nheads, int32_t F, int concat, int act, float* dpre, int64_t ldp, float* dact,
-                                      int64_t ldact, void* stream) {
+                                      int64_t ldact, float* dx_skip, int64_t ldx, void* stream) {
   B2_REQUIRE(n >= 0 && nheads > 0 && F > 0, "b2_gat_combine_bwd_f32: bad arguments");
+  B2_REQUIRE(!dx_skip || ldx >= F, "b2_gat_combine_bwd_f32: dx_skip needs ldx >= F");
   if (n == 0) return B2_OK;
   B2_REQUIRE(dout && out && dpre, "b2_gat_combine_bwd_f32: null pointer");
-  gat_combine_bwd_kernel<<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
-      dout, lddo, out, ldo, n, nheads, F, concat, act, dpre, ldp, dact, ldact);
-  B2_CHECK_LAUNCH("gat_combine_bwd_kernel");
-  return B2_OK;
-}
-
-extern "C" int b2_gat_combine_bwd_identity_f32(const float* dout, int64_t lddo, const float* out, int64_t ldo, int32_t n,
-                                               int32_t nheads, int32_t F, int concat, int act, float* dpre, int64_t ldp, float* dact,
-                                               int64_t ldact, float* dx_skip, int64_t ldx, void* stream) {
-  B2_REQUIRE(n >= 0 && nheads > 0 && F > 0 && ldx >= F, "b2_gat_combine_bwd_identity_f32: bad arguments");
-  if (n == 0) return B2_OK;
-  B2_REQUIRE(dout && out && dpre && dx_skip, "b2_gat_combine_bwd_identity_f32: null pointer");
-  gat_combine_bwd_identity_kernel<<<ew_blocks((int64_t)n * F), 256, 0, as_stream(stream)>>>(dout, lddo, out, ldo, n, nheads, F, concat,
-                                                                                           act, dpre, ldp, dact, ldact, dx_skip, ldx);
-  B2_CHECK_LAUNCH("gat_combine_bwd_identity_kernel");
+  if (dx_skip) {
+    gat_combine_bwd_identity_kernel<<<ew_blocks((int64_t)n * F), 256, 0, as_stream(stream)>>>(dout, lddo, out, ldo, n, nheads, F, concat,
+                                                                                             act, dpre, ldp, dact, ldact, dx_skip, ldx);
+    B2_CHECK_LAUNCH("gat_combine_bwd_identity_kernel");
+  } else {
+    gat_combine_bwd_kernel<<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
+        dout, lddo, out, ldo, n, nheads, F, concat, act, dpre, ldp, dact, ldact);
+    B2_CHECK_LAUNCH("gat_combine_bwd_kernel");
+  }
   return B2_OK;
 }

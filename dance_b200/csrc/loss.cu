@@ -171,59 +171,14 @@ gae_allpairs_kernel(const float* __restrict__ z, int64_t ldz, int32_t n, int32_t
   }
 }
 
-// edge (label) correction: one warp per row i, lanes stride over the row's entries
-template <int D>
-__global__ void __launch_bounds__(256)
-gae_edges_kernel(const float* __restrict__ z, int64_t ldz, const int32_t* __restrict__ rowptr,
-                 const int32_t* __restrict__ colidx, int32_t row_begin, int32_t n_rows, float coef, float pw, int use_pw,
-                 float* __restrict__ dz, double* __restrict__ loss_acc) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  double loss = 0.0;
-  for (int64_t i = warp; i < n_rows; i += nwarps) {
-    float zi[D], acc[D];
-#pragma unroll
-    for (int d = 0; d < D; ++d) { zi[d] = __ldg(z + (row_begin + i) * ldz + d); acc[d] = 0.f; }
-    const int32_t s = rowptr[i], e = rowptr[i + 1];
-    for (int32_t p = s + lane; p < e; p += 32) {
-      const int32_t j = colidx[p];
-      float zjv[D];
-      float x = 0.f;
-#pragma unroll
-      for (int d = 0; d < D; ++d) { zjv[d] = __ldg(z + (int64_t)j * ldz + d); x = fmaf(zi[d], zjv[d], x); }
-      float hval, hgrad;
-      if (use_pw) {
-        const float sg = sigmoid_f(x);
-        hval = pw * softplus_f(-x) - softplus_f(x);
-        hgrad = -pw * (1.f - sg) - sg;
-      } else {
-        hval = -x;
-        hgrad = -1.f;
-      }
-      loss += (double)hval;
-#pragma unroll
-      for (int d = 0; d < D; ++d) acc[d] = fmaf(hgrad, zjv[d], acc[d]);
-    }
-#pragma unroll
-    for (int d = 0; d < D; ++d) acc[d] = warp_sum(acc[d]);
-    if (lane == 0) {
-      const float c2 = 2.f * coef;
-#pragma unroll
-      for (int d = 0; d < D; ++d) dz[i * D + d] += c2 * acc[d];
-    }
-  }
-  loss = warp_sum(loss);
-  if (lane == 0 && loss != 0.0) atomicAdd(loss_acc, loss * (double)coef);
-}
-
-// Label correction for real-valued, asymmetric labels y (graph_AE_retain_weights, scgnn2.py:555-569, 603-619).
+// Label correction (graph_AE_retain_weights: real-valued, asymmetric labels y, scgnn2.py:555-569, 603-619).
 // Per entry ℓ = (1−y)·softplus(x) + y·(y·pw)·softplus(−x)  (pos_weight = labels·pw), so over the label pattern
 //   h(x, y) = y²·pw·softplus(−x) − y·softplus(x),   h' = −y²·pw·σ(−x) − y·σ(x)     (pos-weighted BCE)
 //   h(x, y) = −y·x,                                 h' = −y                        (plain BCE)
 // x_ij = x_ji, so dS/dz_i = 2·Σ_j σ(x_ij) z_j + Σ_{j∈L_i} h'(x_ij, y_ij) z_j + Σ_{j∈Lᵀ_i} h'(x_ij, y_ji) z_j:
 // row i of L (entries (i, j), values y_ij) gives the loss and the first sum, row i of Lᵀ (entries (j, i), values y_ji) the
-// second.  One warp per row, lanes stride over the row's entries.
+// second.  Unit labels (!WEIGHTED, y = 1) have L = Lᵀ: one pass over row i of L with the label sum doubled.
+// One warp per row, lanes stride over the row's entries.
 __device__ __forceinline__ void gae_label_terms(float x, float y, float pw, int use_pw, float& hval, float& hgrad) {
   if (use_pw) {
     const float sg = sigmoid_f(x), ypw = y * y * pw;
@@ -235,7 +190,7 @@ __device__ __forceinline__ void gae_label_terms(float x, float y, float pw, int 
   }
 }
 
-template <int D>
+template <int D, bool WEIGHTED>
 __global__ void __launch_bounds__(256)
 gae_edges_weighted_kernel(const float* __restrict__ z, int64_t ldz, const int32_t* __restrict__ rowptr,
                           const int32_t* __restrict__ colidx, const float* __restrict__ y, const int32_t* __restrict__ t_rowptr,
@@ -250,7 +205,7 @@ gae_edges_weighted_kernel(const float* __restrict__ z, int64_t ldz, const int32_
 #pragma unroll
     for (int d = 0; d < D; ++d) { zi[d] = __ldg(z + (row_begin + i) * ldz + d); acc[d] = 0.f; }
 #pragma unroll 1
-    for (int pass = 0; pass < 2; ++pass) {          // pass 0: row i of L (loss + gradient), pass 1: row i of Lᵀ (gradient)
+    for (int pass = 0; pass < (WEIGHTED ? 2 : 1); ++pass) {   // pass 0: row i of L (loss + gradient), pass 1: row i of Lᵀ (gradient)
       const int32_t* rp = pass ? t_rowptr : rowptr;
       const int32_t* ci = pass ? t_colidx : colidx;
       const float* yv = pass ? t_y : y;
@@ -262,7 +217,7 @@ gae_edges_weighted_kernel(const float* __restrict__ z, int64_t ldz, const int32_
 #pragma unroll
         for (int d = 0; d < D; ++d) { zjv[d] = __ldg(z + (int64_t)j * ldz + d); x = fmaf(zi[d], zjv[d], x); }
         float hval, hgrad;
-        gae_label_terms(x, yv[p], pw, use_pw, hval, hgrad);
+        gae_label_terms(x, WEIGHTED ? yv[p] : 1.f, pw, use_pw, hval, hgrad);
         if (pass == 0) loss += (double)hval;
 #pragma unroll
         for (int d = 0; d < D; ++d) acc[d] = fmaf(hgrad, zjv[d], acc[d]);
@@ -271,8 +226,9 @@ gae_edges_weighted_kernel(const float* __restrict__ z, int64_t ldz, const int32_
 #pragma unroll
     for (int d = 0; d < D; ++d) acc[d] = warp_sum(acc[d]);
     if (lane == 0) {
+      const float c = WEIGHTED ? coef : 2.f * coef;
 #pragma unroll
-      for (int d = 0; d < D; ++d) dz[i * D + d] += coef * acc[d];
+      for (int d = 0; d < D; ++d) dz[i * D + d] += c * acc[d];
     }
   }
   loss = warp_sum(loss);
@@ -343,20 +299,8 @@ static int launch_gae_allpairs(const float* z, int64_t ldz, int32_t n, int32_t r
   return B2_OK;
 }
 
-template <int D>
-static int launch_gae_edges(const float* z, int64_t ldz, const int32_t* rp, const int32_t* ci, int32_t row_begin, int32_t n_rows,
-                            float coef, float pw, int use_pw, float* dz, double* acc, cudaStream_t st) {
-  int64_t blocks = ceil_div<int64_t>(n_rows, 8);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  gae_edges_kernel<D><<<(unsigned)blocks, 256, 0, st>>>(z, ldz, rp, ci, row_begin, n_rows, coef, pw, use_pw, dz, acc);
-  B2_CHECK_LAUNCH("gae_edges_kernel");
-  return B2_OK;
-}
-
-// The label matrix of a call: the local rows of L (unit entries when vals is NULL, then L must be symmetric), and for
-// real-valued labels also the local rows of Lᵀ with their values.
+// The label matrix of a call: the local rows of L, with unit entries when vals is NULL (then L must be symmetric and the
+// transposed rows are not read), else with their values and the local rows of Lᵀ with theirs.
 struct Labels {
   const int32_t *rowptr, *colidx;
   const float* vals;
@@ -365,14 +309,15 @@ struct Labels {
 };
 
 template <int D>
-static int launch_gae_edges_weighted(const float* z, int64_t ldz, const Labels& lab, int32_t row_begin, int32_t n_rows, float coef,
-                                     float pw, int use_pw, float* dz, double* acc, cudaStream_t st) {
+static int launch_gae_edges(const float* z, int64_t ldz, const Labels& lab, int32_t row_begin, int32_t n_rows, float coef, float pw,
+                            int use_pw, float* dz, double* acc, cudaStream_t st) {
   int64_t blocks = ceil_div<int64_t>(n_rows, 8);
   const int64_t cap = (int64_t)sm_count() * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  gae_edges_weighted_kernel<D><<<(unsigned)blocks, 256, 0, st>>>(z, ldz, lab.rowptr, lab.colidx, lab.vals, lab.t_rowptr, lab.t_colidx,
-                                                                  lab.t_vals, row_begin, n_rows, coef, pw, use_pw, dz, acc);
+  const auto kernel = lab.vals ? gae_edges_weighted_kernel<D, true> : gae_edges_weighted_kernel<D, false>;
+  kernel<<<(unsigned)blocks, 256, 0, st>>>(z, ldz, lab.rowptr, lab.colidx, lab.vals, lab.t_rowptr, lab.t_colidx, lab.t_vals, row_begin,
+                                           n_rows, coef, pw, use_pw, dz, acc);
   B2_CHECK_LAUNCH("gae_edges_weighted_kernel");
   return B2_OK;
 }
@@ -386,12 +331,12 @@ struct AllPairs {
 
 // Every decoder entry point; fn names the one called in error messages.
 static int gae_loss_grad(const char* fn, const AllPairs& ap, const float* z, int64_t ldz, const float* mu, const float* logvar,
-                         int64_t ldm, const Labels& lab, bool weighted, int32_t n, int32_t d, int32_t row_begin,
+                         int64_t ldm, const Labels& lab, int32_t n, int32_t d, int32_t row_begin,
                          int32_t n_rows, float norm, float pos_weight, int use_pos_weight, float* dz, float* dmu, float* dlogvar,
                          int64_t ldd, float* loss_out, void* workspace, size_t workspace_bytes, cudaStream_t st) {
   B2_REQUIRE(z && lab.rowptr && lab.colidx && dz && loss_out, "%s: null pointer", fn);
-  if (weighted)
-    B2_REQUIRE(lab.vals && lab.t_rowptr && lab.t_colidx && lab.t_vals, "%s: null pointer (label values and the transposed labels are required)", fn);
+  if (lab.vals)
+    B2_REQUIRE(lab.t_rowptr && lab.t_colidx && lab.t_vals, "%s: null pointer (label values need the transposed labels)", fn);
   B2_REQUIRE(n > 0 && d > 0 && ldz >= d, "%s: bad shape", fn);
   B2_REQUIRE(row_begin >= 0 && n_rows >= 0 && row_begin + n_rows <= n, "%s: bad row range", fn);
   B2_REQUIRE((mu == nullptr) == (logvar == nullptr), "%s: mu/logvar must both be given or both NULL", fn);
@@ -422,9 +367,7 @@ static int gae_loss_grad(const char* fn, const AllPairs& ap, const float* z, int
     rc = with_d(d, [&](auto D) { return launch_gae_allpairs<D>(z, ldz, n, row_begin, n_rows, coef, dz, acc, st); });
   if (rc != B2_OK) return rc;
   rc = with_d(d, [&](auto D) {
-    return weighted ? launch_gae_edges_weighted<D>(z, ldz, lab, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz_rows, acc, st)
-                    : launch_gae_edges<D>(z, ldz, lab.rowptr, lab.colidx, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz_rows,
-                                          acc, st);
+    return launch_gae_edges<D>(z, ldz, lab, row_begin, n_rows, coef, pos_weight, use_pos_weight, dz_rows, acc, st);
   });
   if (rc != B2_OK) return rc;
   if (mu) {
@@ -465,26 +408,14 @@ extern "C" size_t b2_gae_loss_workspace_bytes(int32_t n, int32_t d) {
 }
 
 extern "C" int b2_gae_loss_grad_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
-                                    const int32_t* lab_rowptr, const int32_t* lab_colidx, int32_t n, int32_t d,
-                                    int32_t row_begin, int32_t n_rows, float norm, float pos_weight, int use_pos_weight, float* dz, float* dmu,
-                                    float* dlogvar, int64_t ldd, float* loss_out, void* workspace,
-                                    size_t workspace_bytes, void* stream) {
+                                    const int32_t* lab_rowptr, const int32_t* lab_colidx, const float* lab_vals,
+                                    const int32_t* labt_rowptr, const int32_t* labt_colidx, const float* labt_vals, int32_t n, int32_t d,
+                                    int32_t row_begin, int32_t n_rows, float norm, float pos_weight, int use_pos_weight, float* dz,
+                                    float* dmu, float* dlogvar, int64_t ldd, float* loss_out, void* workspace, size_t workspace_bytes,
+                                    void* stream) {
   return gae_loss_grad("b2_gae_loss_grad_f32", AllPairs{false, 0, 0}, z, ldz, mu, logvar, ldm,
-                       Labels{lab_rowptr, lab_colidx, nullptr, nullptr, nullptr, nullptr}, false, n, d, row_begin, n_rows, norm,
+                       Labels{lab_rowptr, lab_colidx, lab_vals, labt_rowptr, labt_colidx, labt_vals}, n, d, row_begin, n_rows, norm,
                        pos_weight, use_pos_weight, dz, dmu, dlogvar, ldd, loss_out, workspace, workspace_bytes, as_stream(stream));
-}
-
-// b2_gae_loss_grad_f32 with real-valued, asymmetric labels (graph_AE_retain_weights): lab_* = the local rows of L,
-// labt_* = the local rows of Lᵀ, both with their label values.
-extern "C" int b2_gae_loss_grad_weighted_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
-                                             const int32_t* lab_rowptr, const int32_t* lab_colidx, const float* lab_vals,
-                                             const int32_t* labt_rowptr, const int32_t* labt_colidx, const float* labt_vals, int32_t n,
-                                             int32_t d, int32_t row_begin, int32_t n_rows, float norm, float pos_weight, int use_pos_weight,
-                                             float* dz, float* dmu, float* dlogvar, int64_t ldd, float* loss_out, void* workspace,
-                                             size_t workspace_bytes, void* stream) {
-  return gae_loss_grad("b2_gae_loss_grad_weighted_f32", AllPairs{false, 0, 0}, z, ldz, mu, logvar, ldm,
-                       Labels{lab_rowptr, lab_colidx, lab_vals, labt_rowptr, labt_colidx, labt_vals}, true, n, d, row_begin, n_rows,
-                       norm, pos_weight, use_pos_weight, dz, dmu, dlogvar, ldd, loss_out, workspace, workspace_bytes, as_stream(stream));
 }
 
 // Pair-sharded form of b2_gae_loss_grad_f32 for multi-GPU runs.  Rank r evaluates the all-pairs part of the super-blocks
@@ -496,23 +427,12 @@ extern "C" int b2_gae_loss_grad_weighted_f32(const float* z, int64_t ldz, const 
 extern "C" int b2_gae_sym_super_blocks(int32_t n) { return b2::gtc::super_blocks(n); }
 
 extern "C" int b2_gae_loss_grad_sym_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
-                                        const int32_t* lab_rowptr, const int32_t* lab_colidx, int32_t n, int32_t d,
-                                        int32_t sb_begin, int32_t sb_end, int32_t row_begin, int32_t n_rows, float norm, float pos_weight,
-                                        int use_pos_weight, float* dz_full, float* dmu, float* dlogvar, int64_t ldd, float* loss_out,
-                                        void* workspace, size_t workspace_bytes, void* stream) {
+                                        const int32_t* lab_rowptr, const int32_t* lab_colidx, const float* lab_vals,
+                                        const int32_t* labt_rowptr, const int32_t* labt_colidx, const float* labt_vals, int32_t n,
+                                        int32_t d, int32_t sb_begin, int32_t sb_end, int32_t row_begin, int32_t n_rows, float norm,
+                                        float pos_weight, int use_pos_weight, float* dz_full, float* dmu, float* dlogvar, int64_t ldd,
+                                        float* loss_out, void* workspace, size_t workspace_bytes, void* stream) {
   return gae_loss_grad("b2_gae_loss_grad_sym_f32", AllPairs{true, sb_begin, sb_end}, z, ldz, mu, logvar, ldm,
-                       Labels{lab_rowptr, lab_colidx, nullptr, nullptr, nullptr, nullptr}, false, n, d, row_begin, n_rows, norm,
+                       Labels{lab_rowptr, lab_colidx, lab_vals, labt_rowptr, labt_colidx, labt_vals}, n, d, row_begin, n_rows, norm,
                        pos_weight, use_pos_weight, dz_full, dmu, dlogvar, ldd, loss_out, workspace, workspace_bytes, as_stream(stream));
-}
-
-extern "C" int b2_gae_loss_grad_sym_weighted_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
-                                                 const int32_t* lab_rowptr, const int32_t* lab_colidx, const float* lab_vals,
-                                                 const int32_t* labt_rowptr, const int32_t* labt_colidx, const float* labt_vals, int32_t n,
-                                                 int32_t d, int32_t sb_begin, int32_t sb_end, int32_t row_begin, int32_t n_rows, float norm,
-                                                 float pos_weight, int use_pos_weight, float* dz_full, float* dmu, float* dlogvar,
-                                                 int64_t ldd, float* loss_out, void* workspace, size_t workspace_bytes, void* stream) {
-  return gae_loss_grad("b2_gae_loss_grad_sym_weighted_f32", AllPairs{true, sb_begin, sb_end}, z, ldz, mu, logvar, ldm,
-                       Labels{lab_rowptr, lab_colidx, lab_vals, labt_rowptr, labt_colidx, labt_vals}, true, n, d, row_begin, n_rows,
-                       norm, pos_weight, use_pos_weight, dz_full, dmu, dlogvar, ldd, loss_out, workspace, workspace_bytes,
-                       as_stream(stream));
 }

@@ -49,7 +49,7 @@ extern "C" {
 
 const char* b2_last_error(void) { return b2::last_error(); }
 
-int b2_version(void) { return 100; }
+int b2_version(void) { return 101; }
 
 int64_t b2_launch_count(void) { return (int64_t)b2::g_launch_count; }
 

@@ -321,7 +321,8 @@ def mse_sum_loss_grad(recon, target, ltmg_regu=None, regu_strength=0.0, relu_mas
 
 
 def _gae_prepare(what, z, labels: CSR, n_rows, mu, logvar, dmu, dlogvar, loss, labels_t: Optional[CSR] = None):
-    """Checks and buffers both decoder calls share; returns (n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, workspace)."""
+    """Checks and buffers both decoder calls share; returns (n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, workspace, label
+    arguments).  The label arguments are the pointers of L and of Lᵀ; the library reads Lᵀ only when L has values."""
     _chk(z, torch.float32, "z", 2)
     n, d = z.shape
     n_rows = n if n_rows is None else n_rows
@@ -347,14 +348,9 @@ def _gae_prepare(what, z, labels: CSR, n_rows, mu, logvar, dmu, dlogvar, loss, l
             raise B2Error(f"{what}: dmu and dlogvar must share a leading dimension")
     if loss is None:
         loss = torch.empty(1, dtype=torch.float32, device=z.device)
-    return n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, _workspace(lib().b2_gae_loss_workspace_bytes(n, d), z.device)
-
-
-def _label_args(labels: CSR, labels_t: Optional[CSR]):
-    """The label arguments of the decoder entry points: (rowptr, colidx) for unit labels, plus values and Lᵀ for real ones."""
-    if labels.vals is None:
-        return [_p(labels.rowptr), _p(labels.colidx)]
-    return [_p(labels.rowptr), _p(labels.colidx), _p(labels.vals), _p(labels_t.rowptr), _p(labels_t.colidx), _p(labels_t.vals)]
+    lt = (labels_t.rowptr, labels_t.colidx, labels_t.vals) if labels_t is not None else (None, None, None)
+    labs = [_p(t) for t in (labels.rowptr, labels.colidx, labels.vals, *lt)]
+    return n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, _workspace(lib().b2_gae_loss_workspace_bytes(n, d), z.device), labs
 
 
 def gae_loss_grad(z, labels: CSR, norm: float, pos_weight: float, mu=None, logvar=None, use_pos_weight=True,
@@ -366,18 +362,17 @@ def gae_loss_grad(z, labels: CSR, norm: float, pos_weight: float, mu=None, logva
     ``labels.vals`` None: unit, symmetric labels.  Otherwise real-valued, possibly asymmetric labels (graph_AE_retain_weights), and
     ``labels_t`` holds the same rows of Lᵀ with their values.
     """
-    n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, ws = _gae_prepare("gae_loss_grad", z, labels, n_rows, mu, logvar, dmu, dlogvar, loss,
-                                                                  labels_t)
+    n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, ws, labs = _gae_prepare("gae_loss_grad", z, labels, n_rows, mu, logvar, dmu, dlogvar,
+                                                                        loss, labels_t)
     if dz is None:
         dz = torch.empty((n_rows, d), dtype=torch.float32, device=z.device)
     else:
         _chk(dz, torch.float32, "dz", 2)
         if tuple(dz.shape) != (n_rows, d) or not dz.is_contiguous():
             raise B2Error(f"gae_loss_grad: dz must be a contiguous [{n_rows}, {d}] buffer, got {tuple(dz.shape)} strides {dz.stride()}")
-    fn = "b2_gae_loss_grad_f32" if labels.vals is None else "b2_gae_loss_grad_weighted_f32"
-    check(getattr(lib(), fn)(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, *_label_args(labels, labels_t), n, d,
-                             row_begin, n_rows, float(norm), float(pos_weight), int(use_pos_weight),
-                             _p(dz), _p(dmu), _p(dlogvar), ldd, _p(loss), _p(ws), ws.numel(), _stream()), fn)
+    check(lib().b2_gae_loss_grad_f32(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, *labs, n, d, row_begin, n_rows, float(norm),
+                                     float(pos_weight), int(use_pos_weight), _p(dz), _p(dmu), _p(dlogvar), ldd, _p(loss), _p(ws),
+                                     ws.numel(), _stream()), "b2_gae_loss_grad_f32")
     return loss, dz, dmu, dlogvar
 
 
@@ -393,17 +388,16 @@ def gae_loss_grad_sym(z, labels: CSR, norm: float, pos_weight: float, sb_begin: 
     ``[sb_begin, sb_end)`` of the unordered block-pair schedule and the label / KLD terms of its rows.  Returns
     ``(loss_share[1], dz_full[n, d], dmu, dlogvar)``; all-reduce ``dz_full`` and ``loss_share`` over ranks.  Real-valued labels
     (``labels.vals`` set) need ``labels_t`` as in :func:`gae_loss_grad`."""
-    n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, ws = _gae_prepare("gae_loss_grad_sym", z, labels, n_rows, mu, logvar, dmu, dlogvar,
-                                                                  loss, labels_t)
+    n, d, n_rows, ldm, ldd, dmu, dlogvar, loss, ws, labs = _gae_prepare("gae_loss_grad_sym", z, labels, n_rows, mu, logvar, dmu,
+                                                                        dlogvar, loss, labels_t)
     if dz_full is None:
         dz_full = torch.empty((n, d), dtype=torch.float32, device=z.device)
     _chk(dz_full, torch.float32, "dz_full", 2)
     if tuple(dz_full.shape) != (n, d) or not dz_full.is_contiguous():
         raise B2Error(f"gae_loss_grad_sym: dz_full must be a contiguous [{n}, {d}] buffer")
-    fn = "b2_gae_loss_grad_sym_f32" if labels.vals is None else "b2_gae_loss_grad_sym_weighted_f32"
-    check(getattr(lib(), fn)(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, *_label_args(labels, labels_t), n, d,
-                             sb_begin, sb_end, row_begin, n_rows, float(norm), float(pos_weight), int(use_pos_weight),
-                             _p(dz_full), _p(dmu), _p(dlogvar), ldd, _p(loss), _p(ws), ws.numel(), _stream()), fn)
+    check(lib().b2_gae_loss_grad_sym_f32(_p(z), _rowmajor(z, "z"), _p(mu), _p(logvar), ldm, *labs, n, d, sb_begin, sb_end,
+                                         row_begin, n_rows, float(norm), float(pos_weight), int(use_pos_weight), _p(dz_full),
+                                         _p(dmu), _p(dlogvar), ldd, _p(loss), _p(ws), ws.numel(), _stream()), "b2_gae_loss_grad_sym_f32")
     return loss, dz_full, dmu, dlogvar
 
 
@@ -600,6 +594,9 @@ def gat_aggregate_fwd(T: CSR, H, s_src, s_trg, nheads: int, score_act="leakyrelu
     the same (dropout, seed, key) to :func:`gat_aggregate_bwd`."""
     n, W = H.shape
     F = _head_width(W, nheads, "gat_aggregate_fwd")
+    if seed is None and dropout:
+        raise ValueError("gat_aggregate_fwd: attention dropout needs a seed")
+    p = _drop_prob(dropout)
     if out is None:
         out = torch.empty((n, W), dtype=torch.float32, device=H.device)
     gmax = torch.empty(1, dtype=torch.float32, device=H.device)
@@ -609,15 +606,9 @@ def gat_aggregate_fwd(T: CSR, H, s_src, s_trg, nheads: int, score_act="leakyrelu
         check(lib().b2_gat_edge_max_f32(_p(T.rowptr), colidx, _p(s_src), _p(s_trg), n, nheads, act, slope, _p(gmax),
                                         _stream()), "b2_gat_edge_max_f32")
     alpha = torch.empty((T.nnz, nheads), dtype=torch.float32, device=H.device) if keep_alpha else None
-    head = (_p(T.rowptr), colidx, _p(H), _rowmajor(H, "H"), _p(s_src), _p(s_trg), n, nheads, F, act, slope, sm, _p(gmax), _p(out),
-            _rowmajor(out, "out"), _p(alpha) if T.nnz else None)
-    if seed is not None:
-        check(lib().b2_gat_aggregate_fwd_drop_f32(*head, _drop_prob(dropout), int(seed) & 0xFFFFFFFF, int(key) & 0xFFFFFFFF,
-                                                  _stream()), "b2_gat_aggregate_fwd_drop_f32")
-    elif dropout:
-        raise ValueError("gat_aggregate_fwd: attention dropout needs a seed")
-    else:
-        check(lib().b2_gat_aggregate_fwd_f32(*head, _stream()), "b2_gat_aggregate_fwd_f32")
+    check(lib().b2_gat_aggregate_fwd_f32(_p(T.rowptr), colidx, _p(H), _rowmajor(H, "H"), _p(s_src), _p(s_trg), n, nheads, F, act, slope,
+                                         sm, _p(gmax), _p(out), _rowmajor(out, "out"), _p(alpha) if T.nnz else None, p,
+                                         int(seed or 0) & 0xFFFFFFFF, int(key) & 0xFFFFFFFF, _stream()), "b2_gat_aggregate_fwd_f32")
     return out, alpha, gmax
 
 
@@ -631,6 +622,9 @@ def gat_aggregate_bwd(T: CSR, Tt: CSR, t_perm, H, a_src, a_trg, s_src, s_trg, al
     ``dropout`` / ``seed`` / ``key``: the forward's attention dropout (not with a tied layer); ``alpha`` is the undropped α."""
     n, W = H.shape
     F = _head_width(W, nheads, "gat_aggregate_bwd")
+    if seed is None and dropout:
+        raise ValueError("gat_aggregate_bwd: attention dropout needs a seed")
+    p = _drop_prob(dropout)
     dev = H.device
     dH = torch.empty((n, W), dtype=torch.float32, device=dev)
     da_src = torch.empty(W, dtype=torch.float32, device=dev)
@@ -641,27 +635,16 @@ def gat_aggregate_bwd(T: CSR, Tt: CSR, t_perm, H, a_src, a_trg, s_src, s_trg, al
     shift_ws = torch.empty(2, dtype=torch.float32, device=dev) if gmax is not None else None
     # an edgeless graph has no colidx / t_perm / alpha storage: any non-NULL pointer stands in, never dereferenced
     edge = (lambda t: _p(t)) if T.nnz else (lambda t: _p(T.rowptr))
-    head = (_p(T.rowptr), edge(T.colidx), _p(Tt.rowptr), edge(Tt.colidx), edge(t_perm), _p(H), _rowmajor(H, "H"), _p(a_src),
-            _p(a_trg), _p(s_src), _p(s_trg), edge(alpha), _p(dOut), _rowmajor(dOut, "dOut"))
-    if seed is None and dropout:
-        raise ValueError("gat_aggregate_bwd: attention dropout needs a seed")
-    if H2 is not None:
-        if seed is not None:
-            raise B2Error("gat_aggregate_bwd: the tied (STAGATE) backward has no attention dropout")
-        dH2 = torch.empty((n, W), dtype=torch.float32, device=dev) if want_dH2 else None
-        check(lib().b2_gat_aggregate_bwd_tied_f32(*head, _p(H2), _rowmajor(H2, "H2"), _p(dOut2), _rowmajor(dOut2, "dOut2"), n, nheads,
-                                                  F, SCORE_ACT[score_act], slope, _p(gmax), _p(dH), _rowmajor(dH, "dH"), _p(dH2),
-                                                  _rowmajor(dH2, "dH2") if want_dH2 else 0, _p(da_src), _p(da_trg), _p(ds_s), _p(ds_t),
-                                                  _p(dpre), _p(shift_ws), _stream()), "b2_gat_aggregate_bwd_tied_f32")
-        return dH, da_src, da_trg, dH2
-    tail = (n, nheads, F, SCORE_ACT[score_act], slope, _p(gmax), _p(dH), _rowmajor(dH, "dH"), _p(da_src), _p(da_trg), _p(ds_s),
-            _p(ds_t), _p(dpre), _p(shift_ws))
-    if seed is not None:
-        check(lib().b2_gat_aggregate_bwd_drop_f32(*head, *tail, _drop_prob(dropout), int(seed) & 0xFFFFFFFF, int(key) & 0xFFFFFFFF,
-                                                  _stream()), "b2_gat_aggregate_bwd_drop_f32")
-    else:
-        check(lib().b2_gat_aggregate_bwd_f32(*head, *tail, _stream()), "b2_gat_aggregate_bwd_f32")
-    return dH, da_src, da_trg
+    tied = H2 is not None
+    dH2 = torch.empty((n, W), dtype=torch.float32, device=dev) if tied and want_dH2 else None
+    check(lib().b2_gat_aggregate_bwd_f32(_p(T.rowptr), edge(T.colidx), _p(Tt.rowptr), edge(Tt.colidx), edge(t_perm), _p(H),
+                                         _rowmajor(H, "H"), _p(a_src), _p(a_trg), _p(s_src), _p(s_trg), edge(alpha), _p(dOut),
+                                         _rowmajor(dOut, "dOut"), _p(H2), _rowmajor(H2, "H2") if tied else 0, _p(dOut2),
+                                         _rowmajor(dOut2, "dOut2") if tied else 0, n, nheads, F, SCORE_ACT[score_act], slope, _p(gmax),
+                                         _p(dH), _rowmajor(dH, "dH"), _p(dH2), _rowmajor(dH2, "dH2") if dH2 is not None else 0,
+                                         _p(da_src), _p(da_trg), _p(ds_s), _p(ds_t), _p(dpre), _p(shift_ws), p,
+                                         int(seed or 0) & 0xFFFFFFFF, int(key) & 0xFFFFFFFF, _stream()), "b2_gat_aggregate_bwd_f32")
+    return (dH, da_src, da_trg, dH2) if tied else (dH, da_src, da_trg)
 
 
 def gat_combine_fwd(agg, skip, bias, nheads: int, concat: bool, act=None, identity: bool = False):
@@ -674,13 +657,9 @@ def gat_combine_fwd(agg, skip, bias, nheads: int, concat: bool, act=None, identi
         _chk(skip, torch.float32, "skip", 2)
         if tuple(skip.shape) != (n, F):
             raise B2Error(f"gat_combine_fwd: an identity skip must have shape {(n, F)}, got {tuple(skip.shape)}")
-        check(lib().b2_gat_combine_fwd_identity_f32(_p(agg), _rowmajor(agg, "agg"), _p(skip), _rowmajor(skip, "skip"), _p(bias), n, nheads,
-                                                    F, int(concat), ACT[act], _p(out), _rowmajor(out, "out"), _stream()),
-              "b2_gat_combine_fwd_identity_f32")
-        return out
     check(lib().b2_gat_combine_fwd_f32(_p(agg), _rowmajor(agg, "agg"), _p(skip), _rowmajor(skip, "skip") if skip is not None else 0,
-                                       _p(bias), n, nheads, F, int(concat), ACT[act], _p(out), _rowmajor(out, "out"), _stream()),
-          "b2_gat_combine_fwd_f32")
+                                       _p(bias), n, nheads, F, int(concat), ACT[act], int(identity), _p(out), _rowmajor(out, "out"),
+                                       _stream()), "b2_gat_combine_fwd_f32")
     return out
 
 
@@ -691,18 +670,15 @@ def gat_combine_bwd(dout, out, nheads: int, F: int, concat: bool, act=None, iden
     if dpre is None:
         dpre = torch.empty((n, nheads * F), dtype=torch.float32, device=dout.device)
     dact = torch.empty_like(out)
-    if identity:
-        if dx_skip is None:
-            dx_skip = torch.empty((n, F), dtype=torch.float32, device=dout.device)
-        check(lib().b2_gat_combine_bwd_identity_f32(_p(dout), _rowmajor(dout, "dout"), _p(out), _rowmajor(out, "out"), n, nheads, F,
-                                                    int(concat), ACT[act], _p(dpre), _rowmajor(dpre, "dpre"), _p(dact),
-                                                    _rowmajor(dact, "dact"), _p(dx_skip), _rowmajor(dx_skip, "dx_skip"), _stream()),
-              "b2_gat_combine_bwd_identity_f32")
-        return dpre, dact, dx_skip
+    if not identity:
+        dx_skip = None
+    elif dx_skip is None:
+        dx_skip = torch.empty((n, F), dtype=torch.float32, device=dout.device)
     check(lib().b2_gat_combine_bwd_f32(_p(dout), _rowmajor(dout, "dout"), _p(out), _rowmajor(out, "out"), n, nheads, F,
                                        int(concat), ACT[act], _p(dpre), _rowmajor(dpre, "dpre"), _p(dact), _rowmajor(dact, "dact"),
-                                       _stream()), "b2_gat_combine_bwd_f32")
-    return dpre, dact
+                                       _p(dx_skip), _rowmajor(dx_skip, "dx_skip") if identity else 0, _stream()),
+          "b2_gat_combine_bwd_f32")
+    return (dpre, dact, dx_skip) if identity else (dpre, dact)
 
 
 # ----------------------------------------------------------------------------- scDeepSort path

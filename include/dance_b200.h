@@ -161,10 +161,15 @@ int b2_mse_sum_loss_grad_f32(const float* recon, const float* target, const floa
  * with InnerProductDecoder scgnn2.py:423-426 (logits = z zᵀ never stored).
  *   cost = norm · mean_{ij} BCEwithLogits(z_i·z_j, L_ij, pos_weight=L_ij·pw)
  *   L = A + I given as CSR (rowptr/colidx, unit entries; diagonal included)
+ *   lab_vals = NULL : unit labels; L must be symmetric (it always is: scgnn2.py:658-664) and labt_* are ignored.
+ *   lab_vals set    : real-valued, asymmetric labels y (graph_AE_retain_weights, scgnn2.py:555-569): lab_* are the local
+ *     rows of L (entries (i, j), values y_ij, diagonal included), labt_* (all three required) the local rows of Lᵀ (row i
+ *     holds the j with (j, i) in L, values y_ji), n_rows+1 row pointers, global column ids.  Per entry
+ *     ℓ = (1−y)·softplus(x) + y²·pw·softplus(−x) (pos_weight = labels·pw); use_pos_weight = 0: ℓ = softplus(x) − y·x.
  *   KLD  = -0.5/n · mean_i Σ_d (1 + 2·logvar - mu² - exp(logvar)²)
  *   loss_out[0] = cost + KLD ; dz [n,d] dense, dmu/dlogvar [n,d] with leading
  *   dimension ldd are OVERWRITTEN with d loss / d z (decoder part) and the KLD
- *   parts respectively.  L must be symmetric (it always is: scgnn2.py:658-664).
+ *   parts respectively.
  *   Row sharding (cell-sharded multi-GPU): z holds all n rows; this call handles rows
  *   [row_begin, row_begin+n_rows): lab_rowptr has n_rows+1 entries (global column ids),
  *   mu/logvar/dz/dmu/dlogvar are the n_rows local rows, and loss_out receives this
@@ -175,23 +180,12 @@ int b2_mse_sum_loss_grad_f32(const float* recon, const float* target, const floa
  *   d ∈ {8, 16, 32, 64}; any other d returns B2_ERR_UNSUPPORTED. */
 size_t b2_gae_loss_workspace_bytes(int32_t n, int32_t d);
 int b2_gae_loss_grad_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
-                         const int32_t* lab_rowptr, const int32_t* lab_colidx,
+                         const int32_t* lab_rowptr, const int32_t* lab_colidx, const float* lab_vals,
+                         const int32_t* labt_rowptr, const int32_t* labt_colidx, const float* labt_vals,
                          int32_t n, int32_t d, int32_t row_begin, int32_t n_rows,
                          float norm, float pos_weight, int use_pos_weight,
                          float* dz, float* dmu, float* dlogvar, int64_t ldd, float* loss_out,
                          void* workspace, size_t workspace_bytes, void* stream);
-/* b2_gae_loss_grad_f32 with real-valued, asymmetric labels y (graph_AE_retain_weights, scgnn2.py:555-569):
- *   lab_*  : the local rows of L (entries (i, j), values y_ij, diagonal included);
- *   labt_* : the local rows of Lᵀ (row i holds the j with (j, i) in L, values y_ji), n_rows+1 row pointers, global column ids.
- * Per entry ℓ = (1−y)·softplus(x) + y²·pw·softplus(−x) (pos_weight = labels·pw); use_pos_weight = 0: ℓ = softplus(x) − y·x.
- * Unit symmetric labels give b2_gae_loss_grad_f32.  The all-pairs part, the KLD and the workspace are those of that call. */
-int b2_gae_loss_grad_weighted_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
-                                  const int32_t* lab_rowptr, const int32_t* lab_colidx, const float* lab_vals,
-                                  const int32_t* labt_rowptr, const int32_t* labt_colidx, const float* labt_vals,
-                                  int32_t n, int32_t d, int32_t row_begin, int32_t n_rows,
-                                  float norm, float pos_weight, int use_pos_weight,
-                                  float* dz, float* dmu, float* dlogvar, int64_t ldd, float* loss_out,
-                                  void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * Optimiser: torch.optim.Adam semantics (scgnn2.py:301,573; default eps 1e-8,
@@ -308,88 +302,63 @@ int b2_gat_scores_f32(const float* H, int64_t ldh, const float* a_src, const flo
 int b2_gat_edge_max_f32(const int32_t* rowptr, const int32_t* colidx,
                         const float* s_src, const float* s_trg, int32_t n, int32_t nheads,
                         int score_act, float slope, float* gmax_dev, void* stream);
+/* Attention dropout (GATLayer, scgnn2.py:1029: α' = drop(α) after the softmax): drop_p in [0, 1], otherwise an error.
+ *   drop_p = 0 is the plain aggregate (seed and key are not read); drop_p > 0 needs nheads <= 32 and drops (edge, head) with
+ *   the keep bit of b2_dropout_f32 at r = the edge's position in the target CSR, c = the head.  alpha_out stays the
+ *   UNDROPPED α, which is what the backward takes with the same (drop_p, seed, key). */
 int b2_gat_aggregate_fwd_f32(const int32_t* rowptr, const int32_t* colidx,
                              const float* H, int64_t ldh, const float* s_src, const float* s_trg,
                              int32_t n, int32_t nheads, int32_t F,
                              int score_act, float slope, int shift_mode, const float* gmax_dev,
-                             float* out, int64_t ldo, float* alpha_out, void* stream);
+                             float* out, int64_t ldo, float* alpha_out,
+                             float drop_p, uint32_t seed, uint32_t key, void* stream);
 /* Backward of scores + aggregate.  (t_rowptr, t_colidx, t_perm) = b2_csr_transpose of the target
  * CSR.  Outputs: dH [n, nheads*F] (overwritten: message path + score path), da_src/da_trg
  * [nheads*F] (overwritten).  ds_src_ws/ds_trg_ws [n*nheads] and dpre_edge_ws [nnz*nheads] are
- * caller-provided scratch.
+ * caller-provided scratch.  nheads <= 32.
  *   gmax_dev : the forward's global shift (shift_mode 0) or NULL (per-target shift, whose max is detached
  *              as in PyG).  The global max is NOT detached in scgnn2.py:1076; since α = p/(Σp + 1e-16) is
  *              shift-invariant only up to the 1e-16, its gradient reaches the argmax score(s) — split evenly
  *              over ties, as torch's max — and matters for targets whose scores lie ~37+ below the max.
- *   shift_ws : [2] caller-provided scratch, needed when gmax_dev is set. */
+ *   shift_ws : [2] caller-provided scratch, needed when gmax_dev is set.
+ *   H2       : NULL, or tied attention (STAGATE, stagate.py:197: conv3 reuses conv1's node scores, so the SAME edge
+ *              coefficients α weight two layers' messages): the second layer's projected features H2 with its upstream
+ *              gradient dOut2 (required):  dα_e = <dOut[v],H[u]> + <dOut2[v],H2[u]> ;  dH2[u] = Σ α dOut2[v] (message path
+ *              only — the scores depend on H; pass dH2 = NULL when the caller already has it).  No attention dropout.
+ *   drop_p, seed, key : the forward's attention dropout. */
 int b2_gat_aggregate_bwd_f32(const int32_t* rowptr, const int32_t* colidx,
                              const int32_t* t_rowptr, const int32_t* t_colidx, const int32_t* t_perm,
                              const float* H, int64_t ldh, const float* a_src, const float* a_trg,
                              const float* s_src, const float* s_trg, const float* alpha,
-                             const float* dOut, int64_t lddo, int32_t n, int32_t nheads, int32_t F,
+                             const float* dOut, int64_t lddo, const float* H2, int64_t ldh2,
+                             const float* dOut2, int64_t lddo2, int32_t n, int32_t nheads, int32_t F,
                              int score_act, float slope, const float* gmax_dev,
-                             float* dH, int64_t lddh, float* da_src, float* da_trg,
-                             float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws, float* shift_ws, void* stream);
-/* Tied attention (STAGATE, stagate.py:197: conv3 reuses conv1's node scores, so the SAME edge coefficients α weight
- * two layers' messages).  As above, plus the second layer's projected features H2 / upstream gradient dOut2:
- *   dα_e = <dOut[v],H[u]> + <dOut2[v],H2[u]> ;  dH2[u] = Σ α dOut2[v] (message path only — the scores depend on H;
- *   pass dH2 = NULL when the caller already has it). */
-int b2_gat_aggregate_bwd_tied_f32(const int32_t* rowptr, const int32_t* colidx,
-                                  const int32_t* t_rowptr, const int32_t* t_colidx, const int32_t* t_perm,
-                                  const float* H, int64_t ldh, const float* a_src, const float* a_trg,
-                                  const float* s_src, const float* s_trg, const float* alpha,
-                                  const float* dOut, int64_t lddo, const float* H2, int64_t ldh2,
-                                  const float* dOut2, int64_t lddo2, int32_t n, int32_t nheads, int32_t F,
-                                  int score_act, float slope, const float* gmax_dev,
-                                  float* dH, int64_t lddh, float* dH2, int64_t lddh2, float* da_src, float* da_trg,
-                                  float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws, float* shift_ws, void* stream);
+                             float* dH, int64_t lddh, float* dH2, int64_t lddh2, float* da_src, float* da_trg,
+                             float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws, float* shift_ws,
+                             float drop_p, uint32_t seed, uint32_t key, void* stream);
 /* skip connection + concat | head-mean + bias + activation (scgnn2.py:1189-1215):
  *   concat: out[n, nheads*F] = act(agg + skip + bias) ; else out[n,F] = act(mean_h(agg + skip) + bias)
- *   skip may be NULL.  Backward: dpre [n, nheads*F] = d(agg) = d(skip); dact [n, OW] (optional) is the
- *   gradient before the bias add (its column sums are the bias gradient). */
+ *   skip may be NULL.  identity_skip != 0 (GATLayer with FIN == FOUT, scgnn2.py:1167-1171): skip is the raw input
+ *   x [n, F] (required, ldskip >= F), added to every head as skip[n, h*F + f] = x[n, f].
+ *   Backward: dpre [n, nheads*F] = d(agg) = d(skip); dact [n, OW] (optional) is the gradient before the bias add (its column
+ *   sums are the bias gradient); dx_skip NULL, or for an identity skip dx_skip[n, F] = Σ_h dpre[n, h*F:(h+1)*F] (overwritten,
+ *   ldx >= F). */
 int b2_gat_combine_fwd_f32(const float* agg, int64_t ldagg, const float* skip, int64_t ldskip, const float* bias,
-                           int32_t n, int32_t nheads, int32_t F, int concat, int act,
+                           int32_t n, int32_t nheads, int32_t F, int concat, int act, int identity_skip,
                            float* out, int64_t ldo, void* stream);
 int b2_gat_combine_bwd_f32(const float* dout, int64_t lddo, const float* out, int64_t ldo,
                            int32_t n, int32_t nheads, int32_t F, int concat, int act,
-                           float* dpre, int64_t ldp, float* dact, int64_t ldact, void* stream);
-/* Identity skip (GATLayer with FIN == FOUT, scgnn2.py:1167-1171: the raw input x [n, F] is added to every head):
- *   forward as b2_gat_combine_fwd_f32 with skip[n, h*F + f] = x[n, f];
- *   backward as b2_gat_combine_bwd_f32, plus dx_skip[n, F] = Σ_h dpre[n, h*F:(h+1)*F] (overwritten). */
-int b2_gat_combine_fwd_identity_f32(const float* agg, int64_t ldagg, const float* x, int64_t ldx, const float* bias,
-                                    int32_t n, int32_t nheads, int32_t F, int concat, int act,
-                                    float* out, int64_t ldo, void* stream);
-int b2_gat_combine_bwd_identity_f32(const float* dout, int64_t lddo, const float* out, int64_t ldo,
-                                    int32_t n, int32_t nheads, int32_t F, int concat, int act,
-                                    float* dpre, int64_t ldp, float* dact, int64_t ldact,
-                                    float* dx_skip, int64_t ldx, void* stream);
+                           float* dpre, int64_t ldp, float* dact, int64_t ldact,
+                           float* dx_skip, int64_t ldx, void* stream);
 
 /* Dropout (scGNN GATLayer, scgnn2.py:1005 / :1010 / :1029: one nn.Dropout(p) at the input, the projection and the
  * attention coefficients).  Keep bits are counter-based, keep(seed, key, r, c) = uniform01(seed, key, r, c) >= p with the
  * hash of CellwiseMaskData: the masks follow torch's distribution (independent Bernoulli(1 - p), kept values scaled by
  * 1 / (1 - p), p = 1 gives zeros) but are not torch's masks.  The backward regenerates them from the same (seed, key).
  *   b2_dropout_f32 : y[r, c] = keep(r, c) ? x[r, c] / (1 - p) : 0 over a strided [rows, cols] matrix; y may be x.
- *   b2_gat_aggregate_fwd_drop_f32 / _bwd_drop_f32 : the aggregate and its backward with α' = drop(α) on (edge, head),
- *     r = the edge's position in the target CSR, c = the head; alpha_out stays the UNDROPPED α, which is what the
- *     backward takes.  nheads <= 32.  drop_p = 0 gives the results of the plain entry points bit for bit.
- *   0 <= p <= 1, otherwise an error. */
+ *   0 <= p <= 1, otherwise an error.  The attention site is the drop_p of b2_gat_aggregate_fwd_f32 / _bwd_f32. */
 int b2_dropout_f32(const float* x, int64_t ldx, int64_t rows, int32_t cols, float p, uint32_t seed, uint32_t key,
                    float* y, int64_t ldy, void* stream);
-int b2_gat_aggregate_fwd_drop_f32(const int32_t* rowptr, const int32_t* colidx,
-                                  const float* H, int64_t ldh, const float* s_src, const float* s_trg,
-                                  int32_t n, int32_t nheads, int32_t F,
-                                  int score_act, float slope, int shift_mode, const float* gmax_dev,
-                                  float* out, int64_t ldo, float* alpha_out,
-                                  float drop_p, uint32_t seed, uint32_t key, void* stream);
-int b2_gat_aggregate_bwd_drop_f32(const int32_t* rowptr, const int32_t* colidx,
-                                  const int32_t* t_rowptr, const int32_t* t_colidx, const int32_t* t_perm,
-                                  const float* H, int64_t ldh, const float* a_src, const float* a_trg,
-                                  const float* s_src, const float* s_trg, const float* alpha,
-                                  const float* dOut, int64_t lddo, int32_t n, int32_t nheads, int32_t F,
-                                  int score_act, float slope, const float* gmax_dev,
-                                  float* dH, int64_t lddh, float* da_src, float* da_trg,
-                                  float* ds_src_ws, float* ds_trg_ws, float* dpre_edge_ws, float* shift_ws,
-                                  float drop_p, uint32_t seed, uint32_t key, void* stream);
 
 /* ------------------------------------------------------------------------
  * NeighborGraph connectivities (transforms/graph/neighbor_graph.py:50-57 → scanpy.pp.neighbors(method="umap") →
@@ -548,20 +517,15 @@ int b2_adj_reparam_bwd_f32(const float* dz, const float* mu, const float* log_st
  * 603-619).  The all-pairs part is partitioned into b2_gae_sym_super_blocks(n) equal-work units (super-block s = the 128-row
  * blocks s and nb-1-s): rank r takes super-blocks [sb_begin, sb_end), plus the label / KLD terms of its own rows
  * [row_begin, row_begin + n_rows).  dz_full [n, d] is zero-filled here and receives this rank's contributions: sum it over
- * ranks (all-reduce); loss_out holds this rank's share of the loss.  d <= 16.  Workspace: b2_gae_loss_workspace_bytes(n, d). */
+ * ranks (all-reduce); loss_out holds this rank's share of the loss.  d <= 16.  Workspace: b2_gae_loss_workspace_bytes(n, d).
+ * Labels (lab_vals NULL: unit; set: real-valued with labt_*) as in b2_gae_loss_grad_f32. */
 int b2_gae_sym_super_blocks(int32_t n);
 int b2_gae_loss_grad_sym_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
-                             const int32_t* lab_rowptr, const int32_t* lab_colidx, int32_t n, int32_t d,
+                             const int32_t* lab_rowptr, const int32_t* lab_colidx, const float* lab_vals,
+                             const int32_t* labt_rowptr, const int32_t* labt_colidx, const float* labt_vals, int32_t n, int32_t d,
                              int32_t sb_begin, int32_t sb_end, int32_t row_begin, int32_t n_rows, float norm, float pos_weight,
                              int use_pos_weight, float* dz_full, float* dmu, float* dlogvar, int64_t ldd, float* loss_out,
                              void* workspace, size_t workspace_bytes, void* stream);
-/* Pair-sharded form with real-valued, asymmetric labels (see b2_gae_loss_grad_weighted_f32). */
-int b2_gae_loss_grad_sym_weighted_f32(const float* z, int64_t ldz, const float* mu, const float* logvar, int64_t ldm,
-                                      const int32_t* lab_rowptr, const int32_t* lab_colidx, const float* lab_vals,
-                                      const int32_t* labt_rowptr, const int32_t* labt_colidx, const float* labt_vals,
-                                      int32_t n, int32_t d, int32_t sb_begin, int32_t sb_end, int32_t row_begin, int32_t n_rows,
-                                      float norm, float pos_weight, int use_pos_weight, float* dz_full, float* dmu, float* dlogvar,
-                                      int64_t ldd, float* loss_out, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------
  * scGNN EM-iteration stages (SURVEY §8f row 3)

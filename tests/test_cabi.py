@@ -33,6 +33,24 @@ def test_python_binding_covers_header():
     assert sorted(_lib.declared_symbols()) == _declared()
 
 
+def test_binding_types_come_from_the_header():
+    """The ctypes signatures are generated from dance_b200.h: spot checks of each mapping, and a type without one raises."""
+    from dance_b200 import _lib
+    sigs = _lib.parse_header((ROOT / "include" / "dance_b200.h").read_text())
+    assert sorted(sigs) == _declared()
+    assert sigs["b2_last_error"] == (ctypes.c_char_p, [])
+    res, args = sigs["b2_radius_graph_count"]
+    assert res is ctypes.c_int and args[4] is ctypes.c_double and args[0] is ctypes.c_void_p
+    args = sigs["b2_dropout_f32"][1]
+    assert args[5] is ctypes.c_uint32 and args[6] is ctypes.c_uint32 and args[4] is ctypes.c_float
+    assert len(sigs["b2_gemm_f32"][1]) == 20 and sigs["b2_gemm_workspace_bytes"][0] is ctypes.c_size_t
+    assert _lib.parse_header("typedef struct s s;\nint b2_f(const s* p, int64_t n, void* stream);") == \
+        {"b2_f": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int64, ctypes.c_void_p])}
+    for bad in ("int b2_f(long n);", "int b2_f(unsigned int n);", "long b2_f(void);", "int b2_f(int);", "struct s { int a; };"):
+        with pytest.raises(_lib.B2Error):
+            _lib.parse_header(bad)
+
+
 def test_error_reporting_without_gpu():
     from dance_b200 import _lib
     lib = _lib.lib()

@@ -553,11 +553,13 @@ def test_gae_launches_per_call(cuda, form, launches, with_mu):
     assert got == launches + with_mu
 
 
+@pytest.mark.parametrize("labels", ["unit", "weighted"])
 @pytest.mark.parametrize("path", ["auto", "tc"])
-def test_gae_loss_no_rows(cuda, path):
-    """The row form with n_rows = 0 (a row shard of no rows, labels [0, n]): nothing to sweep, the loss share is 0 and no row of
-    dz, dmu or dlogvar is written.  Called through the C-ABI, which refuses null pointers: torch gives an empty tensor none, so the
-    row buffers point into a guard buffer that must stay as it is."""
+def test_gae_loss_no_rows(cuda, path, labels):
+    """The row form with n_rows = 0 (a row shard of no rows, labels [0, n]), with unit labels and with label values (plus the
+    transposed labels): nothing to sweep, the loss share is 0 and no row of dz, dmu or dlogvar is written.  Called through the
+    C-ABI, which refuses null pointers: torch gives an empty tensor none, so the row buffers point into a guard buffer that must
+    stay as it is."""
     from dance_b200 import _lib, ops
     n, d, r = 300, 16, 120
     lib = _lib.lib()
@@ -570,8 +572,10 @@ def test_gae_loss_no_rows(cuda, path):
     g = guard.data_ptr()
     ops.set_path("gae", path)
     try:
-        status = lib.b2_gae_loss_grad_f32(z.data_ptr(), d, g, g, d, rowptr.data_ptr(), colidx.data_ptr(), n, d, r, 0, 0.5, 20.0, 1,
-                                          g, g, g, d, loss.data_ptr(), ws.data_ptr(), ws.numel(), ops._stream())
+        lab = [rowptr.data_ptr(), colidx.data_ptr()]
+        lab += [None] * 4 if labels == "unit" else [g, rowptr.data_ptr(), colidx.data_ptr(), g]
+        status = lib.b2_gae_loss_grad_f32(z.data_ptr(), d, g, g, d, *lab, n, d, r, 0, 0.5, 20.0, 1, g, g, g, d, loss.data_ptr(),
+                                          ws.data_ptr(), ws.numel(), ops._stream())
     finally:
         ops.set_path("gae", "auto")
     assert status == 0

@@ -82,7 +82,6 @@ struct Tiles {
   static constexpr uint32_t RING = ZS_PLANES * ZS_BYTES + 2 * ZIT + 4 * GT;
   static constexpr size_t SMEM = RING + STAGES * STAGE + 16 * STAGES + (TRI ? 32 : 0) + 1024;   // + Gᵀ full / empty x 2
 };
-static_assert(Tiles<MAX_D, false>::SMEM <= MAX_SMEM && Tiles<MAX_D, true>::SMEM <= MAX_SMEM, "decoder shared memory");
 
 // position of column jj of a tile in the permuted order of the dZ MMA (see header)
 __host__ __device__ __forceinline__ int zt_pos(int jj) { const int q = jj & 7; return (jj & ~7) | ((q & 1) ? 4 + (q >> 1) : (q >> 1)); }
@@ -614,6 +613,7 @@ static int launch_sweep(const Params& p, int units, cudaStream_t st) {
   if (splits < 1) splits = 1;
   auto kernel = TRI ? gae_tri_tc_kernel<DP> : gae_allpairs_tc_kernel<DP>;
   constexpr size_t smem = Tiles<DP, TRI>::SMEM;
+  static_assert(smem <= MAX_SMEM, "decoder shared memory");
   static bool attr_set = false;
   if (!attr_set) {
     B2_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -17,6 +17,10 @@
 //                          hi / lo planes of Gᵀ (K-major in i, the A operand) and Z_Iᵀ is the B operand.  Both dZ products
 //                          issue their three products as two: hi·hi and hi·lo as one m64n(2·DP)k8 against a B operand laid
 //                          out [hi | lo], and lo·hi.  dZ_J runs on a fourth warpgroup of its own (below).
+//   gae_tri_f16_tc_kernel   the same triangle with both dZ products as fp16 m64nNk16 (half the wgmmas of tf32 k8 at the same
+//                          cost each): G·2^14 and each 64-row tile of z scaled by 2^e_t into fp16's range, split into fp16
+//                          hi / lo; the tile sums are unscaled exactly in fp32.  S is unchanged.  The call over all rows runs
+//                          it; the tf32 triangle stays selectable (B2_PATH_GAE_DECODER mode 6).
 //
 // Schedule: each product is issued as one batch of wgmmas with one commit and one wait, which needs S, both halves of G and
 // the dZ accumulators live in registers at once; the producer warpgroup gives its registers to the consumers (setmaxnreg) to
@@ -38,6 +42,7 @@
 // The J sweep of a unit can be cut into step ranges (grid.y), which then add into dz atomically.
 #include "tc_common.cuh"
 
+#include <cuda_fp16.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -71,14 +76,16 @@ template <int DP> constexpr uint32_t zt_bytes() { return (uint32_t)DP * 4 * 128;
 
 // Shared memory of a sweep.  Full sweep (DP = 32): Z_I 32 KB + 3 x 64 KB stages.  Triangle (DP = 32): Z_I 32 KB, Z_Iᵀ 32 KB,
 // Gᵀ 64 KB, 3 x 32 KB stages; the 64-column J tiles are the halves of a 128-row workspace tile (contiguous in both planes).
-template <int DP, bool TRI>
+// fp16 triangle (F16): a J tile's Z_Jᵀ is one [hi | lo] block of 2·DP rows x 64 fp16; Z_Iᵀ the same per warpgroup; Gᵀ planes
+// of 64 j x 64 fp16.  DP = 32: Z_I 32 KB, Z_Iᵀ 16 KB, Gᵀ 32 KB, 3 x 24 KB stages.
+template <int DP, bool TRI, bool F16 = false>
 struct Tiles {
   static constexpr int JW = TRI ? 64 : BT;                        // J tile width
   static constexpr uint32_t JS = JW * 128;                        // one plane of a J tile for S
-  static constexpr uint32_t JT = zt_bytes<DP>() / (BT / JW);      // one plane of a J tile's Z_Jᵀ
-  static constexpr uint32_t STAGE = ZS_PLANES * JS + 2 * JT;
-  static constexpr uint32_t ZIT = TRI ? zt_bytes<DP>() : 0;       // one plane of Z_Iᵀ
-  static constexpr uint32_t GT = TRI ? 64 * 64 * 4 : 0;           // one plane of a warpgroup's Gᵀ: 64 j x 64 i, 2 atoms
+  static constexpr uint32_t JT = F16 ? 2 * DP * 128 : zt_bytes<DP>() / (BT / JW);   // one plane of a J tile's Z_Jᵀ (F16: both)
+  static constexpr uint32_t STAGE = ZS_PLANES * JS + (F16 ? 1 : 2) * JT;
+  static constexpr uint32_t ZIT = !TRI ? 0 : F16 ? 2 * DP * 128 : zt_bytes<DP>();   // one plane of Z_Iᵀ (F16: one warpgroup's)
+  static constexpr uint32_t GT = !TRI ? 0 : F16 ? 64 * 128 : 64 * 64 * 4;          // one plane of a warpgroup's Gᵀ: 64 j x 64 i
   static constexpr uint32_t RING = ZS_PLANES * ZS_BYTES + 2 * ZIT + 4 * GT;
   static constexpr size_t SMEM = RING + STAGES * STAGE + 16 * STAGES + (TRI ? 32 : 0) + 1024;   // + Gᵀ full / empty x 2
 };
@@ -114,6 +121,53 @@ gae_split_kernel(const float* __restrict__ z, int64_t ldz, int32_t n, int32_t d,
   }
 }
 
+// fp16 triangle: z → the tf32 hi / lo planes for S as above, and per 64-row tile t the fp16 [hi | lo] block of Z_Jᵀ
+// (2·DP rows x 64 j, K-major, 128-byte swizzle) of z·2^e_t, with e_t (exps[t]) chosen from the tile's largest |z| so that the
+// scaled values stay ≤ 2^14: hi = rn(x·2^e), lo = rn(x·2^e − hi), 22 significant bits like the tf32 split.  A zero tile
+// gets e = 0.  One block per 64-row tile.
+template <int DP>
+__global__ void __launch_bounds__(256)
+gae_split_f16_kernel(const float* __restrict__ z, int64_t ldz, int32_t n, int32_t d, uint8_t* __restrict__ zs_hi,
+                     uint8_t* __restrict__ zs_lo, uint8_t* __restrict__ zt, int* __restrict__ exps) {
+  __shared__ float wmax[8];
+  const int64_t row0 = (int64_t)blockIdx.x * 64;
+  auto load = [&](int e) {
+    const int64_t row = row0 + e / DP;
+    const int k = e % DP;
+    return (row < n && k < d) ? z[row * ldz + k] : 0.f;
+  };
+  float m = 0.f;
+  for (int e = threadIdx.x; e < 64 * DP; e += 256) m = fmaxf(m, fabsf(load(e)));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) m = fmaxf(m, wmax[w]);
+  int ex = 0;
+  if (m > 0.f) { int e2; frexpf(m, &e2); ex = min(100, max(-100, 14 - e2)); }   // m < 2^e2
+  if (threadIdx.x == 0) exps[blockIdx.x] = ex;
+  const float sc = ldexpf(1.f, ex);
+  uint8_t* zt_t = zt + (size_t)blockIdx.x * (2 * DP * 128);
+  for (int e = threadIdx.x; e < 64 * DP; e += 256) {
+    const int r = e / DP, k = e % DP;
+    const int64_t row = row0 + r;
+    const float v = load(e);
+    const float h = tf32_trunc(v);
+    const size_t so = (size_t)(row / BT) * ZS_BYTES + sw128_offset32((uint32_t)(row % BT), (uint32_t)k);
+    *reinterpret_cast<float*>(zs_hi + so) = h;
+    *reinterpret_cast<float*>(zs_lo + so) = v - h;
+    const float x = v * sc;
+    const __half xh = __float2half_rn(x);
+    *reinterpret_cast<__half*>(zt_t + sw128_offset16((uint32_t)k, (uint32_t)r)) = xh;
+    *reinterpret_cast<__half*>(zt_t + sw128_offset16((uint32_t)(DP + k), (uint32_t)r)) = __float2half_rn(x - __half2float(xh));
+  }
+}
+
+// 2^(−14−e): undoes the scale of a product of G·2^14 and a tile scaled by 2^e, exactly (e ∈ [−100, 100])
+__device__ __forceinline__ float unscale(int e) { return __int_as_float((127 - 14 - e) << 23); }
+
 struct Params {
   const float* z;
   int64_t ldz;
@@ -125,6 +179,7 @@ struct Params {
   int row_begin, row_end;      // row form: rows [row_begin, row_end), dz row i at dz[(i - row_begin) * d]
   int sb_begin, nb, sym;       // pair-sharded form: grid.x = 2 x super-blocks from sb_begin, dz row i at dz[i * d]
   int n_jt;                    // J tiles
+  const int* exps;             // fp16 triangle: scale exponent of each 64-row tile (zt_hi holds the fp16 blocks)
 };
 
 template <int N>
@@ -143,18 +198,37 @@ __device__ __forceinline__ void mma_ss(float (&d)[N / 2], uint64_t a, uint64_t b
   else wgmma_tf32_ss_n128(d, a, b, scale_d);
 }
 
+template <int N>
+__device__ __forceinline__ void mma_rs16(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
+  if constexpr (N == 8) wgmma_f16_rs_n8(d, a, b, scale_d);
+  else if constexpr (N == 16) wgmma_f16_rs_n16(d, a, b, scale_d);
+  else if constexpr (N == 32) wgmma_f16_rs_n32(d, a, b, scale_d);
+  else wgmma_f16_rs_n64(d, a, b, scale_d);
+}
+template <int N>
+__device__ __forceinline__ void mma_ss16(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
+  if constexpr (N == 8) wgmma_f16_ss_n8(d, a, b, scale_d);
+  else if constexpr (N == 16) wgmma_f16_ss_n16(d, a, b, scale_d);
+  else if constexpr (N == 32) wgmma_f16_ss_n32(d, a, b, scale_d);
+  else wgmma_f16_ss_n64(d, a, b, scale_d);
+}
+
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ void sts_v2(uint32_t addr, float x, float y) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
 }
+__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t x) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(x) : "memory");
+}
 
 // σ and softplus of one thread's logits S (the m64nJW accumulator), in place: S becomes the hi part of G = σ(S) and L its lo
 // part, ready to be the register A operand of the dZ product.  Returns the thread's share of Σ softplus.  MASKED zeroes G and
 // drops the loss of columns j ≥ n and of rows past the range (the last J tile, a partial I block); interior tiles skip the
-// per-logit mask and its selects.
-template <bool MASKED, int V>
+// per-logit mask and its selects.  F16: G·2^14 is split into fp16 hi / lo, packed two columns per register (the f16 A
+// fragment) into S[0 .. V/2) and L[0 .. V/2).
+template <bool MASKED, int V, bool F16 = false>
 __device__ __forceinline__ float sigmoid_softplus(float (&S)[V], float (&L)[V], int jbase, int n, bool live_a, bool live_b) {
   constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
   float relu = 0.f, lg = 0.f, prod = 1.f;
@@ -175,9 +249,23 @@ __device__ __forceinline__ float sigmoid_softplus(float (&S)[V], float (&L)[V], 
       relu += fmaxf(x, 0.f);
       prod *= 1.f + e;
     }
-    const float hi = tf32_trunc(sg);
-    S[v] = hi;
-    L[v] = sg - hi;
+    if constexpr (F16) {
+      S[v] = sg * 16384.f;
+    } else {
+      const float hi = tf32_trunc(sg);
+      S[v] = hi;
+      L[v] = sg - hi;
+    }
+  }
+  if constexpr (F16) {
+#pragma unroll
+    for (int q = 0; q < V / 2; ++q) {
+      const __half2 h = __floats2half2_rn(S[2 * q], S[2 * q + 1]);
+      const float2 hf = __half22float2(h);
+      const __half2 l = __floats2half2_rn(S[2 * q] - hf.x, S[2 * q + 1] - hf.y);
+      S[q] = __uint_as_float(*reinterpret_cast<const uint32_t*>(&h));
+      L[q] = __uint_as_float(*reinterpret_cast<const uint32_t*>(&l));
+    }
   }
   return relu + LN2 * (lg + lg2_approx(prod));
 }
@@ -192,10 +280,11 @@ __device__ __forceinline__ float merged(const float (&acc)[NBM][DP], const float
   return t;
 }
 
-// The sweep of one work unit; TRI selects the triangle (see header).
-template <int DP, bool TRI>
+// The sweep of one work unit; TRI selects the triangle, F16 its fp16 gradient products (see header).
+template <int DP, bool TRI, bool F16 = false>
 __device__ __forceinline__ void decoder_sweep(const Params& p) {
-  using T = Tiles<DP, TRI>;
+  static_assert(TRI || !F16, "fp16 gradient products are a triangle variant");
+  using T = Tiles<DP, TRI, F16>;
   constexpr int JW = T::JW;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -253,17 +342,38 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
       asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TriRegs<DP>::DJ));
       if (handed0 >= nt) return;
       const int t = tid - THREADS, warp = t >> 5, lane = t & 31;
-      // Z_Iᵀ (B of dZ_J), per consumer warpgroup 2 atoms of [DP hi rows | DP lo rows] x 32 i in the gt_pos order; rows past the
-      // range are zero
-      for (int e = t; e < BT * DP; e += 128) {
-        const int r = e / DP, k = e % DP;
-        const int row = row0 + r;
-        const float v = (row < row_end && k < p.d) ? p.z[(int64_t)row * p.ldz + k] : 0.f;
-        const float h = tf32_trunc(v);
-        const int q = gt_pos(r & 63);
-        const uint32_t ot = (uint32_t)(r >> 6) * (4 * ATOM) + (uint32_t)(q >> 5) * (2 * ATOM) + sw128_offset32((uint32_t)k, (uint32_t)(q & 31));
-        *reinterpret_cast<float*>(zit + ot) = h;
-        *reinterpret_cast<float*>(zit + ot + ATOM) = v - h;
+      // F16: each warpgroup half of Z_I in its 64-row tile's scale; the half's sum is unscaled before the two are added
+      float sc_i[2] = {1.f, 1.f};
+      if constexpr (F16) {
+        const int e0 = p.exps[2 * blockIdx.x], e1 = p.exps[2 * blockIdx.x + 1];
+        sc_i[0] = unscale(e0);
+        sc_i[1] = unscale(e1);
+        // Z_Iᵀ per consumer warpgroup: [DP hi rows | DP lo rows] x 64 i (fp16) in the gt_pos order, scaled by 2^e; rows past
+        // the range are zero
+        for (int e = t; e < BT * DP; e += 128) {
+          const int r = e / DP, k = e % DP;
+          const int row = row0 + r;
+          const float v = (row < row_end && k < p.d) ? p.z[(int64_t)row * p.ldz + k] : 0.f;
+          const float x = ldexpf(v, (r >> 6) ? e1 : e0);
+          const __half xh = __float2half_rn(x);
+          const uint32_t q = (uint32_t)gt_pos(r & 63);
+          uint8_t* b = zit + (r >> 6) * T::ZIT;
+          *reinterpret_cast<__half*>(b + sw128_offset16((uint32_t)k, q)) = xh;
+          *reinterpret_cast<__half*>(b + sw128_offset16((uint32_t)(DP + k), q)) = __float2half_rn(x - __half2float(xh));
+        }
+      } else {
+        // Z_Iᵀ (B of dZ_J), per consumer warpgroup 2 atoms of [DP hi rows | DP lo rows] x 32 i in the gt_pos order; rows past
+        // the range are zero
+        for (int e = t; e < BT * DP; e += 128) {
+          const int r = e / DP, k = e % DP;
+          const int row = row0 + r;
+          const float v = (row < row_end && k < p.d) ? p.z[(int64_t)row * p.ldz + k] : 0.f;
+          const float h = tf32_trunc(v);
+          const int q = gt_pos(r & 63);
+          const uint32_t ot = (uint32_t)(r >> 6) * (4 * ATOM) + (uint32_t)(q >> 5) * (2 * ATOM) + sw128_offset32((uint32_t)k, (uint32_t)(q & 31));
+          *reinterpret_cast<float*>(zit + ot) = h;
+          *reinterpret_cast<float*>(zit + ot + ATOM) = v - h;
+        }
       }
       fence_proxy_async();
       asm volatile("bar.sync 4, 128;" ::: "memory");
@@ -276,14 +386,23 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
         for (int h = 0; h < 2; ++h) {
           mbar_wait(gt_full + 8 * h, parity);
           const uint32_t ag_hi = smem_u32(zit + 2 * T::ZIT + h * 2 * T::GT), ag_lo = ag_hi + T::GT;
-          const uint32_t bi = smem_u32(zit) + h * (4 * ATOM);
+          const uint32_t bi = smem_u32(zit) + h * (F16 ? T::ZIT : 4 * ATOM);
           wgmma_fence();
+          if constexpr (F16) {
 #pragma unroll
-          for (int kk = 0; kk < 64 / 8; ++kk) {
-            const uint32_t oa = (uint32_t)(kk >> 2) * (64 * 128) + (uint32_t)(kk & 3) * 32;
-            const uint32_t ob = (uint32_t)(kk >> 2) * (2 * ATOM) + (uint32_t)(kk & 3) * 32;
-            mma_ss<DP>(djs, wgmma_desc_sw128(ag_lo + oa), wgmma_desc_sw128(bi + ob), kk > 0);
-            mma_ss<2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + oa), wgmma_desc_sw128(bi + ob), kk >= NBM);
+            for (int kk = 0; kk < 64 / 16; ++kk) {
+              const uint32_t o = (uint32_t)kk * 32;
+              mma_ss16<DP>(djs, wgmma_desc_sw128(ag_lo + o), wgmma_desc_sw128(bi + o), kk > 0);
+              mma_ss16<2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + o), wgmma_desc_sw128(bi + o), kk >= NBM);
+            }
+          } else {
+#pragma unroll
+            for (int kk = 0; kk < 64 / 8; ++kk) {
+              const uint32_t oa = (uint32_t)(kk >> 2) * (64 * 128) + (uint32_t)(kk & 3) * 32;
+              const uint32_t ob = (uint32_t)(kk >> 2) * (2 * ATOM) + (uint32_t)(kk & 3) * 32;
+              mma_ss<DP>(djs, wgmma_desc_sw128(ag_lo + oa), wgmma_desc_sw128(bi + ob), kk > 0);
+              mma_ss<2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + oa), wgmma_desc_sw128(bi + ob), kk >= NBM);
+            }
           }
           wgmma_commit();
           wgmma_wait<0>();
@@ -293,7 +412,10 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
           __syncwarp();
           if (lane == 0) mbar_arrive(gt_empty + 8 * h);     // this warpgroup's Gᵀ is read
 #pragma unroll
-          for (int v = 0; v < DP / 2; ++v) djt[v] = (h ? djt[v] : 0.f) + merged(djm, djs, v);
+          for (int v = 0; v < DP / 2; ++v) {
+            if constexpr (F16) djt[v] = (h ? djt[v] : 0.f) + merged(djm, djs, v) * sc_i[h];
+            else djt[v] = (h ? djt[v] : 0.f) + merged(djm, djs, v);
+          }
         }
         const int ja = (jt0 + i) * JW + warp * 16 + (lane >> 2);
 #pragma unroll
@@ -327,7 +449,9 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
         mbar_expect_tx(fb, T::STAGE);
         bulk_load(dst, p.zs_hi + t * T::JS, T::JS, fb);
         bulk_load(dst + T::JS, p.zs_lo + t * T::JS, T::JS, fb);
-        if constexpr (TRI) {
+        if constexpr (F16) {
+          bulk_load(dst + 2 * T::JS, p.zt_hi + t * T::JT, T::JT, fb);   // [hi | lo], as the split kernel wrote it
+        } else if constexpr (TRI) {
           // atom by atom, lo after hi: the B operand [Z_Jᵀ hi | Z_Jᵀ lo] of the merged dZ_I products
           for (uint32_t a = 0; a < T::JT / ATOM; ++a) {
             bulk_load(dst + 2 * T::JS + 2 * a * ATOM, p.zt_hi + t * T::JT + a * ATOM, ATOM, fb);
@@ -419,22 +543,35 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   auto issue_dz = [&](int i, float (&S)[JW / 2]) {
     const uint32_t bt_hi = smem_u32(ring + (i % STAGES) * T::STAGE) + 2 * T::JS, bt_lo = bt_hi + T::JT;
     wgmma_fence();
+    if constexpr (F16) {
+      // A = G·2^14 as packed fp16 (sigmoid_softplus), in the natural column order; B = [Z_Jᵀ hi | Z_Jᵀ lo] rows, K = j
 #pragma unroll
-    for (int kb = 0; kb < JW / 8; ++kb) {
-      // A fragment (r, t) (r+8, t) (r, t+4) (r+8, t+4) in the permuted column order: (r, 2t) (r+8, 2t) (r, 2t+1) (r+8, 2t+1)
-      const uint32_t ahi[4] = {__float_as_uint(S[4 * kb]), __float_as_uint(S[4 * kb + 2]), __float_as_uint(S[4 * kb + 1]),
-                               __float_as_uint(S[4 * kb + 3])};
-      const uint32_t alo[4] = {__float_as_uint(L[4 * kb]), __float_as_uint(L[4 * kb + 2]), __float_as_uint(L[4 * kb + 1]),
-                               __float_as_uint(L[4 * kb + 3])};
-      if constexpr (TRI) {
-        const uint32_t o = (uint32_t)(kb >> 2) * (2 * ATOM) + (uint32_t)(kb & 3) * 32;   // atom [hi | lo]
-        mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
-        mma_rs<2 * DP>(dzm[kb % NBM], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NBM);
-      } else {
-        const uint32_t o = (uint32_t)(kb >> 2) * ATOM + (uint32_t)(kb & 3) * 32;
-        mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
-        mma_rs<DP>(dzs, ahi, wgmma_desc_sw128(bt_lo + o), 1);
-        mma_rs<DP>(dzb[kb % NB], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NB);
+      for (int kb = 0; kb < JW / 16; ++kb) {
+        const uint32_t ahi[4] = {__float_as_uint(S[4 * kb]), __float_as_uint(S[4 * kb + 1]), __float_as_uint(S[4 * kb + 2]),
+                                 __float_as_uint(S[4 * kb + 3])};
+        const uint32_t alo[4] = {__float_as_uint(L[4 * kb]), __float_as_uint(L[4 * kb + 1]), __float_as_uint(L[4 * kb + 2]),
+                                 __float_as_uint(L[4 * kb + 3])};
+        mma_rs16<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + kb * 32), kb > 0);
+        mma_rs16<2 * DP>(dzm[kb % NBM], ahi, wgmma_desc_sw128(bt_hi + kb * 32), kb >= NBM);
+      }
+    } else {
+#pragma unroll
+      for (int kb = 0; kb < JW / 8; ++kb) {
+        // A fragment (r, t) (r+8, t) (r, t+4) (r+8, t+4) in the permuted column order: (r, 2t) (r+8, 2t) (r, 2t+1) (r+8, 2t+1)
+        const uint32_t ahi[4] = {__float_as_uint(S[4 * kb]), __float_as_uint(S[4 * kb + 2]), __float_as_uint(S[4 * kb + 1]),
+                                 __float_as_uint(S[4 * kb + 3])};
+        const uint32_t alo[4] = {__float_as_uint(L[4 * kb]), __float_as_uint(L[4 * kb + 2]), __float_as_uint(L[4 * kb + 1]),
+                                 __float_as_uint(L[4 * kb + 3])};
+        if constexpr (TRI) {
+          const uint32_t o = (uint32_t)(kb >> 2) * (2 * ATOM) + (uint32_t)(kb & 3) * 32;   // atom [hi | lo]
+          mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
+          mma_rs<2 * DP>(dzm[kb % NBM], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NBM);
+        } else {
+          const uint32_t o = (uint32_t)(kb >> 2) * ATOM + (uint32_t)(kb & 3) * 32;
+          mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
+          mma_rs<DP>(dzs, ahi, wgmma_desc_sw128(bt_lo + o), 1);
+          mma_rs<DP>(dzb[kb % NB], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NB);
+        }
       }
     }
     wgmma_commit();
@@ -450,10 +587,12 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
     }
   };
   // the tile's dZ_I joins the fp32 total and its stage goes back to the producer
-  auto retire_dz = [&](int i) {
+  auto retire_dz = [&](int i, float sc) {
 #pragma unroll
     for (int v = 0; v < DP / 2; ++v) {
-      if constexpr (TRI) {
+      if constexpr (F16) {
+        dzt[v] += merged(dzm, dzs, v) * sc;
+      } else if constexpr (TRI) {
         dzt[v] += merged(dzm, dzs, v);
       } else {
         float t = dzs[v];
@@ -469,14 +608,33 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   // dZ_J warpgroup, once that warpgroup has read the previous one
   auto elementwise = [&](int i, float (&S)[JW / 2]) {
     const int jbase = (jt0 + i) * JW + 2 * (lane & 3);
-    const float l = full_rows && (jt0 + i + 1) * JW <= p.n ? sigmoid_softplus<false>(S, L, jbase, p.n, live_a, live_b)
-                                                           : sigmoid_softplus<true>(S, L, jbase, p.n, live_a, live_b);
+    const float l = full_rows && (jt0 + i + 1) * JW <= p.n ? sigmoid_softplus<false, JW / 2, F16>(S, L, jbase, p.n, live_a, live_b)
+                                                           : sigmoid_softplus<true, JW / 2, F16>(S, L, jbase, p.n, live_a, live_b);
     if constexpr (TRI) {
       if (i >= handed0) {
         loss += 2.0 * (double)l;   // a tile above the diagonal block stands for its mirror too
         mbar_wait(gt_empty + 8 * wg, (uint32_t)(((i - handed0) & 1) ^ 1));
         // column jj of G is row jj of Gᵀ; the thread's rows r, r + 8 sit at K positions gt_pos(r), gt_pos(r) + 1
         const uint32_t k = (uint32_t)gt_pos(warp * 16 + (lane >> 2));
+        if constexpr (F16) {
+          // one 32-bit store per column and plane: (r, j) and (r + 8, j) from the two registers that hold column j
+#pragma unroll
+          for (int c = 0; c < JW / 8; ++c) {
+            const uint32_t h0 = __float_as_uint(S[2 * c]), h1 = __float_as_uint(S[2 * c + 1]);
+            const uint32_t l0 = __float_as_uint(L[2 * c]), l1 = __float_as_uint(L[2 * c + 1]);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const uint32_t sel = e ? 0x7632u : 0x5410u;
+              const uint32_t o = sw128_offset16((uint32_t)(8 * c + 2 * (lane & 3) + e), k);
+              sts_u32(smem_u32(gt_hi) + o, __byte_perm(h0, h1, sel));
+              sts_u32(smem_u32(gt_lo) + o, __byte_perm(l0, l1, sel));
+            }
+          }
+          fence_proxy_async();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(gt_full + 8 * wg);
+          return;
+        }
         const uint32_t base = (k >> 5) * (64 * 128);
 #pragma unroll
         for (int c = 0; c < JW / 8; ++c) {
@@ -501,14 +659,17 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   if constexpr (OVERLAP) {
     float S2[JW / 2];
     // the turn of tile i ≥ 1: dZ of tile i − 1 from (Sp, L), then S of tile i into Sn
+    // F16: the scale of tile i − 1 is loaded before the waits
+    auto tile_unscale = [&](int i) { return F16 ? unscale(__ldg(p.exps + jt0 + i)) : 1.f; };
     auto turn = [&](int i, float (&Sp)[JW / 2], float (&Sn)[JW / 2]) {
       take_turn();
       issue_dz(i - 1, Sp);
       issue_s(i, Sn);
       pass_turn();
+      const float sc = tile_unscale(i - 1);
       wgmma_wait<1>();     // dZ is done, S may still run
       dz_fence();
-      retire_dz(i - 1);
+      retire_dz(i - 1, sc);
       wgmma_wait<0>();
       reg_fence(Sn);
       elementwise(i, Sn);
@@ -518,9 +679,10 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
       take_turn();
       issue_dz(nt - 1, Sp);
       if (wg == 0) pass_turn();
+      const float sc = tile_unscale(nt - 1);
       wgmma_wait<0>();
       dz_fence();
-      retire_dz(nt - 1);
+      retire_dz(nt - 1, sc);
     };
     if (wg == 1) take_turn();
     issue_s(0, S);
@@ -556,12 +718,12 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
       take_turn();
       run_dz(i - 1);
       issue_s(i, S);       // S runs while the previous tile's dZ is summed
-      retire_dz(i - 1);
+      retire_dz(i - 1, 1.f);
       finish_s(i);
     }
     take_turn();
     run_dz(nt - 1);
-    retire_dz(nt - 1);
+    retire_dz(nt - 1, 1.f);
     if (wg == 0) pass_turn();
   }
 
@@ -594,25 +756,31 @@ gae_tri_tc_kernel(const __grid_constant__ Params p) {
   decoder_sweep<DP, true>(p);
 }
 
+template <int DP>
+__global__ void __launch_bounds__(TRI_THREADS, 1)
+gae_tri_f16_tc_kernel(const __grid_constant__ Params p) {
+  decoder_sweep<DP, true, true>(p);
+}
+
 size_t workspace_bytes(int32_t n) { return (size_t)padded_n(n) / BT * (ZS_PLANES * ZS_BYTES + 2 * zt_bytes<MAX_D>()); }
 
 int super_blocks(int32_t n) { return (int)((padded_n(n) / BT + 1) / 2); }
 
 bool eligible(int32_t n, int32_t d, int32_t n_rows, size_t ws_bytes) {
-  const int mode = path_mode(B2_PATH_GAE_DECODER);           // 0 auto · 1 CUDA cores · 2 this kernel
+  const int mode = path_mode(B2_PATH_GAE_DECODER);           // 0 auto · 1 CUDA cores · 2 these kernels · 6 with the tf32 triangle
   if (d < 1 || d > MAX_D || mode == 1 || ws_bytes < workspace_bytes(n)) return false;
-  return mode == 2 || (int64_t)n * n_rows >= (1ll << 22);
+  return mode == 2 || mode == 6 || (int64_t)n * n_rows >= (1ll << 22);
 }
 
-template <int DP, bool TRI>
+template <int DP, bool TRI, bool F16 = false>
 static int launch_sweep(const Params& p, int units, cudaStream_t st) {
   // J step ranges: b2_set_tuning(B2_TUNE_GAE_SPLITS) when set, else enough to fill one wave of SMs
   int splits = tuning(B2_TUNE_GAE_SPLITS);
   if (splits <= 0) splits = ceil_div(sm_count(), units);
   if (splits > p.n_jt) splits = p.n_jt;
   if (splits < 1) splits = 1;
-  auto kernel = TRI ? gae_tri_tc_kernel<DP> : gae_allpairs_tc_kernel<DP>;
-  constexpr size_t smem = Tiles<DP, TRI>::SMEM;
+  auto kernel = F16 ? gae_tri_f16_tc_kernel<DP> : TRI ? gae_tri_tc_kernel<DP> : gae_allpairs_tc_kernel<DP>;
+  constexpr size_t smem = Tiles<DP, TRI, F16>::SMEM;
   static_assert(smem <= MAX_SMEM, "decoder shared memory");
   static bool attr_set = false;
   if (!attr_set) {
@@ -620,12 +788,12 @@ static int launch_sweep(const Params& p, int units, cudaStream_t st) {
     attr_set = true;
   }
   kernel<<<dim3((unsigned)units, (unsigned)splits), TRI ? TRI_THREADS : THREADS, smem, st>>>(p);
-  B2_CHECK_LAUNCH(TRI ? "gae_tri_tc_kernel" : "gae_allpairs_tc_kernel");
+  B2_CHECK_LAUNCH(F16 ? "gae_tri_f16_tc_kernel" : TRI ? "gae_tri_tc_kernel" : "gae_allpairs_tc_kernel");
   return B2_OK;
 }
 
 // Splits z into the workspace planes, then sweeps `units` work units (none: the split only).  tri: every row against every
-// column by the triangle (units must be the nb row blocks).
+// column by the triangle (units must be the nb row blocks), with fp16 gradient products unless tf32 is asked for.
 template <int DP>
 static int launch_dp(Params p, int units, bool tri, void* ws, cudaStream_t st) {
   const int64_t npad = padded_n(p.n);
@@ -633,6 +801,16 @@ static int launch_dp(Params p, int units, bool tri, void* ws, cudaStream_t st) {
   uint8_t* zs_hi = reinterpret_cast<uint8_t*>(ws);
   uint8_t* zs_lo = zs_hi + (size_t)p.nb * ZS_BYTES;
   uint8_t* zt_hi = zs_lo + (size_t)p.nb * ZS_BYTES;
+  if (tri && units > 0 && path_mode(B2_PATH_GAE_DECODER) != 6) {
+    // the fp16 Z_Jᵀ blocks (2·nb of 2·DP·128 bytes) and the tile exponents take the place of the tf32 Z_Jᵀ planes
+    static_assert(2 * 2 * DP * 128 + 2 * sizeof(int) <= 2 * zt_bytes<MAX_D>(), "fp16 triangle workspace");
+    int* exps = reinterpret_cast<int*>(zt_hi + (size_t)(2 * p.nb) * (2 * DP * 128));
+    gae_split_f16_kernel<DP><<<(unsigned)(2 * p.nb), 256, 0, st>>>(p.z, p.ldz, p.n, p.d, zs_hi, zs_lo, zt_hi, exps);
+    B2_CHECK_LAUNCH("gae_split_f16_kernel");
+    p.zs_hi = zs_hi; p.zs_lo = zs_lo; p.zt_hi = zt_hi; p.exps = exps;
+    p.n_jt = ceil_div(p.n, Tiles<DP, true, true>::JW);
+    return launch_sweep<DP, true, true>(p, units, st);
+  }
   uint8_t* zt_lo = zt_hi + (size_t)p.nb * zt_bytes<DP>();
   int64_t blocks = ceil_div<int64_t>(npad * DP, 256);
   const int64_t cap = (int64_t)sm_count() * 16;

@@ -2,19 +2,17 @@
 
 CUDA events around each call after a warm-up; prints one JSON line per d and kernel with the median and minimum time, the
 ordered pairs per second (n², what the loss covers) and the logits the kernel evaluates per second with their fraction of the
-SFU floor and of the tensor-instruction floor.  Three kernels run on the same z:
-  "triangle"    the call over all rows (gae_tri_f16_tc_kernel): each block sweeps the 64-column J tiles from its own 128-row
+SFU floor (and, for the triangle, of the tensor-instruction floor).  Two kernels run on the same z:
+  "triangle"    the call over all rows (gae_tri_tc_kernel): each block sweeps the 64-column J tiles from its own 128-row
                 block on, so it evaluates about n²/2 logits plus the diagonal blocks; S in tf32, the gradient products in fp16;
-  "triangle_tf32"  the same sweep with every product in tf32 (gae_tri_tc_kernel, ops.set_path("gae", "tc_tf32"));
   "full_sweep"  the same rows as two row-shard calls (gae_allpairs_tc_kernel): every row against every column, n² logits
                 (rounded up to whole 128-column tiles).
 The SFU floor: the triangle issues 32 ex2 + 32 rcp + 2 lg2 per 32 logits, the full sweep 64 + 64 + 3 per 64, and an SM
 completes 16 MUFU results per clock, so neither can exceed 16 / (MUFU per logit) logits per clock per SM at the card's reported
 maximum SM clock.  The tensor-instruction floor: per 128 x 64 triangle tile (8 192 logits) the two consumer warpgroups issue
-2 x 3·DP/8 S products m64n64k8 (32 clocks each), 2 x 4 dZ_I products m64n(2·DP)k16 + m64nDPk16 (fp16; tf32: 2 x 8 of the k8
-ones) and the dZ_J warpgroup 2 x the same from shared memory; the clocks per instruction are those benchmarks/wgmma_rate.py
-measured at two warpgroups (RS: 13 / 16 / 32 clocks at N = 16 / 32 / 64, SS: 20 / 24 / 32, N = 8 taken as N = 16; tf32 k8
-and fp16 k16 alike).  The card name, its power limit and that clock are printed with the numbers."""
+2 x 3·DP/8 S products m64n64k8 (32 clocks each), 2 x 4 dZ_I products m64n(2·DP)k16 + m64nDPk16 and the dZ_J warpgroup
+2 x the same from shared memory; the clocks per instruction are those benchmarks/wgmma_rate.py measured at two warpgroups
+(RS: 13 / 16 / 32 clocks at N = 16 / 32 / 64, SS: 20 / 24 / 32, N = 8 taken as N = 16).  The card name, its power limit and that clock are printed with the numbers."""
 from __future__ import annotations
 
 import argparse
@@ -29,15 +27,15 @@ import torch
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 from dance_b200 import ops  # noqa: E402
 
-MUFU_PER_LOGIT = {"triangle": (32 + 32 + 2) / 32, "triangle_tf32": (32 + 32 + 2) / 32, "full_sweep": (64 + 64 + 3) / 64}
+MUFU_PER_LOGIT = {"triangle": (32 + 32 + 2) / 32, "full_sweep": (64 + 64 + 3) / 64}
 MUFU_PER_CLK_SM = 16
 RS_CLK = {8: 13, 16: 13, 32: 16, 64: 32}
 SS_CLK = {8: 20, 16: 20, 32: 24, 64: 32}
 
 
-def tensor_clocks_per_tile(dp: int, kernel: str) -> int:
+def tensor_clocks_per_tile(dp: int) -> int:
     """tensor-pipe clocks of one 128 x 64 triangle tile above the diagonal block (see the module docstring)"""
-    k = 4 if kernel == "triangle" else 8          # k-steps over 64 columns: fp16 k16 or tf32 k8
+    k = 4                                          # fp16 k16 steps over 64 columns
     s = 2 * (3 * dp // 8) * 32
     dzi = 2 * k * (RS_CLK[2 * dp] + RS_CLK[dp])
     dzj = 2 * k * (SS_CLK[2 * dp] + SS_CLK[dp])
@@ -102,16 +100,8 @@ def main():
     try:
         for d in (int(x) for x in args.d.split(",")):
             z = (torch.randn(n, d, device=dev, generator=gen) * 0.3).contiguous()
-            def tf32_triangle():
-                ops.set_path("gae", "tc_tf32")
-                try:
-                    return ops.gae_loss_grad(z, L, 0.5, 50.0)[0]
-                finally:
-                    ops.set_path("gae", "tc")
-
             runs = {
                 "triangle": lambda: ops.gae_loss_grad(z, L, 0.5, 50.0)[0],
-                "triangle_tf32": tf32_triangle,
                 "full_sweep": lambda: ops.gae_loss_grad(z, top, 0.5, 50.0, row_begin=0, n_rows=h)[0]
                 + ops.gae_loss_grad(z, bot, 0.5, 50.0, row_begin=h, n_rows=n - h)[0],
             }
@@ -122,9 +112,9 @@ def main():
                 row = {"kernel": kernel, "n": n, "d": d, "ms": round(ms, 2), "ms_min": round(min(ts), 2),
                        "pairs_per_s": float(n) * n / (ms * 1e-3), "evaluated_logits_per_s": evaluated,
                        "sfu_floor_fraction": round(evaluated / floor[kernel], 3), "loss": float(loss.item())}
-                if kernel != "full_sweep":
+                if kernel == "triangle":
                     dp = 8 if d <= 8 else 16 if d <= 16 else 32
-                    tensor_floor = sms * info["max_sm_clock_mhz"] * 1e6 * 8192 / tensor_clocks_per_tile(dp, kernel)
+                    tensor_floor = sms * info["max_sm_clock_mhz"] * 1e6 * 8192 / tensor_clocks_per_tile(dp)
                     row["tensor_floor_fraction"] = round(evaluated / tensor_floor, 3)
                 print(json.dumps(row))
     finally:

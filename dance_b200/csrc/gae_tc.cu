@@ -4,23 +4,23 @@
 //   S  = Z_I · Z_Jᵀ        wgmma m64nJWk8 tf32, 3-product split (Z pre-split into hi = x & 0xFFFFE000 and lo = x − hi,
 //                          lo·hi + hi·lo + hi·hi), fp32 accumulators in registers
 //   G  = σ(S), loss       SFU math on the accumulator registers (e = 2^(−|x|·log2e), r = 1/(1+e), one lg2 per 32 logits)
-//   dZ_I += G · Z_J       wgmma m64nDk8 tf32 with A = G taken straight from the registers (hi / lo split of G and Z_J, three
-//                          products) and B = Z_Jᵀ from shared memory
+//   dZ_I += G · Z_J       wgmma with A = G taken straight from the registers (split into hi / lo, three products) and
+//                          B = Z_Jᵀ from shared memory
 // A producer warpgroup (one thread of it) copies the pre-split J tiles into a three-stage ring with 1-D bulk copies (the tiles
 // are laid out in global memory exactly as wgmma reads them: K-major, 128-byte swizzle).
 //
 // Two kernels share that sweep:
 //   gae_allpairs_tc_kernel  J tiles of 128 columns over every column: row subsets (row shards) and the pair-sharded form.
+//                          dZ_I in tf32 m64nDPk8: the hi / lo split of G and of Z_J, lo·hi + hi·lo + hi·hi.
 //   gae_tri_tc_kernel       the full-row call.  S is symmetric, so block I only sweeps J ≥ I in tiles of 64 columns.  The
 //                          128 x 128 diagonal block is evaluated as in the full sweep (it holds both orders of each pair); every
 //                          tile above it counts its loss twice and also yields dZ_J += Gᵀ · Z_I: G goes to shared memory as
-//                          hi / lo planes of Gᵀ (K-major in i, the A operand) and Z_Iᵀ is the B operand.  Both dZ products
-//                          issue their three products as two: hi·hi and hi·lo as one m64n(2·DP)k8 against a B operand laid
-//                          out [hi | lo], and lo·hi.  dZ_J runs on a fourth warpgroup of its own (below).
-//   gae_tri_f16_tc_kernel   the same triangle with both dZ products as fp16 m64nNk16 (half the wgmmas of tf32 k8 at the same
-//                          cost each): G·2^14 and each 64-row tile of z scaled by 2^e_t into fp16's range, split into fp16
-//                          hi / lo; the tile sums are unscaled exactly in fp32.  S is unchanged.  The call over all rows runs
-//                          it; the tf32 triangle stays selectable (B2_PATH_GAE_DECODER mode 6).
+//                          hi / lo planes of Gᵀ (K-major in i, the A operand) and Z_Iᵀ is the B operand.  Both dZ products run
+//                          in fp16 m64nNk16 (half the wgmmas of tf32 k8 at the same cost each): G·2^14 and each 64-row tile of
+//                          z scaled by 2^e_t into fp16's range, split into fp16 hi / lo (22 significant bits like the tf32
+//                          split); the tile sums are unscaled exactly in fp32.  Each issues its three products as two: hi·hi
+//                          and hi·lo as one m64n(2·DP)k16 against a B operand laid out [hi | lo], and lo·hi.  dZ_J runs on a
+//                          fourth warpgroup of its own (below).
 //
 // Schedule: each product is issued as one batch of wgmmas with one commit and one wait, which needs S, both halves of G and
 // the dZ accumulators live in registers at once; the producer warpgroup gives its registers to the consumers (setmaxnreg) to
@@ -30,11 +30,12 @@
 // mbarrier pair (Gᵀ full / Gᵀ empty), issues both halves of a tile's dZ_J (K = warpgroup 0's rows, then warpgroup 1's) into
 // the same accumulators in turn, adds the halves in fp32 and sends the tile's sum to dz with one set of red.global.add.
 //
-// Register fragment trick: the accumulator of S gives a thread columns (2t, 2t+1) of each 8-column block, the tf32 A fragment
-// wants columns (t, t+4).  The sum over j does not care about order, so the 8 columns of each block are fed to the second
-// MMA in the order (0, 2, 4, 6, 1, 3, 5, 7) and Z_Jᵀ is stored with its columns permuted the same way.  Likewise the sum over i
-// of dZ_J: rows r and r + 8 of a thread's fragment are put side by side in the K order of Gᵀ and Z_Iᵀ (gt_pos), so that each
-// thread writes its two Gᵀ values of a column with one 64-bit store.
+// Register fragments: the accumulator of S gives a thread columns (2t, 2t+1) of each 8-column block.  That is the triangle's
+// fp16 A fragment (two columns packed per register), so its dZ_I takes G in the natural column order.  The full sweep's tf32
+// A fragment wants columns (t, t+4); the sum over j does not care about order, so the 8 columns of each block are fed to its
+// dZ MMA in the order (0, 2, 4, 6, 1, 3, 5, 7) and Z_Jᵀ is stored with its columns permuted the same way (zt_pos).  The
+// triangle's dZ_J reorders the sum over i likewise: rows r and r + 8 of a thread's fragment are put side by side in the K
+// order of Gᵀ and Z_Iᵀ (gt_pos), so that each thread writes its two Gᵀ values of a column with one 32-bit store per plane.
 //
 // Work units: row blocks.  The row form covers [row_begin, row_begin + n_rows); the pair-sharded form (multi-GPU) takes
 // "super-blocks" s = {block s, block nb−1−s} (a lone middle block when nb is odd), so that super-block ranges split the work
@@ -74,18 +75,18 @@ constexpr size_t MAX_SMEM = 227 * 1024; // dynamic shared memory a CTA may have 
 static int64_t padded_n(int32_t n) { return ((int64_t)n + BT - 1) / BT * BT; }
 template <int DP> constexpr uint32_t zt_bytes() { return (uint32_t)DP * 4 * 128; }   // one plane of Z_Jᵀ: 4 atoms of DP x 128 B
 
-// Shared memory of a sweep.  Full sweep (DP = 32): Z_I 32 KB + 3 x 64 KB stages.  Triangle (DP = 32): Z_I 32 KB, Z_Iᵀ 32 KB,
-// Gᵀ 64 KB, 3 x 32 KB stages; the 64-column J tiles are the halves of a 128-row workspace tile (contiguous in both planes).
-// fp16 triangle (F16): a J tile's Z_Jᵀ is one [hi | lo] block of 2·DP rows x 64 fp16; Z_Iᵀ the same per warpgroup; Gᵀ planes
-// of 64 j x 64 fp16.  DP = 32: Z_I 32 KB, Z_Iᵀ 16 KB, Gᵀ 32 KB, 3 x 24 KB stages.
-template <int DP, bool TRI, bool F16 = false>
+// Shared memory of a sweep.  Full sweep (DP = 32): Z_I 32 KB + 3 x 64 KB stages.  Triangle: a J tile's Z_Jᵀ is one fp16
+// [hi | lo] block of 2·DP rows x 64 j, Z_Iᵀ the same per warpgroup, Gᵀ planes of 64 j x 64 i fp16; the 64-column J tiles of S
+// are the halves of a 128-row workspace tile (contiguous in both planes).  DP = 32: Z_I 32 KB, Z_Iᵀ 16 KB, Gᵀ 32 KB,
+// 3 x 24 KB stages.
+template <int DP, bool TRI>
 struct Tiles {
   static constexpr int JW = TRI ? 64 : BT;                        // J tile width
   static constexpr uint32_t JS = JW * 128;                        // one plane of a J tile for S
-  static constexpr uint32_t JT = F16 ? 2 * DP * 128 : zt_bytes<DP>() / (BT / JW);   // one plane of a J tile's Z_Jᵀ (F16: both)
-  static constexpr uint32_t STAGE = ZS_PLANES * JS + (F16 ? 1 : 2) * JT;
-  static constexpr uint32_t ZIT = !TRI ? 0 : F16 ? 2 * DP * 128 : zt_bytes<DP>();   // one plane of Z_Iᵀ (F16: one warpgroup's)
-  static constexpr uint32_t GT = !TRI ? 0 : F16 ? 64 * 128 : 64 * 64 * 4;          // one plane of a warpgroup's Gᵀ: 64 j x 64 i
+  static constexpr uint32_t JT = TRI ? 2 * DP * 128 : zt_bytes<DP>();   // a J tile's Z_Jᵀ: one plane (triangle: [hi | lo])
+  static constexpr uint32_t STAGE = ZS_PLANES * JS + (TRI ? 1 : 2) * JT;
+  static constexpr uint32_t ZIT = TRI ? 2 * DP * 128 : 0;         // triangle: one warpgroup's Z_Iᵀ, [hi | lo]
+  static constexpr uint32_t GT = TRI ? 64 * 128 : 0;              // triangle: one plane of a warpgroup's Gᵀ, 64 j x 64 i
   static constexpr uint32_t RING = ZS_PLANES * ZS_BYTES + 2 * ZIT + 4 * GT;
   static constexpr size_t SMEM = RING + STAGES * STAGE + 16 * STAGES + (TRI ? 32 : 0) + 1024;   // + Gᵀ full / empty x 2
 };
@@ -121,7 +122,7 @@ gae_split_kernel(const float* __restrict__ z, int64_t ldz, int32_t n, int32_t d,
   }
 }
 
-// fp16 triangle: z → the tf32 hi / lo planes for S as above, and per 64-row tile t the fp16 [hi | lo] block of Z_Jᵀ
+// Triangle: z → the tf32 hi / lo planes for S as above, and per 64-row tile t the fp16 [hi | lo] block of Z_Jᵀ
 // (2·DP rows x 64 j, K-major, 128-byte swizzle) of z·2^e_t, with e_t (exps[t]) chosen from the tile's largest |z| so that the
 // scaled values stay ≤ 2^14: hi = rn(x·2^e), lo = rn(x·2^e − hi), 22 significant bits like the tf32 split.  A zero tile
 // gets e = 0.  One block per 64-row tile.
@@ -179,24 +180,23 @@ struct Params {
   int row_begin, row_end;      // row form: rows [row_begin, row_end), dz row i at dz[(i - row_begin) * d]
   int sb_begin, nb, sym;       // pair-sharded form: grid.x = 2 x super-blocks from sb_begin, dz row i at dz[i * d]
   int n_jt;                    // J tiles
-  const int* exps;             // fp16 triangle: scale exponent of each 64-row tile (zt_hi holds the fp16 blocks)
+  const int* exps;             // triangle: scale exponent of each 64-row tile (zt_hi holds the fp16 blocks)
 };
 
+// tf32: the full sweep's dZ (N = DP) and S (N = JW)
 template <int N>
 __device__ __forceinline__ void mma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
   if constexpr (N == 8) wgmma_tf32_rs_n8(d, a, b, scale_d);
   else if constexpr (N == 16) wgmma_tf32_rs_n16(d, a, b, scale_d);
-  else if constexpr (N == 32) wgmma_tf32_rs_n32(d, a, b, scale_d);
-  else wgmma_tf32_rs_n64(d, a, b, scale_d);
+  else wgmma_tf32_rs_n32(d, a, b, scale_d);
 }
 template <int N>
 __device__ __forceinline__ void mma_ss(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
-  if constexpr (N == 8) wgmma_tf32_ss_n8(d, a, b, scale_d);
-  else if constexpr (N == 16) wgmma_tf32_ss_n16(d, a, b, scale_d);
-  else if constexpr (N == 32) wgmma_tf32_ss_n32(d, a, b, scale_d);
-  else if constexpr (N == 64) wgmma_tf32_ss_n64(d, a, b, scale_d);
+  if constexpr (N == 64) wgmma_tf32_ss_n64(d, a, b, scale_d);
   else wgmma_tf32_ss_n128(d, a, b, scale_d);
 }
+
+// fp16: the triangle's dZ_I and dZ_J (N = DP and 2·DP)
 
 template <int N>
 __device__ __forceinline__ void mma_rs16(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
@@ -216,9 +216,6 @@ __device__ __forceinline__ void mma_ss16(float (&d)[N / 2], uint64_t a, uint64_t
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ void sts_v2(uint32_t addr, float x, float y) {
-  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
-}
 __device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t x) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(x) : "memory");
 }
@@ -226,9 +223,9 @@ __device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t x) {
 // σ and softplus of one thread's logits S (the m64nJW accumulator), in place: S becomes the hi part of G = σ(S) and L its lo
 // part, ready to be the register A operand of the dZ product.  Returns the thread's share of Σ softplus.  MASKED zeroes G and
 // drops the loss of columns j ≥ n and of rows past the range (the last J tile, a partial I block); interior tiles skip the
-// per-logit mask and its selects.  F16: G·2^14 is split into fp16 hi / lo, packed two columns per register (the f16 A
-// fragment) into S[0 .. V/2) and L[0 .. V/2).
-template <bool MASKED, int V, bool F16 = false>
+// per-logit mask and its selects.  F16 (the triangle): G·2^14 is split into fp16 hi / lo, packed two columns per register
+// (the f16 A fragment) into S[0 .. V/2) and L[0 .. V/2).
+template <bool MASKED, int V, bool F16>
 __device__ __forceinline__ float sigmoid_softplus(float (&S)[V], float (&L)[V], int jbase, int n, bool live_a, bool live_b) {
   constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
   float relu = 0.f, lg = 0.f, prod = 1.f;
@@ -280,19 +277,18 @@ __device__ __forceinline__ float merged(const float (&acc)[NBM][DP], const float
   return t;
 }
 
-// The sweep of one work unit; TRI selects the triangle, F16 its fp16 gradient products (see header).
-template <int DP, bool TRI, bool F16 = false>
+// The sweep of one work unit; TRI selects the triangle (see header).
+template <int DP, bool TRI>
 __device__ __forceinline__ void decoder_sweep(const Params& p) {
-  static_assert(TRI || !F16, "fp16 gradient products are a triangle variant");
-  using T = Tiles<DP, TRI, F16>;
+  using T = Tiles<DP, TRI>;
   constexpr int JW = T::JW;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* zi_hi = smem;
   uint8_t* zi_lo = smem + ZS_BYTES;
-  uint8_t* zit = smem + ZS_PLANES * ZS_BYTES;      // triangle: Z_Iᵀ [warpgroup][atom][hi, lo]; then Gᵀ [warpgroup][hi, lo]
+  uint8_t* zit = smem + ZS_PLANES * ZS_BYTES;      // triangle: Z_Iᵀ [warpgroup]; then Gᵀ [warpgroup][hi, lo]
   uint8_t* ring = smem + T::RING;
-  constexpr uint32_t ATOM = DP * 128;              // DP rows of 32 tf32 along K
+  constexpr uint32_t ATOM = DP * 128;              // full sweep: DP rows of 32 tf32 along K
   constexpr int NB = DP <= 16 ? 4 : 2;             // full sweep: hi·hi accumulators
   constexpr int NBM = DP <= 16 ? 2 : 1;            // triangle: [hi·hi | hi·lo] accumulators
   const uint32_t full_bar = smem_u32(ring + STAGES * T::STAGE), empty_bar = full_bar + 8 * STAGES;
@@ -342,38 +338,21 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
       asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(TriRegs<DP>::DJ));
       if (handed0 >= nt) return;
       const int t = tid - THREADS, warp = t >> 5, lane = t & 31;
-      // F16: each warpgroup half of Z_I in its 64-row tile's scale; the half's sum is unscaled before the two are added
-      float sc_i[2] = {1.f, 1.f};
-      if constexpr (F16) {
-        const int e0 = p.exps[2 * blockIdx.x], e1 = p.exps[2 * blockIdx.x + 1];
-        sc_i[0] = unscale(e0);
-        sc_i[1] = unscale(e1);
-        // Z_Iᵀ per consumer warpgroup: [DP hi rows | DP lo rows] x 64 i (fp16) in the gt_pos order, scaled by 2^e; rows past
-        // the range are zero
-        for (int e = t; e < BT * DP; e += 128) {
-          const int r = e / DP, k = e % DP;
-          const int row = row0 + r;
-          const float v = (row < row_end && k < p.d) ? p.z[(int64_t)row * p.ldz + k] : 0.f;
-          const float x = ldexpf(v, (r >> 6) ? e1 : e0);
-          const __half xh = __float2half_rn(x);
-          const uint32_t q = (uint32_t)gt_pos(r & 63);
-          uint8_t* b = zit + (r >> 6) * T::ZIT;
-          *reinterpret_cast<__half*>(b + sw128_offset16((uint32_t)k, q)) = xh;
-          *reinterpret_cast<__half*>(b + sw128_offset16((uint32_t)(DP + k), q)) = __float2half_rn(x - __half2float(xh));
-        }
-      } else {
-        // Z_Iᵀ (B of dZ_J), per consumer warpgroup 2 atoms of [DP hi rows | DP lo rows] x 32 i in the gt_pos order; rows past
-        // the range are zero
-        for (int e = t; e < BT * DP; e += 128) {
-          const int r = e / DP, k = e % DP;
-          const int row = row0 + r;
-          const float v = (row < row_end && k < p.d) ? p.z[(int64_t)row * p.ldz + k] : 0.f;
-          const float h = tf32_trunc(v);
-          const int q = gt_pos(r & 63);
-          const uint32_t ot = (uint32_t)(r >> 6) * (4 * ATOM) + (uint32_t)(q >> 5) * (2 * ATOM) + sw128_offset32((uint32_t)k, (uint32_t)(q & 31));
-          *reinterpret_cast<float*>(zit + ot) = h;
-          *reinterpret_cast<float*>(zit + ot + ATOM) = v - h;
-        }
+      // each warpgroup half of Z_I in its 64-row tile's scale; the half's sum is unscaled before the two are added
+      const int e0 = p.exps[2 * blockIdx.x], e1 = p.exps[2 * blockIdx.x + 1];
+      const float sc_i[2] = {unscale(e0), unscale(e1)};
+      // Z_Iᵀ (B of dZ_J) per consumer warpgroup: [DP hi rows | DP lo rows] x 64 i (fp16) in the gt_pos order, scaled by 2^e;
+      // rows past the range are zero
+      for (int e = t; e < BT * DP; e += 128) {
+        const int r = e / DP, k = e % DP;
+        const int row = row0 + r;
+        const float v = (row < row_end && k < p.d) ? p.z[(int64_t)row * p.ldz + k] : 0.f;
+        const float x = ldexpf(v, (r >> 6) ? e1 : e0);
+        const __half xh = __float2half_rn(x);
+        const uint32_t q = (uint32_t)gt_pos(r & 63);
+        uint8_t* b = zit + (r >> 6) * T::ZIT;
+        *reinterpret_cast<__half*>(b + sw128_offset16((uint32_t)k, q)) = xh;
+        *reinterpret_cast<__half*>(b + sw128_offset16((uint32_t)(DP + k), q)) = __float2half_rn(x - __half2float(xh));
       }
       fence_proxy_async();
       asm volatile("bar.sync 4, 128;" ::: "memory");
@@ -386,23 +365,13 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
         for (int h = 0; h < 2; ++h) {
           mbar_wait(gt_full + 8 * h, parity);
           const uint32_t ag_hi = smem_u32(zit + 2 * T::ZIT + h * 2 * T::GT), ag_lo = ag_hi + T::GT;
-          const uint32_t bi = smem_u32(zit) + h * (F16 ? T::ZIT : 4 * ATOM);
+          const uint32_t bi = smem_u32(zit) + h * T::ZIT;
           wgmma_fence();
-          if constexpr (F16) {
 #pragma unroll
-            for (int kk = 0; kk < 64 / 16; ++kk) {
-              const uint32_t o = (uint32_t)kk * 32;
-              mma_ss16<DP>(djs, wgmma_desc_sw128(ag_lo + o), wgmma_desc_sw128(bi + o), kk > 0);
-              mma_ss16<2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + o), wgmma_desc_sw128(bi + o), kk >= NBM);
-            }
-          } else {
-#pragma unroll
-            for (int kk = 0; kk < 64 / 8; ++kk) {
-              const uint32_t oa = (uint32_t)(kk >> 2) * (64 * 128) + (uint32_t)(kk & 3) * 32;
-              const uint32_t ob = (uint32_t)(kk >> 2) * (2 * ATOM) + (uint32_t)(kk & 3) * 32;
-              mma_ss<DP>(djs, wgmma_desc_sw128(ag_lo + oa), wgmma_desc_sw128(bi + ob), kk > 0);
-              mma_ss<2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + oa), wgmma_desc_sw128(bi + ob), kk >= NBM);
-            }
+          for (int kk = 0; kk < 64 / 16; ++kk) {
+            const uint32_t o = (uint32_t)kk * 32;
+            mma_ss16<DP>(djs, wgmma_desc_sw128(ag_lo + o), wgmma_desc_sw128(bi + o), kk > 0);
+            mma_ss16<2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + o), wgmma_desc_sw128(bi + o), kk >= NBM);
           }
           wgmma_commit();
           wgmma_wait<0>();
@@ -412,10 +381,7 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
           __syncwarp();
           if (lane == 0) mbar_arrive(gt_empty + 8 * h);     // this warpgroup's Gᵀ is read
 #pragma unroll
-          for (int v = 0; v < DP / 2; ++v) {
-            if constexpr (F16) djt[v] = (h ? djt[v] : 0.f) + merged(djm, djs, v) * sc_i[h];
-            else djt[v] = (h ? djt[v] : 0.f) + merged(djm, djs, v);
-          }
+          for (int v = 0; v < DP / 2; ++v) djt[v] = (h ? djt[v] : 0.f) + merged(djm, djs, v) * sc_i[h];
         }
         const int ja = (jt0 + i) * JW + warp * 16 + (lane >> 2);
 #pragma unroll
@@ -449,14 +415,8 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
         mbar_expect_tx(fb, T::STAGE);
         bulk_load(dst, p.zs_hi + t * T::JS, T::JS, fb);
         bulk_load(dst + T::JS, p.zs_lo + t * T::JS, T::JS, fb);
-        if constexpr (F16) {
+        if constexpr (TRI) {
           bulk_load(dst + 2 * T::JS, p.zt_hi + t * T::JT, T::JT, fb);   // [hi | lo], as the split kernel wrote it
-        } else if constexpr (TRI) {
-          // atom by atom, lo after hi: the B operand [Z_Jᵀ hi | Z_Jᵀ lo] of the merged dZ_I products
-          for (uint32_t a = 0; a < T::JT / ATOM; ++a) {
-            bulk_load(dst + 2 * T::JS + 2 * a * ATOM, p.zt_hi + t * T::JT + a * ATOM, ATOM, fb);
-            bulk_load(dst + 2 * T::JS + (2 * a + 1) * ATOM, p.zt_lo + t * T::JT + a * ATOM, ATOM, fb);
-          }
         } else {
           bulk_load(dst + 2 * T::JS, p.zt_hi + t * T::JT, T::JT, fb);
           bulk_load(dst + 2 * T::JS + T::JT, p.zt_lo + t * T::JT, T::JT, fb);
@@ -539,11 +499,11 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
     wgmma_commit();
   };
   // dZ_I += G · Z_J of tile i with A = (S, L) from the registers; one batch, committed (the caller waits, then dz_fence).
-  // Full sweep: 3·16 products; triangle: 2·8.
+  // Full sweep: 3·16 products; triangle: 2·4.
   auto issue_dz = [&](int i, float (&S)[JW / 2]) {
     const uint32_t bt_hi = smem_u32(ring + (i % STAGES) * T::STAGE) + 2 * T::JS, bt_lo = bt_hi + T::JT;
     wgmma_fence();
-    if constexpr (F16) {
+    if constexpr (TRI) {
       // A = G·2^14 as packed fp16 (sigmoid_softplus), in the natural column order; B = [Z_Jᵀ hi | Z_Jᵀ lo] rows, K = j
 #pragma unroll
       for (int kb = 0; kb < JW / 16; ++kb) {
@@ -562,16 +522,10 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
                                  __float_as_uint(S[4 * kb + 3])};
         const uint32_t alo[4] = {__float_as_uint(L[4 * kb]), __float_as_uint(L[4 * kb + 2]), __float_as_uint(L[4 * kb + 1]),
                                  __float_as_uint(L[4 * kb + 3])};
-        if constexpr (TRI) {
-          const uint32_t o = (uint32_t)(kb >> 2) * (2 * ATOM) + (uint32_t)(kb & 3) * 32;   // atom [hi | lo]
-          mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
-          mma_rs<2 * DP>(dzm[kb % NBM], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NBM);
-        } else {
-          const uint32_t o = (uint32_t)(kb >> 2) * ATOM + (uint32_t)(kb & 3) * 32;
-          mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
-          mma_rs<DP>(dzs, ahi, wgmma_desc_sw128(bt_lo + o), 1);
-          mma_rs<DP>(dzb[kb % NB], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NB);
-        }
+        const uint32_t o = (uint32_t)(kb >> 2) * ATOM + (uint32_t)(kb & 3) * 32;
+        mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
+        mma_rs<DP>(dzs, ahi, wgmma_desc_sw128(bt_lo + o), 1);
+        mma_rs<DP>(dzb[kb % NB], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NB);
       }
     }
     wgmma_commit();
@@ -590,10 +544,8 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   auto retire_dz = [&](int i, float sc) {
 #pragma unroll
     for (int v = 0; v < DP / 2; ++v) {
-      if constexpr (F16) {
+      if constexpr (TRI) {
         dzt[v] += merged(dzm, dzs, v) * sc;
-      } else if constexpr (TRI) {
-        dzt[v] += merged(dzm, dzs, v);
       } else {
         float t = dzs[v];
 #pragma unroll
@@ -608,41 +560,25 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   // dZ_J warpgroup, once that warpgroup has read the previous one
   auto elementwise = [&](int i, float (&S)[JW / 2]) {
     const int jbase = (jt0 + i) * JW + 2 * (lane & 3);
-    const float l = full_rows && (jt0 + i + 1) * JW <= p.n ? sigmoid_softplus<false, JW / 2, F16>(S, L, jbase, p.n, live_a, live_b)
-                                                           : sigmoid_softplus<true, JW / 2, F16>(S, L, jbase, p.n, live_a, live_b);
+    const float l = full_rows && (jt0 + i + 1) * JW <= p.n ? sigmoid_softplus<false, JW / 2, TRI>(S, L, jbase, p.n, live_a, live_b)
+                                                           : sigmoid_softplus<true, JW / 2, TRI>(S, L, jbase, p.n, live_a, live_b);
     if constexpr (TRI) {
       if (i >= handed0) {
         loss += 2.0 * (double)l;   // a tile above the diagonal block stands for its mirror too
         mbar_wait(gt_empty + 8 * wg, (uint32_t)(((i - handed0) & 1) ^ 1));
         // column jj of G is row jj of Gᵀ; the thread's rows r, r + 8 sit at K positions gt_pos(r), gt_pos(r) + 1
         const uint32_t k = (uint32_t)gt_pos(warp * 16 + (lane >> 2));
-        if constexpr (F16) {
-          // one 32-bit store per column and plane: (r, j) and (r + 8, j) from the two registers that hold column j
-#pragma unroll
-          for (int c = 0; c < JW / 8; ++c) {
-            const uint32_t h0 = __float_as_uint(S[2 * c]), h1 = __float_as_uint(S[2 * c + 1]);
-            const uint32_t l0 = __float_as_uint(L[2 * c]), l1 = __float_as_uint(L[2 * c + 1]);
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const uint32_t sel = e ? 0x7632u : 0x5410u;
-              const uint32_t o = sw128_offset16((uint32_t)(8 * c + 2 * (lane & 3) + e), k);
-              sts_u32(smem_u32(gt_hi) + o, __byte_perm(h0, h1, sel));
-              sts_u32(smem_u32(gt_lo) + o, __byte_perm(l0, l1, sel));
-            }
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(gt_full + 8 * wg);
-          return;
-        }
-        const uint32_t base = (k >> 5) * (64 * 128);
+        // one 32-bit store per column and plane: (r, j) and (r + 8, j) from the two registers that hold column j
 #pragma unroll
         for (int c = 0; c < JW / 8; ++c) {
+          const uint32_t h0 = __float_as_uint(S[2 * c]), h1 = __float_as_uint(S[2 * c + 1]);
+          const uint32_t l0 = __float_as_uint(L[2 * c]), l1 = __float_as_uint(L[2 * c + 1]);
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const uint32_t o = base + sw128_offset32((uint32_t)(8 * c + 2 * (lane & 3) + e), k & 31);
-            sts_v2(smem_u32(gt_hi) + o, S[4 * c + e], S[4 * c + 2 + e]);
-            sts_v2(smem_u32(gt_lo) + o, L[4 * c + e], L[4 * c + 2 + e]);
+            const uint32_t sel = e ? 0x7632u : 0x5410u;
+            const uint32_t o = sw128_offset16((uint32_t)(8 * c + 2 * (lane & 3) + e), k);
+            sts_u32(smem_u32(gt_hi) + o, __byte_perm(h0, h1, sel));
+            sts_u32(smem_u32(gt_lo) + o, __byte_perm(l0, l1, sel));
           }
         }
         fence_proxy_async();
@@ -659,8 +595,8 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   if constexpr (OVERLAP) {
     float S2[JW / 2];
     // the turn of tile i ≥ 1: dZ of tile i − 1 from (Sp, L), then S of tile i into Sn
-    // F16: the scale of tile i − 1 is loaded before the waits
-    auto tile_unscale = [&](int i) { return F16 ? unscale(__ldg(p.exps + jt0 + i)) : 1.f; };
+    // the scale of tile i − 1 is loaded before the waits
+    auto tile_unscale = [&](int i) { return unscale(__ldg(p.exps + jt0 + i)); };
     auto turn = [&](int i, float (&Sp)[JW / 2], float (&Sn)[JW / 2]) {
       take_turn();
       issue_dz(i - 1, Sp);
@@ -756,31 +692,25 @@ gae_tri_tc_kernel(const __grid_constant__ Params p) {
   decoder_sweep<DP, true>(p);
 }
 
-template <int DP>
-__global__ void __launch_bounds__(TRI_THREADS, 1)
-gae_tri_f16_tc_kernel(const __grid_constant__ Params p) {
-  decoder_sweep<DP, true, true>(p);
-}
-
 size_t workspace_bytes(int32_t n) { return (size_t)padded_n(n) / BT * (ZS_PLANES * ZS_BYTES + 2 * zt_bytes<MAX_D>()); }
 
 int super_blocks(int32_t n) { return (int)((padded_n(n) / BT + 1) / 2); }
 
 bool eligible(int32_t n, int32_t d, int32_t n_rows, size_t ws_bytes) {
-  const int mode = path_mode(B2_PATH_GAE_DECODER);           // 0 auto · 1 CUDA cores · 2 these kernels · 6 with the tf32 triangle
+  const int mode = path_mode(B2_PATH_GAE_DECODER);           // 0 auto · 1 CUDA cores · 2 these kernels
   if (d < 1 || d > MAX_D || mode == 1 || ws_bytes < workspace_bytes(n)) return false;
-  return mode == 2 || mode == 6 || (int64_t)n * n_rows >= (1ll << 22);
+  return mode == 2 || (int64_t)n * n_rows >= (1ll << 22);
 }
 
-template <int DP, bool TRI, bool F16 = false>
+template <int DP, bool TRI>
 static int launch_sweep(const Params& p, int units, cudaStream_t st) {
   // J step ranges: b2_set_tuning(B2_TUNE_GAE_SPLITS) when set, else enough to fill one wave of SMs
   int splits = tuning(B2_TUNE_GAE_SPLITS);
   if (splits <= 0) splits = ceil_div(sm_count(), units);
   if (splits > p.n_jt) splits = p.n_jt;
   if (splits < 1) splits = 1;
-  auto kernel = F16 ? gae_tri_f16_tc_kernel<DP> : TRI ? gae_tri_tc_kernel<DP> : gae_allpairs_tc_kernel<DP>;
-  constexpr size_t smem = Tiles<DP, TRI, F16>::SMEM;
+  auto kernel = TRI ? gae_tri_tc_kernel<DP> : gae_allpairs_tc_kernel<DP>;
+  constexpr size_t smem = Tiles<DP, TRI>::SMEM;
   static_assert(smem <= MAX_SMEM, "decoder shared memory");
   static bool attr_set = false;
   if (!attr_set) {
@@ -788,12 +718,12 @@ static int launch_sweep(const Params& p, int units, cudaStream_t st) {
     attr_set = true;
   }
   kernel<<<dim3((unsigned)units, (unsigned)splits), TRI ? TRI_THREADS : THREADS, smem, st>>>(p);
-  B2_CHECK_LAUNCH(F16 ? "gae_tri_f16_tc_kernel" : TRI ? "gae_tri_tc_kernel" : "gae_allpairs_tc_kernel");
+  B2_CHECK_LAUNCH(TRI ? "gae_tri_tc_kernel" : "gae_allpairs_tc_kernel");
   return B2_OK;
 }
 
 // Splits z into the workspace planes, then sweeps `units` work units (none: the split only).  tri: every row against every
-// column by the triangle (units must be the nb row blocks), with fp16 gradient products unless tf32 is asked for.
+// column by the triangle (units must be the nb row blocks), which takes the fp16 split.
 template <int DP>
 static int launch_dp(Params p, int units, bool tri, void* ws, cudaStream_t st) {
   const int64_t npad = padded_n(p.n);
@@ -801,15 +731,15 @@ static int launch_dp(Params p, int units, bool tri, void* ws, cudaStream_t st) {
   uint8_t* zs_hi = reinterpret_cast<uint8_t*>(ws);
   uint8_t* zs_lo = zs_hi + (size_t)p.nb * ZS_BYTES;
   uint8_t* zt_hi = zs_lo + (size_t)p.nb * ZS_BYTES;
-  if (tri && units > 0 && path_mode(B2_PATH_GAE_DECODER) != 6) {
+  if (tri && units > 0) {
     // the fp16 Z_Jᵀ blocks (2·nb of 2·DP·128 bytes) and the tile exponents take the place of the tf32 Z_Jᵀ planes
-    static_assert(2 * 2 * DP * 128 + 2 * sizeof(int) <= 2 * zt_bytes<MAX_D>(), "fp16 triangle workspace");
+    static_assert(2 * 2 * DP * 128 + 2 * sizeof(int) <= 2 * zt_bytes<MAX_D>(), "triangle workspace");
     int* exps = reinterpret_cast<int*>(zt_hi + (size_t)(2 * p.nb) * (2 * DP * 128));
     gae_split_f16_kernel<DP><<<(unsigned)(2 * p.nb), 256, 0, st>>>(p.z, p.ldz, p.n, p.d, zs_hi, zs_lo, zt_hi, exps);
     B2_CHECK_LAUNCH("gae_split_f16_kernel");
     p.zs_hi = zs_hi; p.zs_lo = zs_lo; p.zt_hi = zt_hi; p.exps = exps;
-    p.n_jt = ceil_div(p.n, Tiles<DP, true, true>::JW);
-    return launch_sweep<DP, true, true>(p, units, st);
+    p.n_jt = ceil_div(p.n, Tiles<DP, true>::JW);   // 64-column tiles holding at least one column j < n
+    return launch_sweep<DP, true>(p, units, st);
   }
   uint8_t* zt_lo = zt_hi + (size_t)p.nb * zt_bytes<DP>();
   int64_t blocks = ceil_div<int64_t>(npad * DP, 256);
@@ -819,10 +749,6 @@ static int launch_dp(Params p, int units, bool tri, void* ws, cudaStream_t st) {
   B2_CHECK_LAUNCH("gae_split_kernel");
   if (units <= 0) return B2_OK;
   p.zs_hi = zs_hi; p.zs_lo = zs_lo; p.zt_hi = zt_hi; p.zt_lo = zt_lo;
-  if (tri) {
-    p.n_jt = ceil_div(p.n, Tiles<DP, true>::JW);   // 64-column tiles holding at least one column j < n
-    return launch_sweep<DP, true>(p, units, st);
-  }
   p.n_jt = p.nb;
   return launch_sweep<DP, false>(p, units, st);
 }

@@ -55,7 +55,7 @@ int64_t b2_launch_count(void) { return (int64_t)b2::g_launch_count; }
 
 int b2_set_path(int which, int mode) {
   B2_REQUIRE(which >= 0 && which < B2_PATH_COUNT, "b2_set_path: unknown selector %d", which);
-  const bool ok = which == B2_PATH_GAE_DECODER ? (mode >= 0 && mode <= 2) || mode == 6 : mode == 0 || mode == 1;
+  const bool ok = which == B2_PATH_GAE_DECODER ? mode >= 0 && mode <= 2 : mode == 0 || mode == 1;
   B2_REQUIRE(ok, "b2_set_path: mode %d out of range for selector %d", mode, which);
   b2::g_path[which] = mode;
   return B2_OK;

@@ -125,14 +125,13 @@ def _workspace(nbytes: int, device) -> torch.Tensor:
     return buf
 
 
-_PATHS = {"gae": (0, {"auto": 0, "cuda": 1, "tc": 2, "tc_tf32": 6}), "knn": (1, {"auto": 0, "simt": 1}),
+_PATHS = {"gae": (0, {"auto": 0, "cuda": 1, "tc": 2}), "knn": (1, {"auto": 0, "simt": 1}),
           "spmm": (2, {"auto": 0, "rowgroup": 1})}
 
 
 def set_path(which: str, mode: str = "auto") -> None:
-    """Select the kernel path of the decoder ("gae": auto | cuda | tc | tc_tf32, the last with the triangle's gradient products
-    in tf32 instead of fp16), of the kNN candidate filter
-    ("knn": auto | simt) or of the aggregate ("spmm": auto | rowgroup).  All paths return the same result; the switch exists
+    """Select the kernel path of the decoder ("gae": auto | cuda | tc), of the kNN candidate filter ("knn": auto | simt) or
+    of the aggregate ("spmm": auto | rowgroup).  All paths return the same result; the switch exists
     for A/B tests and timing."""
     sel, modes = _PATHS[which]
     check(lib().b2_set_path(sel, modes[mode]), "b2_set_path")

@@ -49,8 +49,7 @@ extern "C" {
 /* Kernel-path selectors for A/B tests: every selectable path returns the same result (bit-exact for the kNN filter, to
  * rounding for the decoder); mode 0 = automatic choice by problem size. */
 #define B2_PATH_GAE_DECODER 0 /* 1 CUDA cores · 2 tensor cores (S in wgmma tf32, 3-product split; the call over all rows takes
-                                 its gradient products in fp16 hi / lo with a power-of-two scale per tile) · 6 = 2 | 4,
-                                 tensor cores with every product in tf32 (bit 4: the tf32 triangle) */
+                                 its gradient products in fp16 hi / lo with a power-of-two scale per tile) */
 #define B2_PATH_KNN_FILTER 1  /* 1 SIMT candidate filter */
 #define B2_PATH_SPMM 2        /* 1 row-per-lane-group kernels for every shape (default: the nnz-stream kernel where it applies) */
 #define B2_PATH_COUNT 3

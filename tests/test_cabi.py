@@ -133,6 +133,7 @@ def test_selector_tables_match_the_header():
     assert lib.b2_set_path(consts["B2_PATH_SPMM"], 1) == 0 and lib.b2_get_path(consts["B2_PATH_SPMM"]) == 1
     assert lib.b2_set_path(consts["B2_PATH_SPMM"], 0) == 0
     assert lib.b2_set_path(consts["B2_PATH_GAE_DECODER"], 2) == 0 and lib.b2_set_path(consts["B2_PATH_GAE_DECODER"], 3) != 0
+    assert lib.b2_set_path(consts["B2_PATH_GAE_DECODER"], 6) != 0
     assert lib.b2_set_path(consts["B2_PATH_GAE_DECODER"], 0) == 0
     for knob, idx in (("gae_splits", consts["B2_TUNE_GAE_SPLITS"]),):
         assert lib.b2_set_tuning(idx, 1) == 0

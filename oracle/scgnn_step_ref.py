@@ -14,7 +14,7 @@ elsewhere) and casts everything to float64.  Gradients come from ``torch.autogra
 """
 from __future__ import annotations
 
-from typing import Dict, Optional
+from typing import Callable, Dict, Optional, Tuple
 
 import torch
 import torch.nn.functional as F
@@ -79,11 +79,14 @@ def feature_ae_step(x: torch.Tensor, params: Dict[str, torch.Tensor], regularize
 
 
 def graph_ae_step(x: torch.Tensor, adj_rowptr, adj_colidx, adj_vals, labels_rowptr, labels_colidx, norm: float, pos_weight: float,
-                  weights: Dict[str, torch.Tensor], eps: Optional[torch.Tensor]) -> dict:
+                  weights: Dict[str, torch.Tensor], eps: Optional[torch.Tensor],
+                  decoder: Optional[Callable[[torch.Tensor], Tuple[float, torch.Tensor]]] = None) -> dict:
     """Forward, loss and backward of one Graph-AE (GCN) epoch on the normalised adjacency Â (CSR, n × n) and the label pattern
     A + I (CSR, unit values), from ``weights`` gc1.weight [dim, 32], gc2.weight / gc3.weight [32, emb] (GraphConvolution layout).
-    ``eps=None`` is eval mode (z = mu).  Returns {"loss", "z", "mu", "logvar", "dz", "dmu", "dlogvar", "grads": {name: …}}, all
-    float64; dmu / dlogvar are the total loss gradients (decoder through z plus KLD)."""
+    ``eps=None`` is eval mode (z = mu).  ``decoder(z)`` → (loss, dz), float64, replaces the unit-label closed form
+    :func:`gae_reference_rows` (then the label arguments are not read): real-valued labels.  Returns {"loss", "z", "mu",
+    "logvar", "dz", "dmu", "dlogvar", "grads": {name: …}}, all float64; dmu / dlogvar are the total loss gradients (decoder through
+    z plus KLD)."""
     names = ("gc1.weight", "gc2.weight", "gc3.weight")
     w = _leaves(weights, names)
     n = x.shape[0]
@@ -100,7 +103,12 @@ def graph_ae_step(x: torch.Tensor, adj_rowptr, adj_colidx, adj_vals, labels_rowp
     kld = -0.5 / n * torch.mean(torch.sum(1 + 2 * logvar - mu.pow(2) - logvar.exp().pow(2), 1))
     for t in (mu, logvar, z):
         t.retain_grad()
-    dec, dz = gae_reference_rows(z.detach(), labels_rowptr.to(dev), labels_colidx.to(dev), norm, pos_weight, torch.arange(n, device=dev))
+    if decoder is None:
+        dec, dz = gae_reference_rows(z.detach(), labels_rowptr.to(dev), labels_colidx.to(dev), norm, pos_weight,
+                                     torch.arange(n, device=dev))
+    else:
+        dec, dz = decoder(z.detach())
+        dz = torch.as_tensor(dz, dtype=torch.float64, device=dev)
     torch.autograd.backward([z, kld], [dz, torch.ones_like(kld)])
     return {"loss": dec + kld.item(), "z": z.detach(), "mu": mu.detach(), "logvar": logvar.detach(), "dz": dz, "dmu": mu.grad,
             "dlogvar": logvar.grad, "grads": {k: w[k].grad for k in names}}

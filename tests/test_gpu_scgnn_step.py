@@ -16,6 +16,7 @@ import torch
 
 from conftest import rel_err
 from oracle import scgnn_step_ref as R
+from step_compare import adam_reference, param_views, row_rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -47,17 +48,6 @@ def _check(case, what, err, tol):
     assert err < tol, f"{case}: {what} error {err:.3g} exceeds {tol:.3g}"
 
 
-def row_rel_err(a, ref):
-    """Worst row of ‖a_i − ref_i‖ / ‖ref_i‖.  Rows whose reference norm is below 1e-3 of the RMS row
-    norm are measured against that floor instead, so that a near-zero row does not turn rounding into a large ratio."""
-    a = torch.as_tensor(a).double()
-    ref = torch.as_tensor(ref).double().to(a.device)
-    a, ref = a.reshape(a.shape[0], -1), ref.reshape(ref.shape[0], -1)
-    den = ref.norm(dim=1)
-    floor = 1e-3 * float(den.pow(2).mean().sqrt())
-    return float(((a - ref).norm(dim=1) / den.clamp(min=max(floor, 1e-300))).max())
-
-
 def _compare(case, what, got, ref, tol, kind):
     """Norm-wise error; for a matrix also the worst row, and for a gradient matrix the worst column.  A 1-D bias gradient is
     compared norm-wise only: each element is one column sum over the batch, and for near-cancelling sums the per-element error
@@ -69,30 +59,13 @@ def _compare(case, what, got, ref, tol, kind):
             _check(case, what + " cols", row_rel_err(got.t(), torch.as_tensor(ref).t()), tol[kind + "_col"])
 
 
-def _adam_reference(flat0, grads, lr):
-    """float64 torch.optim.Adam (the engines' defaults: betas 0.9 / 0.999, eps 1e-8, no weight decay) over the flat parameter
-    vector, applied to the given sequence of gradients."""
-    p = flat0.double().clone().requires_grad_()
-    opt = torch.optim.Adam([p], lr=lr)
-    for g in grads:
-        p.grad = g.double()
-        opt.step()
-    return p.detach()
-
-
 def _check_adam(case, flat0, flat1, grads, lr, tol):
     """The optimiser's move of every weight, against float64 Adam on the same gradients: norm-wise, and worst element in units
     of lr (each step moves a weight by at most about lr)."""
-    ref = _adam_reference(flat0, grads, lr)
+    ref = adam_reference(flat0, grads, lr)
     moved, want = flat1.double() - flat0.double(), ref - flat0.double()
     _check(case, "adam update", rel_err(moved, want), tol["adam"])
     _check(case, "adam update max/lr", float((moved - want).abs().max()) / lr, tol["adam_max"])
-
-
-def _views(params, flat):
-    """The named parameters of a FlatParams, as views into a copy `flat` of its flat buffer."""
-    base = params.flat.storage_offset()
-    return {k: flat[v.storage_offset() - base:v.storage_offset() - base + v.numel()].view(v.shape) for k, v in params.p.items()}
 
 
 def _gemm_ws(M, N, K, precision):
@@ -139,15 +112,15 @@ def feature_ae_case(cuda, n_rows, genes, precision, seed):
     assert len(steps) == len(batches)
     ref_loss = 0.0
     for (b0, b1), (flat, grad) in zip(batches, steps):
-        ref = R.feature_ae_step(X[b0:b1], _views(eng.params, flat), "LTMG", 0.9, None)
+        ref = R.feature_ae_step(X[b0:b1], param_views(eng.params, flat), "LTMG", 0.9, None)
         ref_loss += ref["loss"].item()
         at = f"{case} rows {b0}:{b1}"
         _compare(at, "z", z_all[b0:b1], ref["z"], tol, "act")
         _compare(at, "recon", r_all[b0:b1], ref["recon"], tol, "act")
-        g = _views(eng.params, grad)
+        g = param_views(eng.params, grad)
         for k in R.FEATURE_AE_PARAMS:
             _compare(at, f"d {k}", g[k], ref["grads"][k], tol, "grad")
-    for k, v in _views(eng.params, steps[-1][1]).items():
+    for k, v in param_views(eng.params, steps[-1][1]).items():
         assert torch.equal(eng.params.g[k], v), k          # params.g still holds the last batch's gradients after Adam
     _check(case, "loss", abs(loss - ref_loss) / abs(ref_loss), tol["loss"])
     _check_adam(case, steps[0][0], eng.params.flat, [g for _, g in steps], eng.lr, tol)

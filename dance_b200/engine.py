@@ -17,6 +17,7 @@ from __future__ import annotations
 import os
 from typing import Callable, Dict, List, Optional, Tuple
 
+import numpy as np
 import torch
 
 from . import ops
@@ -504,3 +505,242 @@ class GATEngine:
         self.params.adam_step(self.lr)
         self.step += 1
         return z
+
+
+class GraphSCEngine:
+    """graph-sc's GCNAE (graphsc.py:290-411) trained by GraphSC.fit's loop (:185-231) on the device.
+
+    Per mini-batch of cell nodes: the block out-degrees (one histogram per layer, ``ops.graphsc_block_degrees``), two train-mode
+    forwards with independent dropout draws (the first one's embedding is recorded in cell order, the second one's logits give
+    the loss), the fused decoder loss / gradient, the backward and one Adam step over the flat parameter bucket.  WeightedGraphConv
+    aggregates before its product with W (linear, so equal to the reference's W-first order up to rounding).  Nothing inside
+    :meth:`train_epoch` synchronises with the host: batch composition is known on the host (the permutation is drawn there), the
+    per-batch losses stay in :attr:`losses` and the embeddings in :attr:`z`.
+
+    Dropout keys (``ops.dropout(ones, p, drop_seed, key)`` reproduces a mask): :meth:`drop_key`; feature-dropout rows are
+    global node ids, decoder rows are positions in the batch.
+    """
+
+    SITES = ("layer1", "layer2", "decoder")
+    DEC_P = 0.1           # InnerProductDecoder's F.dropout(z, 0.1), always in training mode (graphsc.py:408-411)
+
+    def __init__(self, *, agg: str = "sum", activation: str = "relu", in_feats: int = 50, n_hidden: int = 1, hidden_dim: int = 200,
+                 hidden_1: int = 300, hidden_2: int = 0, dropout: float = 0.1, n_layers: int = 1, hidden_relu: bool = False,
+                 hidden_bn: bool = False, device="cuda", drop_seed: int = 0, precision: Optional[str] = None):
+        if agg not in ("sum", "mean"):
+            raise ValueError(f"agg must be 'sum' or 'mean', got {agg!r}")
+        if n_layers not in (1, 2):
+            raise ValueError(f"n_layers must be 1 or 2, got {n_layers}")
+        if n_hidden not in (0, 1, 2):
+            raise ValueError(f"n_hidden must be 0, 1 or 2, got {n_hidden}")
+        if not 0.0 <= float(dropout) < 1.0:
+            raise ValueError(f"dropout must be in [0, 1), got {dropout}")
+        hidden = [hidden_1, hidden_2][:n_hidden]
+        for name, w in (("in_feats", in_feats), ("hidden_dim", hidden_dim), ("hidden_1", hidden_1 if n_hidden >= 1 else 1),
+                        ("hidden_2", hidden_2 if n_hidden == 2 else 1)):
+            if int(w) <= 0:
+                raise ValueError(f"{name} must be a positive layer width, got {w}")
+        self.agg, self.activation, self.n_layers, self.hidden = agg, activation, n_layers, hidden
+        self.dropout, self.hidden_relu, self.hidden_bn = float(dropout), bool(hidden_relu), bool(hidden_bn)
+        self.device, self.drop_seed, self.precision = torch.device(device), int(drop_seed), precision
+        self.stride = 1 + self.hidden_bn + self.hidden_relu
+        self.emb_dim = hidden[-1] if hidden else hidden_dim
+        shapes = [(f"layer{l + 1}.weight", (in_feats if l == 0 else hidden_dim, hidden_dim)) for l in range(n_layers)]
+        shapes = [s for l in range(n_layers) for s in (shapes[l], (f"layer{l + 1}.bias", (hidden_dim, )))]
+        self.lin, prev = [], hidden_dim
+        for i, w in enumerate(hidden):
+            li = f"encoder.{i * self.stride}"
+            shapes += [(li + ".weight", (w, prev)), (li + ".bias", (w, ))]
+            bn = f"encoder.{i * self.stride + 1}" if self.hidden_bn else None
+            if bn:
+                shapes += [(bn + ".weight", (w, )), (bn + ".bias", (w, ))]
+            self.lin.append((li, bn))
+            prev = w
+        self.params = FlatParams(shapes, self.device)
+        self.running = {bn + k: torch.zeros(self.params.shapes[bn + ".weight"], dtype=torch.float32, device=self.device)
+                        for _, bn in self.lin if bn for k in (".running_mean", ".running_var")}
+        self.num_batches_tracked = 0
+        self.reset_parameters()
+        self.step = 0
+        self.z: Optional[torch.Tensor] = None
+        self.losses: Optional[torch.Tensor] = None
+        self._ones_buf: Optional[torch.Tensor] = None
+
+    def reset_parameters(self, gen: Optional[torch.Generator] = None):
+        """GraphConv: xavier_uniform weight, zero bias; nn.Linear: kaiming-uniform; BatchNorm1d: 1 / 0, running 0 / 1."""
+        P = self.params.p
+        for l in range(self.n_layers):
+            w = torch.empty(P[f"layer{l + 1}.weight"].shape)
+            _xavier_uniform_(w, gen)
+            P[f"layer{l + 1}.weight"].copy_(w)
+            P[f"layer{l + 1}.bias"].zero_()
+        for li, bn in self.lin:
+            w, b = torch.empty(P[li + ".weight"].shape), torch.empty(P[li + ".bias"].shape)
+            _linear_init_(w, b, gen)
+            P[li + ".weight"].copy_(w)
+            P[li + ".bias"].copy_(b)
+            if bn:
+                P[bn + ".weight"].fill_(1.0)
+                P[bn + ".bias"].zero_()
+                self.running[bn + ".running_mean"].zero_()
+                self.running[bn + ".running_var"].fill_(1.0)
+        self.num_batches_tracked = 0
+
+    # ---- state --------------------------------------------------------------------------------------------------------------
+    def state_dict(self) -> Dict[str, torch.Tensor]:
+        """The reference GCNAE's state_dict keys and shapes (layer weights [in, out], Linear weights [out, in])."""
+        sd = {}
+        for n in self.params.names:
+            sd[n] = self.params.p[n].detach().clone()
+            if n.endswith(".bias") and n[:-5] + ".running_mean" in self.running:
+                for k in (".running_mean", ".running_var"):
+                    sd[n[:-5] + k] = self.running[n[:-5] + k].clone()
+                sd[n[:-5] + ".num_batches_tracked"] = torch.tensor(self.num_batches_tracked, dtype=torch.long)
+        return sd
+
+    def load_state_dict(self, sd):
+        missing = [k for k in self.state_dict() if k not in sd]
+        if missing:
+            raise KeyError(f"state_dict lacks {missing}")
+        for n in self.params.names:
+            self.params.p[n].copy_(torch.as_tensor(sd[n], dtype=torch.float32))
+        for k, v in self.running.items():
+            v.copy_(torch.as_tensor(sd[k], dtype=torch.float32))
+        for _, bn in self.lin:
+            if bn:
+                self.num_batches_tracked = int(sd[bn + ".num_batches_tracked"])
+
+    def drop_key(self, step: int, pas: int, site: str) -> int:
+        """Key of the dropout draw at ``site`` of forward ``pas`` (0: embedding, 1: loss) in mini-batch ``step``."""
+        return (step * 2 + pas) * len(self.SITES) + self.SITES.index(site)
+
+    # ---- one mini-batch -----------------------------------------------------------------------------------------------------
+    def _ones(self, n: int) -> torch.Tensor:
+        """[1, n] of ones (bias gradients are 1×n by n×out products): a view of one grow-only buffer."""
+        if self._ones_buf is None or self._ones_buf.shape[1] < n:
+            self._ones_buf = torch.ones(1, max(n, 256), dtype=torch.float32, device=self.device)
+        return self._ones_buf[:, :n]
+
+    def _conv(self, l: int, A, dst, deg, x, x_pos, pas: int, keep: dict):
+        P, act = self.params.p, self.activation
+        a = ops.graphsc_block_aggregate(A, dst, deg, x, self.agg, self.dropout, self.drop_seed,
+                                        self.drop_key(self.step, pas, f"layer{l + 1}"), x_pos=x_pos)
+        if act in ops.ACT:              # relu: in the GEMM epilogue; leaky_relu / gelu: their own pass over the pre-activation
+            h = ops.gemm(a, P[f"layer{l + 1}.weight"], bias=P[f"layer{l + 1}.bias"], act=act, precision=self.precision)
+        else:
+            keep[f"pre{l}"] = ops.gemm(a, P[f"layer{l + 1}.weight"], bias=P[f"layer{l + 1}.bias"], precision=self.precision)
+            h = ops.act(keep[f"pre{l}"], act)
+        keep[f"agg{l}"], keep[f"h{l}"] = a, h
+        return h
+
+    def _forward(self, blk: dict, pas: int, keep: dict) -> torch.Tensor:
+        A, X = blk["A"], blk["X"]
+        if self.n_layers == 1:
+            x = self._conv(0, A, blk["dst"], blk["deg"][0], X, None, pas, keep)
+        else:
+            h1 = self._conv(0, A, blk["src"], blk["deg"][0], X, None, pas, keep)
+            x = self._conv(1, A, blk["dst"], blk["deg"][1], h1, blk["pos"], pas, keep)
+        P = self.params.p
+        for i, (li, bn) in enumerate(self.lin):
+            keep[f"in{i}"] = x
+            relu = "relu" if self.hidden_relu else None
+            y = ops.gemm(x, P[li + ".weight"], transB=True, bias=P[li + ".bias"], act=None if bn else relu, precision=self.precision)
+            if bn:
+                keep[f"lin{i}"] = y
+                y, sm, si = ops.batchnorm_fwd(y, P[bn + ".weight"], P[bn + ".bias"], self.running[bn + ".running_mean"],
+                                              self.running[bn + ".running_var"], True, 0.1, 1e-5, act=relu)
+                keep[f"bn{i}"] = (sm, si)
+            keep[f"out{i}"] = y
+            x = y
+        return x
+
+    def _backward(self, blk: dict, dz: torch.Tensor, keep: dict):
+        P, G, pr = self.params.p, self.params.g, self.precision
+        ones = self._ones(dz.shape[0])
+        dx = dz
+        for i in reversed(range(len(self.lin))):
+            li, bn = self.lin[i]
+            if bn:
+                sm, si = keep[f"bn{i}"]
+                dx, _, _ = ops.batchnorm_bwd(dx, keep[f"out{i}"], keep[f"lin{i}"], P[bn + ".weight"], sm, si,
+                                             act="relu" if self.hidden_relu else None, dgamma=G[bn + ".weight"], dbeta=G[bn + ".bias"])
+            elif self.hidden_relu:
+                dx = ops.act_bwd(dx, "relu", y=keep[f"out{i}"])
+            ops.gemm(dx, keep[f"in{i}"], transA=True, out=G[li + ".weight"], precision="fp32")
+            ops.gemm(ones, dx, out=G[li + ".bias"].view(1, -1), precision="fp32")
+            dx = ops.gemm(dx, P[li + ".weight"], precision=pr)
+        for l in reversed(range(self.n_layers)):
+            W = P[f"layer{l + 1}.weight"]
+            a = keep[f"agg{l}"]
+            dpre = ops.act_bwd(dx, self.activation, y=keep[f"h{l}"], x=keep.get(f"pre{l}"))
+            ops.gemm(a, dpre, transA=True, out=G[f"layer{l + 1}.weight"], precision="fp32")
+            ops.gemm(self._ones(a.shape[0]), dpre, out=G[f"layer{l + 1}.bias"].view(1, -1), precision="fp32")
+            if l == 1:
+                da = ops.gemm(dpre, W, transB=True, precision=pr)
+                dx = ops.graphsc_block_aggregate(A=blk["A"], dst=blk["dst"], outdeg=blk["deg"][1], x=da, agg=self.agg, p=self.dropout,
+                                                 seed=self.drop_seed, key=self.drop_key(self.step, 1, "layer2"), x_pos=blk["pos"],
+                                                 transposed=True, out_rows=keep["agg0"].shape[0])
+
+    def train_batch(self, blk: dict, lr: float, loss_out: torch.Tensor):
+        """Both forwards, the loss into ``loss_out`` [1], the backward and one Adam step for the batch ``blk`` (see train_epoch)."""
+        B = blk["dst"].numel()
+        if self.hidden_bn and B == 1:
+            raise ValueError(f"Expected more than 1 value per channel when training, got input size torch.Size([1, {self.hidden[0]}])")
+        self._ones(max(B, blk["src"].numel() if blk["src"] is not None else 0))     # sized before the step: no allocation in it
+        keep = {}
+        z = self._forward(blk, 0, keep)
+        ops.graphsc_scatter_rows(z, blk["dst"], self.z, offset=blk["cell_offset"])
+        keep = {}
+        z = self._forward(blk, 1, keep)
+        _, dz = ops.graphsc_batch_decoder(z, self.DEC_P, self.drop_seed, self.drop_key(self.step, 1, "decoder"), loss=loss_out)
+        self._backward(blk, dz, keep)
+        self.params.adam_step(lr)
+        if self.hidden_bn:
+            self.num_batches_tracked += 2
+        self.step += 1
+
+    def train_epoch(self, graph: dict, train_ids, batch_size: int, lr: float) -> torch.Tensor:
+        """One epoch of GraphSC.fit: the batch order is ``train_ids[torch.randperm(n_train)]`` on torch's default CPU generator
+        (as dgl's DataLoader(shuffle=True) draws it), batches of ``batch_size`` with the short last one kept.  ``graph`` comes from
+        :func:`prepare_graph`.  Returns the per-batch losses (device) and leaves the embeddings of this epoch in :attr:`z`
+        [n_cells, d] (cell order)."""
+        train_ids = torch.as_tensor(train_ids, dtype=torch.long)
+        order = train_ids[torch.randperm(train_ids.numel())]
+        self.last_order = order
+        order_dev = order.to(torch.int32).pin_memory().to(self.device, non_blocking=True)
+        n_cells = graph["n_cells"]
+        if self.z is None or self.z.shape[0] != n_cells:
+            self.z = torch.zeros(n_cells, self.emb_dim, dtype=torch.float32, device=self.device)
+        nb = (order.numel() + batch_size - 1) // batch_size
+        self.losses = torch.empty(nb, dtype=torch.float32, device=self.device)
+        indptr, A = graph["indptr_host"], graph["A"]
+        for b in range(nb):
+            dst = order_dev[b * batch_size:(b + 1) * batch_size]
+            blk = dict(A=A, X=graph["X"], dst=dst, cell_offset=graph["cell_offset"], src=None, pos=None)
+            if self.n_layers == 1:
+                blk["deg"] = [ops.graphsc_block_degrees(A, dst)]
+            else:
+                ids = order[b * batch_size:(b + 1) * batch_size].numpy()
+                cap = int(min(A.shape[0], (indptr[ids + 1] - indptr[ids]).sum()))       # Σ row lengths bounds the sources
+                deg2, src, pos = ops.graphsc_block_degrees(A, dst, src_cap=cap)
+                blk.update(src=src, pos=pos, deg=[ops.graphsc_block_degrees(A, src), deg2])
+            self.train_batch(blk, lr, self.losses[b:b + 1])
+        return self.losses
+
+
+def prepare_graph(graph, device="cuda") -> dict:
+    """The device view of a cell–gene graph (GraphLite with ndata 'features', 'feat_id' and edata 'weight'): the
+    destination-indexed CSR with edge weights, the node features, the training (cell) node ids and the first cell's node id."""
+    dev = torch.device(device)
+    A, _ = graph.to(dev).csr_by_destination("weight")
+    if A.vals is not None and A.vals.dtype != torch.float32:
+        A = CSR(A.rowptr, A.colidx, A.vals.float().contiguous(), A.shape)
+    feat_id = torch.as_tensor(graph.ndata["feat_id"]).cpu()
+    train_ids = torch.nonzero(feat_id != -1).flatten()
+    off = int(train_ids[0]) if train_ids.numel() else 0
+    if not torch.equal(feat_id[train_ids].long(), torch.arange(train_ids.numel())) or not torch.equal(
+            train_ids, torch.arange(off, off + train_ids.numel())):
+        raise ValueError("expected the cell nodes to follow the gene nodes in cell order (CellFeatureGraph's layout)")
+    X = torch.as_tensor(graph.ndata["features"]).to(dev, torch.float32).contiguous()
+    return dict(A=A, X=X, indptr_host=A.rowptr.cpu().numpy().astype(np.int64), train_ids=train_ids, cell_offset=off,
+                n_cells=train_ids.numel())

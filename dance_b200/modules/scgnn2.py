@@ -364,9 +364,11 @@ def cluster_output_handler(listResult):
     return list(listResult), [np.nonzero(lab == c)[0].tolist() for c in range(len(set(lab.tolist())))]
 
 
-def kmeans_fit_predict(embed, k: int, device, seed: int = 0, init_max_cells: int = 200_000):
-    """``KMeans(n_clusters=k, n_init="auto", random_state=0).fit_predict(embed)`` (scgnn2.py:186): k-means++ seeding by
-    sklearn's own routine on the host (on a fixed-seed subsample above ``init_max_cells`` cells), Lloyd iterations on the device."""
+def kmeans_fit_predict(embed, k: int, device, seed: int = 0, init_max_cells: int = 200_000, n_init: int = 1):
+    """``KMeans(n_clusters=k, n_init=n_init, random_state=seed).fit_predict(embed)`` (scgnn2.py:186 with n_init 1, graphsc.py:260
+    with 10): k-means++ seeding by sklearn's own routine on the host (on a fixed-seed subsample above ``init_max_cells`` cells),
+    Lloyd iterations on the device.  The n_init seedings draw in turn from one ``RandomState(seed)`` and the run with the lowest
+    inertia wins, as sklearn chooses (a later run replaces the best only when it is lower and partitions differently)."""
     from sklearn.cluster import kmeans_plusplus
     xe = embed if isinstance(embed, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(embed, dtype=np.float32))
     xe = xe.to(device).float().contiguous()
@@ -377,13 +379,30 @@ def kmeans_fit_predict(embed, k: int, device, seed: int = 0, init_max_cells: int
     else:
         host = xe.cpu().numpy()
     host = host - host.mean(0)                      # KMeans centres the data before seeding (sklearn _kmeans.py: X -= X_mean)
-    # KMeans.fit hands its RandomState(random_state) straight to the k-means++ routine (sklearn _kmeans.py, _init_centroids)
-    centers, _ = kmeans_plusplus(host.astype(np.float32), k, random_state=np.random.RandomState(seed))
     mean = xe.mean(0, keepdim=True)
     xc = (xe - mean).contiguous()
-    C0 = torch.from_numpy(np.ascontiguousarray(centers, dtype=np.float32)).to(device)
-    labels, _, _ = ops.kmeans(xc, C0)
-    return labels
+    # KMeans.fit hands its RandomState(random_state) straight to the k-means++ routine (sklearn _kmeans.py, _init_centroids)
+    rs = np.random.RandomState(seed)
+    best, best_inertia = None, None
+    for _ in range(int(n_init)):
+        centers, _ = kmeans_plusplus(host.astype(np.float32), k, random_state=rs)
+        C0 = torch.from_numpy(np.ascontiguousarray(centers, dtype=np.float32)).to(device)
+        labels, inertia, _ = ops.kmeans(xc, C0)
+        if best is None or (inertia < best_inertia and not _same_clustering(labels, best, k)):
+            best, best_inertia = labels, inertia
+    return best
+
+
+def _same_clustering(a: torch.Tensor, b: torch.Tensor, k: int) -> bool:
+    """sklearn's _is_same_clustering: the two labelings are one partition up to a relabelling."""
+    a, b = a.cpu().numpy(), b.cpu().numpy()
+    mapping = np.full(k, -1)
+    for x, y in zip(a, b):
+        if mapping[x] == -1:
+            mapping[x] = y
+        elif mapping[x] != y:
+            return False
+    return True
 
 
 def clustering_handler(edgeList, args, param):

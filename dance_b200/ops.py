@@ -15,6 +15,8 @@ from ._lib import B2Error, check
 from ._lib import lib as _raw_lib
 
 ACT = {"none": 0, None: 0, "relu": 1, "elu": 2, "tanh": 3}
+# every activation code, for act / act_bwd; the GEMM / SpMM epilogues take ACT only
+ACT_ALL = {**ACT, "leaky_relu": 4, "gelu": 5}
 PREC = {"fp32": 0, "simt": 0, "tf32x3": 1, "tf32": 2, "bf16": 3}
 
 _DEFAULT_PRECISION = "tf32x3"
@@ -1280,3 +1282,96 @@ def concat_normalized(left: torch.Tensor, right: torch.Tensor, base: Optional[to
                                      _p(cmax), lo, hi, int(base is not None), _p(out), pitch, _p(ws), ws.numel(), _stream()),
           "b2_concat_scaled_f32")
     return out[:, :a + e]
+
+
+# ----------------------------------------------------------------------------- graph-sc mini-batch blocks (csrc/graphsc.cu)
+def act(x, act: Optional[str], out=None):
+    """``act(x)`` elementwise, for the activations the GEMM epilogue does not take (leaky_relu, gelu) as well as the others."""
+    _chk(x, torch.float32, "x", 2)
+    out = torch.empty_like(x) if out is None else out
+    check(lib().b2_act_f32(_p(x), _rowmajor(x, "x"), x.shape[0], x.shape[1], ACT_ALL[act], _p(out), _rowmajor(out, "out"), _stream()),
+          "b2_act_f32")
+    return out
+
+
+def act_bwd(dy, act: Optional[str], y=None, x=None, out=None):
+    """``dy ⊙ act'``: from the output ``y`` for relu / elu / tanh / leaky_relu, from the pre-activation ``x`` for gelu."""
+    _chk(dy, torch.float32, "dy", 2)
+    out = torch.empty_like(dy) if out is None else out
+    check(lib().b2_act_bwd_f32(_p(dy), _rowmajor(dy, "dy"), _p(y), _rowmajor(y, "y") if y is not None else 0, _p(x),
+                               _rowmajor(x, "x") if x is not None else 0, dy.shape[0], dy.shape[1], ACT_ALL[act], _p(out),
+                               _rowmajor(out, "out"), _stream()), "b2_act_bwd_f32")
+    return out
+
+
+def graphsc_block_degrees(A: CSR, dst: torch.Tensor, outdeg: Optional[torch.Tensor] = None, src_cap: int = 0):
+    """Out-degrees of the block whose destinations are ``dst`` (int32, −1 = padding) over the destination-indexed CSR ``A``.
+    Returns ``outdeg`` [n_nodes] int32, or with ``src_cap`` > 0 ``(outdeg, src_list [src_cap], src_pos [n_nodes])``: the block's
+    source nodes (first-touch order, −1 padded) and each one's slot."""
+    _chk(dst, torch.int32, "dst", 1)
+    n = A.shape[0]
+    dev = dst.device
+    outdeg = torch.empty(n, dtype=torch.int32, device=dev) if outdeg is None else outdeg
+    _chk(outdeg, torch.int32, "outdeg", 1)
+    if outdeg.numel() < n:
+        raise B2Error(f"graphsc_block_degrees: outdeg has {outdeg.numel()} entries, the graph {n} nodes")
+    lst = pos = cnt = None
+    if src_cap > 0:
+        lst = torch.empty(src_cap, dtype=torch.int32, device=dev)
+        pos = torch.empty(n, dtype=torch.int32, device=dev)
+        cnt = torch.empty(1, dtype=torch.int32, device=dev)
+    check(lib().b2_graphsc_block_degrees(_p(A.rowptr), _p(A.colidx), n, _p(dst), dst.numel(), _p(outdeg), _p(lst), _p(pos), _p(cnt),
+                                         int(src_cap), _stream()), "b2_graphsc_block_degrees")
+    return outdeg if src_cap <= 0 else (outdeg, lst, pos)
+
+
+def graphsc_block_aggregate(A: CSR, dst: torch.Tensor, outdeg: torch.Tensor, x: torch.Tensor, agg: str = "sum", p: float = 0.0,
+                            seed: int = 0, key: int = 0, x_pos: Optional[torch.Tensor] = None, transposed: bool = False,
+                            out_rows: int = 0, out: Optional[torch.Tensor] = None):
+    """WeightedGraphConv's normalised aggregation over a block (graphsc.py:445-477, before the product with W), with the
+    layer's input dropout (rows keyed by global node id).  ``transposed``: its adjoint, from [len(dst), F] to [out_rows, F]
+    rows ``x_pos[u]`` (or u).  See include/dance_b200.h."""
+    _chk(dst, torch.int32, "dst", 1)
+    _chk(outdeg, torch.int32, "outdeg", 1)
+    _chk(x, torch.float32, "x", 2)
+    if x_pos is not None:
+        _chk(x_pos, torch.int32, "x_pos", 1)
+    if agg not in ("sum", "mean"):
+        raise ValueError(f"agg must be 'sum' or 'mean', got {agg!r}")
+    F = x.shape[1]
+    rows = int(out_rows) if transposed else dst.numel()
+    if out is None:
+        out = torch.empty((rows, F), dtype=torch.float32, device=x.device)
+    _chk(out, torch.float32, "out", 2)
+    check(lib().b2_graphsc_block_aggregate_f32(_p(A.rowptr), _p(A.colidx), _p(A.vals), _p(dst), dst.numel(), _p(outdeg), _p(x),
+                                               _rowmajor(x, "x"), _p(x_pos), F, int(agg == "mean"), float(p), int(seed) & 0xFFFFFFFF,
+                                               int(key) & 0xFFFFFFFF, int(transposed), _p(out), _rowmajor(out, "out"),
+                                               out.shape[0] if transposed else 0, _stream()), "b2_graphsc_block_aggregate_f32")
+    return out
+
+
+def graphsc_batch_decoder(z: torch.Tensor, p: float = 0.1, seed: int = 0, key: int = 0, dz: Optional[torch.Tensor] = None,
+                          loss: Optional[torch.Tensor] = None):
+    """graph-sc's loss on one batch (graphsc.py:208-216 with InnerProductDecoder :408-411): ``norm · BCEWithLogits(z̃z̃ᵀ, I,
+    pos_weight)`` with the decoder's own dropout (rows = batch positions).  Returns (loss [1] on the device, dz)."""
+    _chk(z, torch.float32, "z", 2)
+    if dz is None:
+        dz = torch.empty_like(z)
+    if loss is None:
+        loss = torch.empty(1, dtype=torch.float32, device=z.device)
+    _chk(dz, torch.float32, "dz", 2)
+    _chk(loss, torch.float32, "loss")
+    check(lib().b2_graphsc_batch_decoder_f32(_p(z), _rowmajor(z, "z"), z.shape[0], z.shape[1], float(p), int(seed) & 0xFFFFFFFF,
+                                             int(key) & 0xFFFFFFFF, _p(dz), _rowmajor(dz, "dz"), _p(loss), _stream()),
+          "b2_graphsc_batch_decoder_f32")
+    return loss, dz
+
+
+def graphsc_scatter_rows(x: torch.Tensor, idx: torch.Tensor, out: torch.Tensor, offset: int = 0):
+    """``out[idx[i] − offset] = x[i]``."""
+    _chk(x, torch.float32, "x", 2)
+    _chk(idx, torch.int32, "idx", 1)
+    _chk(out, torch.float32, "out", 2)
+    check(lib().b2_graphsc_scatter_rows_f32(_p(x), _rowmajor(x, "x"), x.shape[0], x.shape[1], _p(idx), int(offset), _p(out),
+                                            _rowmajor(out, "out"), _stream()), "b2_graphsc_scatter_rows_f32")
+    return out

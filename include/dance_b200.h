@@ -34,11 +34,14 @@ extern "C" {
 #define B2_ERR_UNSUPPORTED (-3)
 #define B2_ERR_WORKSPACE (-4)
 
-/* activation codes shared by GEMM / SpMM epilogues */
+/* activation codes shared by GEMM / SpMM epilogues (NONE..TANH); LEAKY_RELU and GELU are taken by b2_act_f32 / b2_act_bwd_f32
+ * only (graph-sc's activations, graphsc.py:324-331) */
 #define B2_ACT_NONE 0
 #define B2_ACT_RELU 1
 #define B2_ACT_ELU 2
 #define B2_ACT_TANH 3
+#define B2_ACT_LEAKY_RELU 4 /* F.leaky_relu, negative slope 0.01 */
+#define B2_ACT_GELU 5       /* F.gelu, exact (erf) form */
 
 /* GEMM precision modes */
 #define B2_PREC_FP32_SIMT 0 /* CUDA-core FFMA, exact fp32 accumulate            */
@@ -631,6 +634,50 @@ int b2_subset_f32(const float* X, int64_t ldx, const int64_t* rows, const int32_
 int b2_cellwise_mask_u8(const float* X, int64_t ldx, int64_t n, int32_t g, float mask_rate, int32_t min_gene_counts,
                         int distr_exp, int add_test_mask, uint32_t seed, uint8_t* train, uint8_t* valid, uint8_t* test,
                         int32_t* overflow_rows, void* stream);
+
+/* ------------------------------------------------------------------------
+ * graph-sc (GraphSC) mini-batch training, graphsc.py:179-216 (fit), :355-411 (GCNAE, InnerProductDecoder), :428-484
+ * (WeightedGraphConv.forward).
+ *
+ * A block is a list of destination node ids `dst` [n_dst] (entries < 0 are padding, skipped) over the parent graph's
+ * destination-indexed CSR `rowptr` [n_nodes + 1] / `colidx` / `weights` (row v = sources of v's in-edges, edge weights;
+ * GraphLite.csr_by_destination()).  Its in-degree is the full row length (the full-neighbour sampler keeps every in-edge),
+ * its out-degree is per block.  No relabelled block CSR is built.
+ *
+ * Dropout: keep(seed, key, row, col) of common.cuh, as b2_dropout_f32 (so b2_dropout_f32 on a matrix of ones with the same
+ * seed and key materialises any mask).  Feature dropout rows are GLOBAL node ids; decoder rows are positions in the batch.
+ * GraphSCEngine's key layout: key = (step·2 + pass)·3 + site, step = mini-batch counter, pass 0 (embedding) | 1 (loss),
+ * site 0 = layer-1 input, 1 = layer-2 input, 2 = decoder.
+ *
+ *   b2_graphsc_block_degrees       : outdeg [n_nodes] ← per-source count of edges into dst (zeroed first).  With src_list
+ *       [src_cap] / src_pos [n_nodes] / n_src [1] (all or none): the block's source set, each source appended once in
+ *       first-touch order (src_pos[u] = its slot), unused slots -1.  src_cap must bound the sources (Σ row lengths does).
+ *   b2_graphsc_block_aggregate_f32 : transposed = 0: out[i, f] = s_v · Σ_{e: u→v} w_e · c_u · keep(u, f) · in[row(u), f] / (1 − p)
+ *       with v = dst[i], c_u = clamp(outdeg[u], 1)^-1/2, s_v = clamp(indeg_v, 1)^-1/2 (· 1/indeg_v when agg_mean),
+ *       row(u) = x_pos[u] (x_pos NULL: u), weights NULL = 1.  Padding slots give zero rows.
+ *       transposed = 1: the adjoint: out[row(u), f] = Σ over the same terms with in[i, f] (dout) in place of in[row(u), f];
+ *       out [out_rows, F] is zeroed first.  Order of the atomic sums is not fixed.
+ *   b2_graphsc_batch_decoder_f32   : z [B, d], 1 ≤ d ≤ 1024: z̃ = keep(row, col) ⊙ z / (1 − p), S = z̃z̃ᵀ, labels I,
+ *       pw = B − 1, norm = B / (2(B − 1)) (B = 1: pw = 0, norm = 1);  loss_out[0] = norm/B² · Σ [pw·y·softplus(−S) +
+ *       (1−y)·softplus(S)] (written, on the device), dz = keep ⊙ 2·(∂loss/∂S)·z̃ / (1 − p) (overwritten).
+ *   b2_act_f32                     : y = act(x), any B2_ACT_* code; in place allowed.
+ *   b2_act_bwd_f32                 : dx = dy ⊙ act'(·): from the output y for relu / elu / tanh / leaky_relu, from the
+ *       pre-activation x for gelu (the other may be NULL); in place allowed.
+ *   b2_graphsc_scatter_rows_f32    : out[idx[i] − offset, :] = x[i, :] (recorded embeddings in cell order).
+ * ---------------------------------------------------------------------- */
+int b2_graphsc_block_degrees(const int32_t* rowptr, const int32_t* colidx, int32_t n_nodes, const int32_t* dst, int32_t n_dst,
+                             int32_t* outdeg, int32_t* src_list, int32_t* src_pos, int32_t* n_src, int32_t src_cap, void* stream);
+int b2_graphsc_block_aggregate_f32(const int32_t* rowptr, const int32_t* colidx, const float* weights, const int32_t* dst,
+                                   int32_t n_dst, const int32_t* outdeg, const float* in, int64_t ldin, const int32_t* x_pos,
+                                   int32_t F, int agg_mean, float p, uint32_t seed, uint32_t key, int transposed, float* out,
+                                   int64_t ldout, int64_t out_rows, void* stream);
+int b2_graphsc_batch_decoder_f32(const float* z, int64_t ldz, int32_t B, int32_t d, float p, uint32_t seed, uint32_t key,
+                                 float* dz, int64_t lddz, float* loss_out, void* stream);
+int b2_act_f32(const float* x, int64_t ldx, int64_t rows, int32_t cols, int act, float* y, int64_t ldy, void* stream);
+int b2_act_bwd_f32(const float* dy, int64_t lddy, const float* y, int64_t ldy, const float* x, int64_t ldx, int64_t rows,
+                   int32_t cols, int act, float* dx, int64_t lddx, void* stream);
+int b2_graphsc_scatter_rows_f32(const float* x, int64_t ldx, int32_t rows, int32_t cols, const int32_t* idx, int32_t offset,
+                                float* out, int64_t ldo, void* stream);
 
 #ifdef __cplusplus
 }

@@ -261,7 +261,9 @@ extern "C" int b2_graphsc_block_aggregate_f32(const int32_t* rowptr, const int32
   B2_REQUIRE(transposed == 0 || transposed == 1, "b2_graphsc_block_aggregate_f32: transposed must be 0 or 1");
   B2_REQUIRE(!transposed || out_rows > 0, "b2_graphsc_block_aggregate_f32: the transposed form needs out_rows > 0");
   cudaStream_t st = as_stream(stream);
-  if (transposed) B2_CHECK_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * (size_t)((out_rows - 1) * ldout + F), st));
+  // the [out_rows, F] block only: the columns past F of a row-padded `out` belong to the caller
+  if (transposed)
+    B2_CHECK_CUDA(cudaMemset2DAsync(out, sizeof(float) * (size_t)ldout, 0, sizeof(float) * (size_t)F, (size_t)out_rows, st));
   if (n_dst == 0) return B2_OK;
   AggArgs a{rowptr, colidx, dst, outdeg, x_pos, weights, in, ldin, out, ldout, n_dst, F, agg_mean, p, 1.f / (1.f - p), seed, key};
   const dim3 grid((unsigned)ceil_div<int64_t>((int64_t)n_dst * 32, 256), (unsigned)ceil_div(F, 128));

@@ -713,19 +713,25 @@ class GraphSCEngine:
             self.z = torch.zeros(n_cells, self.emb_dim, dtype=torch.float32, device=self.device)
         nb = (order.numel() + batch_size - 1) // batch_size
         self.losses = torch.empty(nb, dtype=torch.float32, device=self.device)
-        indptr, A = graph["indptr_host"], graph["A"]
         for b in range(nb):
-            dst = order_dev[b * batch_size:(b + 1) * batch_size]
-            blk = dict(A=A, X=graph["X"], dst=dst, cell_offset=graph["cell_offset"], src=None, pos=None)
-            if self.n_layers == 1:
-                blk["deg"] = [ops.graphsc_block_degrees(A, dst)]
-            else:
-                ids = order[b * batch_size:(b + 1) * batch_size].numpy()
-                cap = int(min(A.shape[0], (indptr[ids + 1] - indptr[ids]).sum()))       # Σ row lengths bounds the sources
-                deg2, src, pos = ops.graphsc_block_degrees(A, dst, src_cap=cap)
-                blk.update(src=src, pos=pos, deg=[ops.graphsc_block_degrees(A, src), deg2])
-            self.train_batch(blk, lr, self.losses[b:b + 1])
+            sl = slice(b * batch_size, (b + 1) * batch_size)
+            self.train_batch(self.block(graph, order[sl], order_dev[sl]), lr, self.losses[b:b + 1])
         return self.losses
+
+    def block(self, graph: dict, ids_host, ids_dev: torch.Tensor) -> dict:
+        """The block of the mini-batch whose cells are the global node ids ``ids_host`` (host) / ``ids_dev`` (int32, device), as
+        :meth:`train_batch` takes it: the destination list and its out-degrees, and for two layers the source list, each
+        source's slot in it and layer 1's out-degrees.  ``graph`` comes from :func:`prepare_graph`; nothing here synchronises."""
+        A = graph["A"]
+        blk = dict(A=A, X=graph["X"], dst=ids_dev, cell_offset=graph["cell_offset"], src=None, pos=None)
+        if self.n_layers == 1:
+            blk["deg"] = [ops.graphsc_block_degrees(A, ids_dev)]
+        else:
+            indptr, ids = graph["indptr_host"], np.asarray(ids_host)
+            cap = int(min(A.shape[0], (indptr[ids + 1] - indptr[ids]).sum()))       # Σ row lengths bounds the sources
+            deg2, src, pos = ops.graphsc_block_degrees(A, ids_dev, src_cap=cap)
+            blk.update(src=src, pos=pos, deg=[ops.graphsc_block_degrees(A, src), deg2])
+        return blk
 
 
 def prepare_graph(graph, device="cuda") -> dict:

@@ -166,12 +166,11 @@ class NativeComm:
         self._ops, self._C = ops, C
         self.rank, self.world, self.enabled = rank, world, world > 1
         self._handle = C.c_void_p()
-        lib = ops.lib()
-        if not lib.b2_comm_available():
+        if not ops.lib().b2_comm_available():
             raise RuntimeError("NativeComm: libnccl.so.2 could not be loaded")
         buf = (C.c_char * 128)()
         if rank == 0:
-            ops.check(lib.b2_comm_unique_id(buf), "b2_comm_unique_id")
+            ops._call("b2_comm_unique_id", buf)
         raw = bytes(buf)
         if world > 1:
             if exchange is None:
@@ -183,26 +182,30 @@ class NativeComm:
                     return bytes(t.cpu().numpy().tobytes())
             raw = exchange(raw)
         idbuf = (C.c_char * 128).from_buffer_copy(raw)
-        ops.check(lib.b2_comm_init_rank(C.byref(self._handle), idbuf, world, rank), "b2_comm_init_rank")
+        ops._call("b2_comm_init_rank", C.byref(self._handle), idbuf, world, rank)
 
     def close(self):
         if self._handle:
-            self._ops.lib().b2_comm_destroy(self._handle)
+            self._ops._call("b2_comm_destroy", self._handle)
             self._handle = self._C.c_void_p()
+
+    def _allgather(self, local: torch.Tensor, full: torch.Tensor):
+        """full[world · local.numel()] ← every rank's ``local``, in rank order."""
+        ops, n = self._ops, local.numel()
+        ops._call("b2_allgather_f32", self._handle, ops._arg(local, "local", torch.float32, n),
+                  ops._arg(full, "full", torch.float32, self.world * n), n, ops._stream())
 
     def allreduce_sum_(self, t: torch.Tensor) -> torch.Tensor:
         if self.enabled:
-            if t.dtype != torch.float32 or not t.is_contiguous():
-                raise ValueError("NativeComm.allreduce_sum_: contiguous float32 tensor required")
-            self._ops.check(self._ops.lib().b2_allreduce_sum_f32(self._handle, t.data_ptr(), t.numel(), self._ops._stream()), "b2_allreduce_sum_f32")
+            ops = self._ops
+            ops._call("b2_allreduce_sum_f32", self._handle, ops._arg(t, "t", torch.float32), t.numel(), ops._stream())
         return t
 
     def allreduce_max_(self, t: torch.Tensor) -> torch.Tensor:
         """max over ranks of a small non-negative vector, via gather + local max (timing bookkeeping only)."""
         if self.enabled:
             full = torch.empty(self.world * t.numel(), dtype=torch.float32, device=t.device)
-            self._ops.check(self._ops.lib().b2_allgather_f32(self._handle, t.contiguous().data_ptr(), full.data_ptr(), t.numel(),
-                                                             self._ops._stream()), "b2_allgather_f32")
+            self._allgather(t.contiguous(), full)
             t.copy_(full.view(self.world, -1).max(0).values.view_as(t))
         return t
 
@@ -214,15 +217,13 @@ class NativeComm:
             out = torch.empty((n_total, F), dtype=local.dtype, device=local.device)
         sizes = [b - a for a, b in bounds]
         mx = max(sizes)
-        lib = self._ops.lib()
         if len(set(sizes)) == 1:
-            self._ops.check(lib.b2_allgather_f32(self._handle, local.contiguous().data_ptr(), out.data_ptr(), mx * F, self._ops._stream()),
-                            "b2_allgather_f32")
+            self._allgather(local.contiguous(), out)
             return out
         pad = torch.zeros((mx, F), dtype=local.dtype, device=local.device)
         pad[:local.shape[0]] = local
         buf = torch.empty((self.world * mx, F), dtype=local.dtype, device=local.device)
-        self._ops.check(lib.b2_allgather_f32(self._handle, pad.data_ptr(), buf.data_ptr(), mx * F, self._ops._stream()), "b2_allgather_f32")
+        self._allgather(pad, buf)
         for r, (a, b) in enumerate(bounds):
             out[a:b] = buf[r * mx:r * mx + (b - a)]
         return out

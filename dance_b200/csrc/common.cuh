@@ -99,4 +99,28 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   }
 }
 
+// apply_act extended by leaky_relu and gelu, the codes the GEMM / SpMM / GAT-combine epilogues do not take (their code stays as
+// it is).
+__device__ __forceinline__ float act_value(float v, int act) {
+  switch (act) {
+    case B2_ACT_LEAKY_RELU: return v > 0.f ? v : 0.01f * v;
+    case B2_ACT_GELU: return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
+    default: return apply_act(v, act);
+  }
+}
+
+// dy · act'(·) for every B2_ACT_* code: from the output *y for relu, elu, tanh and leaky_relu (y > 0 exactly where x > 0), from
+// the pre-activation *x for gelu.  Only the operand the code needs is read, so the other may point anywhere (NONE reads neither).
+// relu selects rather than multiplies, as torch's threshold_backward does: 0 wherever y <= 0, whatever dy is.
+__device__ __forceinline__ float act_bwd(float dy, const float* y, const float* x, int act) {
+  switch (act) {
+    case B2_ACT_RELU: return *y > 0.f ? dy : 0.f;
+    case B2_ACT_ELU: { const float v = *y; return dy * (v > 0.f ? 1.f : v + 1.f); }
+    case B2_ACT_TANH: { const float v = *y; return dy * (1.f - v * v); }
+    case B2_ACT_LEAKY_RELU: return dy * (*y > 0.f ? 1.f : 0.01f);
+    case B2_ACT_GELU: { const float v = *x; return dy * (normcdff(v) + v * 0.39894228040143268f * __expf(-0.5f * v * v)); }
+    default: return dy;
+  }
+}
+
 }  // namespace b2

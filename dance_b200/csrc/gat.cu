@@ -441,13 +441,6 @@ gat_combine_fwd_kernel(const float* __restrict__ agg, int64_t lda, const float* 
   }
 }
 
-__device__ __forceinline__ float combine_act_bwd(float g, const float* __restrict__ o, int act) {
-  if (act == B2_ACT_ELU) { const float v = *o; g *= (v > 0.f ? 1.f : v + 1.f); }
-  else if (act == B2_ACT_RELU) { g = *o > 0.f ? g : 0.f; }
-  else if (act == B2_ACT_TANH) { const float v = *o; g *= (1.f - v * v); }
-  return g;
-}
-
 // d(pre-combine)[n, nh*F] and d(pre-activation)[n, OW] (the latter feeds the bias gradient)
 __global__ void __launch_bounds__(256)
 gat_combine_bwd_kernel(const float* __restrict__ dout, int64_t lddo, const float* __restrict__ out, int64_t ldo,
@@ -458,7 +451,7 @@ gat_combine_bwd_kernel(const float* __restrict__ dout, int64_t lddo, const float
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t i = t / OW;
     const int c = (int)(t % OW);
-    const float g = combine_act_bwd(dout[i * lddo + c], out + i * ldo + c, act);
+    const float g = act_bwd(dout[i * lddo + c], out + i * ldo + c, nullptr, act);
     if (dact) dact[i * ldact + c] = g;
     if (concat) dpre[i * ldp + c] = g;
     else for (int h = 0; h < nh; ++h) dpre[i * ldp + h * F + c] = g / (float)nh;
@@ -479,13 +472,13 @@ gat_combine_bwd_identity_kernel(const float* __restrict__ dout, int64_t lddo, co
     if (concat) {
       for (int h = 0; h < nh; ++h) {
         const int c = h * F + f;
-        const float g = combine_act_bwd(dout[i * lddo + c], out + i * ldo + c, act);
+        const float g = act_bwd(dout[i * lddo + c], out + i * ldo + c, nullptr, act);
         if (dact) dact[i * ldact + c] = g;
         dpre[i * ldp + c] = g;
         sum += g;
       }
     } else {
-      const float g = combine_act_bwd(dout[i * lddo + f], out + i * ldo + f, act);
+      const float g = act_bwd(dout[i * lddo + f], out + i * ldo + f, nullptr, act);
       if (dact) dact[i * ldact + f] = g;
       const float gh = g / (float)nh;
       for (int h = 0; h < nh; ++h) { dpre[i * ldp + h * F + f] = gh; sum += gh; }
@@ -609,6 +602,7 @@ extern "C" int b2_gat_combine_fwd_f32(const float* agg, int64_t ldagg, const flo
                                       int32_t n, int32_t nheads, int32_t F, int concat, int act, int identity_skip, float* out,
                                       int64_t ldo, void* stream) {
   B2_REQUIRE(n >= 0 && nheads > 0 && F > 0, "b2_gat_combine_fwd_f32: bad arguments");
+  B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_TANH, "b2_gat_combine_fwd_f32: activation %d is not an epilogue code", act);
   B2_REQUIRE(!identity_skip || ldskip >= F, "b2_gat_combine_fwd_f32: an identity skip needs ldskip >= F");
   if (n == 0) return B2_OK;
   B2_REQUIRE(agg && out && (skip || !identity_skip), "b2_gat_combine_fwd_f32: null pointer");
@@ -623,6 +617,7 @@ extern "C" int b2_gat_combine_bwd_f32(const float* dout, int64_t lddo, const flo
                                       int32_t nheads, int32_t F, int concat, int act, float* dpre, int64_t ldp, float* dact,
                                       int64_t ldact, float* dx_skip, int64_t ldx, void* stream) {
   B2_REQUIRE(n >= 0 && nheads > 0 && F > 0, "b2_gat_combine_bwd_f32: bad arguments");
+  B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_TANH, "b2_gat_combine_bwd_f32: activation %d is not an epilogue code", act);
   B2_REQUIRE(!dx_skip || ldx >= F, "b2_gat_combine_bwd_f32: dx_skip needs ldx >= F");
   if (n == 0) return B2_OK;
   B2_REQUIRE(dout && out && dpre, "b2_gat_combine_bwd_f32: null pointer");

@@ -163,48 +163,7 @@ batch_decoder_kernel(const float* __restrict__ z, int64_t ldz, int B, int d, flo
   }
 }
 
-// ---- activations, scatter -----------------------------------------------------------------------------------------------------
-// leaky_relu and gelu are applied here rather than in the GEMM / SpMM epilogues, whose code stays as it is.
-__device__ __forceinline__ float act_value(float v, int act) {
-  switch (act) {
-    case B2_ACT_LEAKY_RELU: return v > 0.f ? v : 0.01f * v;
-    case B2_ACT_GELU: return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));
-    default: return apply_act(v, act);
-  }
-}
-// d act / d x from the output y (relu, elu, tanh, leaky_relu: y > 0 exactly where x > 0) or, for gelu, the input x.
-__device__ __forceinline__ float act_grad(float y, float x, int act) {
-  switch (act) {
-    case B2_ACT_RELU: return y > 0.f ? 1.f : 0.f;
-    case B2_ACT_ELU: return y > 0.f ? 1.f : y + 1.f;
-    case B2_ACT_TANH: return 1.f - y * y;
-    case B2_ACT_LEAKY_RELU: return y > 0.f ? 1.f : 0.01f;
-    case B2_ACT_GELU: return normcdff(x) + x * 0.39894228040143268f * __expf(-0.5f * x * x);
-    default: return 1.f;
-  }
-}
-
-__global__ void __launch_bounds__(256)
-act_fwd_kernel(const float* __restrict__ x, int64_t ldx, int64_t rows, int32_t cols, int act, float* y, int64_t ldy) {
-  const int64_t total = rows * cols;
-  for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t r = q / cols;
-    const int c = (int)(q % cols);
-    y[r * ldy + c] = act_value(x[r * ldx + c], act);
-  }
-}
-
-__global__ void __launch_bounds__(256)
-act_bwd_kernel(const float* __restrict__ dy, int64_t lddy, const float* __restrict__ y, int64_t ldy, const float* __restrict__ x,
-               int64_t ldx, int64_t rows, int32_t cols, int act, float* dx, int64_t lddx) {
-  const int64_t total = rows * cols;
-  for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t r = q / cols;
-    const int c = (int)(q % cols);
-    dx[r * lddx + c] = dy[r * lddy + c] * act_grad(y ? y[r * ldy + c] : 0.f, x ? x[r * ldx + c] : 0.f, act);
-  }
-}
-
+// ---- scatter -------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 scatter_rows_kernel(const float* __restrict__ x, int64_t ldx, int32_t rows, int32_t cols, const int32_t* __restrict__ idx,
                     int32_t offset, float* out, int64_t ldo) {
@@ -288,29 +247,6 @@ extern "C" int b2_graphsc_batch_decoder_f32(const float* z, int64_t ldz, int32_t
   batch_decoder_kernel<<<ceil_div(B, DEC_TI), DEC_THREADS, sizeof(float) * DEC_TI * d, st>>>(z, ldz, B, d, p, 1.f / (1.f - p), seed,
                                                                                             key, pw, coef, dz, lddz, loss_out);
   B2_CHECK_LAUNCH("batch_decoder_kernel");
-  return B2_OK;
-}
-
-extern "C" int b2_act_f32(const float* x, int64_t ldx, int64_t rows, int32_t cols, int act, float* y, int64_t ldy, void* stream) {
-  B2_REQUIRE(rows >= 0 && cols >= 0 && ldx >= cols && ldy >= cols, "b2_act_f32: bad shape");
-  B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_GELU, "b2_act_f32: unknown activation %d", act);
-  if (rows == 0 || cols == 0) return B2_OK;
-  B2_REQUIRE(x && y, "b2_act_f32: null pointer");
-  act_fwd_kernel<<<grid_for(rows * cols), 256, 0, as_stream(stream)>>>(x, ldx, rows, cols, act, y, ldy);
-  B2_CHECK_LAUNCH("act_fwd_kernel");
-  return B2_OK;
-}
-
-extern "C" int b2_act_bwd_f32(const float* dy, int64_t lddy, const float* y, int64_t ldy, const float* x, int64_t ldx, int64_t rows,
-                              int32_t cols, int act, float* dx, int64_t lddx, void* stream) {
-  B2_REQUIRE(rows >= 0 && cols >= 0 && lddy >= cols && lddx >= cols, "b2_act_bwd_f32: bad shape");
-  B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_GELU, "b2_act_bwd_f32: unknown activation %d", act);
-  if (rows == 0 || cols == 0) return B2_OK;
-  B2_REQUIRE(dy && dx, "b2_act_bwd_f32: null pointer");
-  if (act == B2_ACT_GELU) B2_REQUIRE(x && ldx >= cols, "b2_act_bwd_f32: gelu needs the pre-activation x");
-  else if (act != B2_ACT_NONE) B2_REQUIRE(y && ldy >= cols, "b2_act_bwd_f32: activation %d needs the output y", act);
-  act_bwd_kernel<<<grid_for(rows * cols), 256, 0, as_stream(stream)>>>(dy, lddy, y, ldy, x, ldx, rows, cols, act, dx, lddx);
-  B2_CHECK_LAUNCH("act_bwd_kernel");
   return B2_OK;
 }
 

@@ -1,4 +1,4 @@
-// Adam update + small elementwise kernels of the Graph-AE / Feature-AE training steps.
+// Adam update, gradient clipping and small elementwise kernels of the training steps (reparameterisation, activations).
 #include "common.cuh"
 
 namespace b2 {
@@ -31,10 +31,31 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restric
   }
 }
 
+// Standalone activation forward / backward over strided [rows, cols] matrices, for every B2_ACT_* code (act_value / act_bwd of
+// common.cuh).
 __global__ void __launch_bounds__(256)
-relu_bwd_kernel(const float* __restrict__ grad, const float* __restrict__ y, float* __restrict__ out, int64_t n) {
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    out[i] = y[i] > 0.f ? grad[i] : 0.f;
+act_fwd_kernel(const float* __restrict__ x, int64_t ldx, int64_t rows, int32_t cols, int act, float* y, int64_t ldy) {
+  const int64_t total = rows * cols;
+  for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = q / cols;
+    const int c = (int)(q % cols);
+    y[r * ldy + c] = act_value(x[r * ldx + c], act);
+  }
+}
+
+__global__ void __launch_bounds__(256)
+act_bwd_kernel(const float* __restrict__ dy, int64_t lddy, const float* __restrict__ y, int64_t ldy, const float* __restrict__ x,
+               int64_t ldx, int64_t rows, int32_t cols, int act, float* dx, int64_t lddx) {
+  // grid-stride over the rows·cols elements, stepping (row, column) by the stride's quotient and remainder: no 64-bit division
+  // per element
+  const int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (int64_t)gridDim.x * blockDim.x;
+  const int64_t dr = stride / cols, dc = stride % cols;
+  for (int64_t r = q / cols, c = q % cols; r < rows;) {
+    dx[r * lddx + c] = act_bwd(dy[r * lddy + c], y + r * ldy + c, x + r * ldx + c, act);
+    r += dr;
+    c += dc;
+    if (c >= cols) { c -= cols; ++r; }
+  }
 }
 
 __global__ void __launch_bounds__(256)
@@ -124,11 +145,26 @@ extern "C" int b2_adam_step_f32(float* param, const float* grad, float* exp_avg,
   return B2_OK;
 }
 
-extern "C" int b2_relu_bwd_f32(const float* grad, const float* y, float* out, int64_t n, void* stream) {
-  B2_REQUIRE(grad && y && out && n >= 0, "b2_relu_bwd_f32: bad arguments");
-  if (n == 0) return B2_OK;
-  relu_bwd_kernel<<<ew_grid(n), 256, 0, as_stream(stream)>>>(grad, y, out, n);
-  B2_CHECK_LAUNCH("relu_bwd_kernel");
+extern "C" int b2_act_f32(const float* x, int64_t ldx, int64_t rows, int32_t cols, int act, float* y, int64_t ldy, void* stream) {
+  B2_REQUIRE(rows >= 0 && cols >= 0 && ldx >= cols && ldy >= cols, "b2_act_f32: bad shape");
+  B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_GELU, "b2_act_f32: unknown activation %d", act);
+  if (rows == 0 || cols == 0) return B2_OK;
+  B2_REQUIRE(x && y, "b2_act_f32: null pointer");
+  act_fwd_kernel<<<ew_grid(rows * cols, 1), 256, 0, as_stream(stream)>>>(x, ldx, rows, cols, act, y, ldy);
+  B2_CHECK_LAUNCH("act_fwd_kernel");
+  return B2_OK;
+}
+
+extern "C" int b2_act_bwd_f32(const float* dy, int64_t lddy, const float* y, int64_t ldy, const float* x, int64_t ldx, int64_t rows,
+                              int32_t cols, int act, float* dx, int64_t lddx, void* stream) {
+  B2_REQUIRE(rows >= 0 && cols >= 0 && lddy >= cols && lddx >= cols, "b2_act_bwd_f32: bad shape");
+  B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_GELU, "b2_act_bwd_f32: unknown activation %d", act);
+  if (rows == 0 || cols == 0) return B2_OK;
+  B2_REQUIRE(dy && dx, "b2_act_bwd_f32: null pointer");
+  if (act == B2_ACT_GELU) B2_REQUIRE(x && ldx >= cols, "b2_act_bwd_f32: gelu needs the pre-activation x");
+  else if (act != B2_ACT_NONE) B2_REQUIRE(y && ldy >= cols, "b2_act_bwd_f32: activation %d needs the output y", act);
+  act_bwd_kernel<<<ew_grid(rows * cols, 1), 256, 0, as_stream(stream)>>>(dy, lddy, y, ldy, x, ldx, rows, cols, act, dx, lddx);
+  B2_CHECK_LAUNCH("act_bwd_kernel");
   return B2_OK;
 }
 

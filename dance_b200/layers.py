@@ -82,15 +82,7 @@ class GraphConvLayer:
 
     def backward(self, dout: torch.Tensor, need_input_grad: bool = True) -> Optional[torch.Tensor]:
         """Accumulates nothing: ``grad_weight`` / ``grad_bias`` are overwritten; returns d(feat) or None."""
-        act = self.activation
-        if act in ("relu", ):
-            dpre = ops.relu_bwd(dout, self._out)
-        elif act in ("tanh", "elu"):
-            dpre, _ = ops.gat_combine_bwd(dout, self._out, 1, self.out_feats, True, act=act)
-        elif act is None:
-            dpre = dout
-        else:
-            raise NotImplementedError(act)
+        dpre = dout if self.activation is None else ops.act_bwd(dout, self.activation, y=self._out)
         if self.bias is not None:
             ops.colsum(dpre, out=self.grad_bias)
         if self.weight_first:
@@ -149,12 +141,7 @@ class AdjLinearLayer:
     __call__ = forward
 
     def backward(self, dout: torch.Tensor, need_input_grad: bool = True) -> Optional[torch.Tensor]:
-        if self._act == "relu":
-            dpre = ops.relu_bwd(dout, self._out)
-        elif self._act is None:
-            dpre = dout
-        else:
-            dpre, _ = ops.gat_combine_bwd(dout, self._out, 1, self.out_features, True, act=self._act)
+        dpre = dout if self._act is None else ops.act_bwd(dout, self._act, y=self._out)
         if self.bias is not None:
             ops.colsum(dpre, out=self.grad_bias)
         ds = ops.spmm(self._AT, dpre)
@@ -208,12 +195,7 @@ class TAGConvLayer:
     __call__ = forward
 
     def backward(self, dout: torch.Tensor, need_input_grad: bool = True) -> Optional[torch.Tensor]:
-        if self.activation == "relu":
-            dpre = ops.relu_bwd(dout, self._out)
-        elif self.activation is None:
-            dpre = dout
-        else:
-            dpre, _ = ops.gat_combine_bwd(dout, self._out, 1, self.out_feats, True, act=self.activation)
+        dpre = dout if self.activation is None else ops.act_bwd(dout, self.activation, y=self._out)
         if self.bias is not None:
             ops.colsum(dpre, out=self.grad_bias)
         ops.gemm(dpre, self._stack, transA=True, out=self.grad_weight, precision=self.precision)

@@ -328,7 +328,7 @@ class GraphSCI:
             dh = ops.gemm(dpre, P[f"aemodel.{lin}.weight"], precision=pr)          # gradient w.r.t. the block's (dropped-out) input
             if bd["m"] is not None:
                 dh = dh * bd["m"]
-        dpre0 = ops.relu_bwd(dh, ac["h0"])                                           # ReLU of the multiply layer
+        dpre0 = ops.act_bwd(dh, "relu", y=ac["h0"])                                    # ReLU of the multiply layer
         ops.colsum(dpre0, out=Gd["aemodel.mul_layer.bias"])
         dzf = ops.gemm(ac["X_d"], dpre0, transA=True, precision=pr)                       # [G, G]
         ops.gemm(dzf, z, transA=True, out=Gd["aemodel.mul_layer.fc_layer.weight"], precision=pr)
@@ -352,13 +352,13 @@ class GraphSCI:
             ops.colsum(dls, out=Gd["gnnmodel.dec_mean.bias"], accumulate=True)
             dh2 = ops.spmm(self.AnT, ops.gemm(dmu, Wm, transB=True, precision=pr)) * gc["m2a"]
             dh2.add_(ops.spmm(self.AnT, ops.gemm(dls, Wm, transB=True, precision=pr)) * gc["m2b"])
-        dpre2 = ops.relu_bwd(dh2, gc["h2"])
+        dpre2 = ops.act_bwd(dh2, "relu", y=gc["h2"])
         ops.gemm(gc["S1"], dpre2, transA=True, out=Gd["gnnmodel.conv2.weight"], precision=pr)
         ops.colsum(dpre2, out=Gd["gnnmodel.conv2.bias"])
         dh1 = ops.spmm(self.AnT, ops.gemm(dpre2, P["gnnmodel.conv2.weight"], transB=True, precision=pr))
         if gc["m1"] is not None:
             dh1 = dh1 * gc["m1"]
-        dpre1, _ = ops.gat_combine_bwd(dh1, gc["h1"], 1, H1, True, act="tanh")
+        dpre1 = ops.act_bwd(dh1, "tanh", y=gc["h1"])
         ops.colsum(dpre1, out=Gd["gnnmodel.conv1.bias"])
         dP = ops.spmm(self.AnT, dpre1)
         ops.gemm(gc["f_d"], dP, transA=True, out=Gd["gnnmodel.conv1.weight"], precision=pr)

@@ -139,12 +139,12 @@ class Stagate:
         _, n, _, T, Tt, perm = self._graph
         P, G = self.params.p, self.params.g
         W1, W2 = P["conv1.lin_src"], P["conv2.lin_src"]
-        in_dim, hid, _ = self.dims
+        in_dim = self.dims[0]
         h2, h4, (H1, s_src, s_dst, alpha, h1, _, H3, h3) = self._forward(X, keep=True)
         loss_sum, dh4 = ops.mse_sum_loss_grad(h4, X)                                    # Σ(h4−X)², 2(h4−X); the mean's 1/(N·D) is applied at the clip
         ops.gemm(dh4, h3, transA=True, out=G["conv4.lin_src.T"], precision=self.precision)    # (h3ᵀ·dh4)ᵀ : conv4's own gradient, W1-shaped
         dh3 = ops.gemm(dh4, W1, precision=self.precision)
-        dagg3, _ = ops.gat_combine_bwd(dh3, h3, 1, hid, True, act="elu")
+        dagg3 = ops.act_bwd(dh3, "elu", y=h3)
         # Layer 3's message path (dH3 = Σ α dagg3) feeds h2 → h1 → dagg1, so it runs first as a plain SpMM on the transposed
         # CSR; dα sums both layers' contributions and is formed in the tied backward once dagg1 exists.
         Tta = ops.CSR(Tt.rowptr, Tt.colidx, alpha.view(-1)[perm.long()], Tt.shape)
@@ -153,7 +153,7 @@ class Stagate:
         dh2 = ops.gemm(dH3, W2, precision=self.precision)
         ops.gemm(h1, dh2, transA=True, out=G["conv2.lin_src"], precision=self.precision)
         dh1 = ops.gemm(dh2, W2, transB=True, precision=self.precision)
-        dagg1, _ = ops.gat_combine_bwd(dh1, h1, 1, hid, True, act="elu")
+        dagg1 = ops.act_bwd(dh1, "elu", y=h1)
         dH1, da_src, da_dst, _ = ops.gat_aggregate_bwd(T, Tt, perm, H1, P["conv1.att_src"], P["conv1.att_dst"], s_src, s_dst, alpha,
                                                        dagg1, 1, score_act="sigmoid", H2=H3, dOut2=dagg3, want_dH2=False)
         G["conv1.att_src"].copy_(da_src)

@@ -405,12 +405,21 @@ def adam_step(param, grad, exp_avg, exp_avg_sq, step: int, lr=1e-3, beta1=0.9, b
           _arg(exp_avg_sq, "exp_avg_sq", _F32, n), n, lr, beta1, beta2, eps, weight_decay, step, _stream())
 
 
-def relu_bwd(grad, y, out=None):
-    g = _arg(grad, "grad", _F32, None)
-    n = grad.numel()
-    if out is None:
-        out = torch.empty_like(grad)
-    _call("b2_relu_bwd_f32", g, _arg(y, "y", _F32, n), _arg(out, "out", _F32, n), n, _stream())
+def act(x, act: Optional[str], out=None):
+    """``act(x)`` elementwise, for the activations the GEMM epilogue does not take (leaky_relu, gelu) as well as the others."""
+    xp, ldx = _arg(x, "x", _F32, (None, None), ld=True)
+    out = torch.empty_like(x) if out is None else out
+    _call("b2_act_f32", xp, ldx, x.shape[0], x.shape[1], ACT_ALL[act], *_arg(out, "out", _F32, tuple(x.shape), ld=True), _stream())
+    return out
+
+
+def act_bwd(dy, act: Optional[str], y=None, x=None, out=None):
+    """``dy ⊙ act'``: from the output ``y`` for relu / elu / tanh / leaky_relu, from the pre-activation ``x`` for gelu."""
+    g, ldg = _arg(dy, "dy", _F32, (None, None), ld=True)
+    shape = tuple(dy.shape)
+    out = torch.empty_like(dy) if out is None else out
+    _call("b2_act_bwd_f32", g, ldg, *_arg(y, "y", _F32, shape, ld=True, optional=True), *_arg(x, "x", _F32, shape, ld=True, optional=True),
+          shape[0], shape[1], ACT_ALL[act], *_arg(out, "out", _F32, shape, ld=True), _stream())
     return out
 
 
@@ -1289,24 +1298,6 @@ def concat_normalized(left: torch.Tensor, right: torch.Tensor, base: Optional[to
 
 
 # ----------------------------------------------------------------------------- graph-sc mini-batch blocks (csrc/graphsc.cu)
-def act(x, act: Optional[str], out=None):
-    """``act(x)`` elementwise, for the activations the GEMM epilogue does not take (leaky_relu, gelu) as well as the others."""
-    xp, ldx = _arg(x, "x", _F32, (None, None), ld=True)
-    out = torch.empty_like(x) if out is None else out
-    _call("b2_act_f32", xp, ldx, x.shape[0], x.shape[1], ACT_ALL[act], *_arg(out, "out", _F32, tuple(x.shape), ld=True), _stream())
-    return out
-
-
-def act_bwd(dy, act: Optional[str], y=None, x=None, out=None):
-    """``dy ⊙ act'``: from the output ``y`` for relu / elu / tanh / leaky_relu, from the pre-activation ``x`` for gelu."""
-    g, ldg = _arg(dy, "dy", _F32, (None, None), ld=True)
-    shape = tuple(dy.shape)
-    out = torch.empty_like(dy) if out is None else out
-    _call("b2_act_bwd_f32", g, ldg, *_arg(y, "y", _F32, shape, ld=True, optional=True), *_arg(x, "x", _F32, shape, ld=True, optional=True),
-          shape[0], shape[1], ACT_ALL[act], *_arg(out, "out", _F32, shape, ld=True), _stream())
-    return out
-
-
 def graphsc_block_degrees(A: CSR, dst: torch.Tensor, outdeg: Optional[torch.Tensor] = None, src_cap: int = 0):
     """Out-degrees of the block whose destinations are ``dst`` (int32, −1 = padding) over the destination-indexed CSR ``A``.
     Returns ``outdeg`` [n_nodes] int32, or with ``src_cap`` > 0 ``(outdeg, src_list [src_cap], src_pos [n_nodes])``: the block's

@@ -208,9 +208,17 @@ int b2_clip_grad_norm_f32(float* grad, int64_t n, float pre_scale, float max_nor
 /* ------------------------------------------------------------------------
  * Elementwise helpers on the GCN path
  * ---------------------------------------------------------------------- */
-/* out = grad ⊙ (y > 0)   (backward of F.relu in GraphConvolution / Graph_AE, scgnn2.py:388,497-502, and of nn.ReLU in
- * graphsci.py:37-45,85-87; in-place allowed) */
-int b2_relu_bwd_f32(const float* grad, const float* y, float* out, int64_t n, void* stream);
+/* Standalone activations over strided [rows, cols] matrices, for every B2_ACT_* code (the activations the GEMM / SpMM
+ * epilogues do not take, and the backward of those they do):
+ *   b2_act_f32     : y = act(x); in place allowed.
+ *   b2_act_bwd_f32 : dx = dy ⊙ act'(·): from the output y for relu / elu / tanh / leaky_relu, from the pre-activation x for
+ *       gelu (the other may be NULL; NONE reads neither and copies dy); in place allowed.  relu is torch's threshold_backward,
+ *       dx = y > 0 ? dy : 0, so dx is +0 wherever y <= 0 whatever dy is.  The backward of the activation of the GCN layers
+ *       (GraphConvolution, scgnn2.py:497-502; dgl's GraphConv), of nn.ReLU / nn.Tanh in GraphSCI (graphsci.py:37-45,
+ *       68-87,111-112), of F.elu in STAGATE (stagate.py:191,197) and of graph-sc's activations (graphsc.py:324-331). */
+int b2_act_f32(const float* x, int64_t ldx, int64_t rows, int32_t cols, int act, float* y, int64_t ldy, void* stream);
+int b2_act_bwd_f32(const float* dy, int64_t lddy, const float* y, int64_t ldy, const float* x, int64_t ldx, int64_t rows,
+                   int32_t cols, int act, float* dx, int64_t lddx, void* stream);
 /* z = mu + eps ⊙ exp(logvar)  (Graph_AE.reparameterize, scgnn2.py:394-400); [n,d] with leading dims */
 int b2_reparam_fwd_f32(const float* mu, const float* logvar, int64_t ldm, const float* eps, int64_t lde,
                        float* z, int64_t ldz, int64_t n, int32_t d, void* stream);
@@ -344,6 +352,7 @@ int b2_gat_aggregate_bwd_f32(const int32_t* rowptr, const int32_t* colidx,
  *   concat: out[n, nheads*F] = act(agg + skip + bias) ; else out[n,F] = act(mean_h(agg + skip) + bias)
  *   skip may be NULL.  identity_skip != 0 (GATLayer with FIN == FOUT, scgnn2.py:1167-1171): skip is the raw input
  *   x [n, F] (required, ldskip >= F), added to every head as skip[n, h*F + f] = x[n, f].
+ *   act: B2_ACT_NONE..B2_ACT_TANH.
  *   Backward: dpre [n, nheads*F] = d(agg) = d(skip); dact [n, OW] (optional) is the gradient before the bias add (its column
  *   sums are the bias gradient); dx_skip NULL, or for an identity skip dx_skip[n, F] = Σ_h dpre[n, h*F:(h+1)*F] (overwritten,
  *   ldx >= F). */
@@ -660,9 +669,6 @@ int b2_cellwise_mask_u8(const float* X, int64_t ldx, int64_t n, int32_t g, float
  *   b2_graphsc_batch_decoder_f32   : z [B, d], 1 ≤ d ≤ 1024: z̃ = keep(row, col) ⊙ z / (1 − p), S = z̃z̃ᵀ, labels I,
  *       pw = B − 1, norm = B / (2(B − 1)) (B = 1: pw = 0, norm = 1);  loss_out[0] = norm/B² · Σ [pw·y·softplus(−S) +
  *       (1−y)·softplus(S)] (written, on the device), dz = keep ⊙ 2·(∂loss/∂S)·z̃ / (1 − p) (overwritten).
- *   b2_act_f32                     : y = act(x), any B2_ACT_* code; in place allowed.
- *   b2_act_bwd_f32                 : dx = dy ⊙ act'(·): from the output y for relu / elu / tanh / leaky_relu, from the
- *       pre-activation x for gelu (the other may be NULL); in place allowed.
  *   b2_graphsc_scatter_rows_f32    : out[idx[i] − offset, :] = x[i, :] (recorded embeddings in cell order).
  * ---------------------------------------------------------------------- */
 int b2_graphsc_block_degrees(const int32_t* rowptr, const int32_t* colidx, int32_t n_nodes, const int32_t* dst, int32_t n_dst,
@@ -673,9 +679,6 @@ int b2_graphsc_block_aggregate_f32(const int32_t* rowptr, const int32_t* colidx,
                                    int64_t ldout, int64_t out_rows, void* stream);
 int b2_graphsc_batch_decoder_f32(const float* z, int64_t ldz, int32_t B, int32_t d, float p, uint32_t seed, uint32_t key,
                                  float* dz, int64_t lddz, float* loss_out, void* stream);
-int b2_act_f32(const float* x, int64_t ldx, int64_t rows, int32_t cols, int act, float* y, int64_t ldy, void* stream);
-int b2_act_bwd_f32(const float* dy, int64_t lddy, const float* y, int64_t ldy, const float* x, int64_t ldx, int64_t rows,
-                   int32_t cols, int act, float* dx, int64_t lddx, void* stream);
 int b2_graphsc_scatter_rows_f32(const float* x, int64_t ldx, int32_t rows, int32_t cols, const int32_t* idx, int32_t offset,
                                 float* out, int64_t ldo, void* stream);
 

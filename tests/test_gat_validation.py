@@ -1,6 +1,6 @@
 """Argument validation of the GAT aggregate and combine entry points' options (no GPU needed): attention dropout, the tied
-second layer and the identity skip.  Every case is rejected before any CUDA call, so the stand-in pointers are never
-dereferenced."""
+second layer, the identity skip and the combine's activation code.  Every case is rejected before any CUDA call, so the
+stand-in pointers are never dereferenced."""
 import pytest
 
 INVALID = -1
@@ -41,6 +41,8 @@ CASES = [
     (CFWD, {"skip": None}),
     (CFWD, {"ldskip": F - 1}),
     (CBWD, {"ldx": F - 1}),
+    # the combine's activation is an epilogue code (NONE..TANH)
+    *[(fn, {"act": a}) for fn in (CFWD, CBWD) for a in (-1, 4, 5)],
 ]
 
 

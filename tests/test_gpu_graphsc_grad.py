@@ -4,7 +4,7 @@ GraphSC.fit (tests/test_gpu_graphsc.py) observes the engine only after Adam, who
 scale of each gradient.  Here GraphSCEngine.train_batch runs one batch with Adam replaced by a no-op, and its loss, its recorded
 embedding, every parameter gradient and the BatchNorm running statistics are compared with float64 autograd through
 tests/graphsc_ref.py (pinned to the reference's own fit by tests/test_graphsc_step_ref_cpu.py) across the layer configurations.
-Then each kernel of csrc/graphsc.cu is compared with a float64 restatement at its width, layout and degree edges: the block
+Then each kernel graph-sc runs is compared with a float64 restatement at its width, layout and degree edges: the block
 degrees and aggregate (hub rows, empty rows, padding, both feature slots and slices, strided operands), the fused batch decoder
 (many CTAs, padded leading dimensions, saturated logits), act / act_bwd for every code, and scatter_rows."""
 import numpy as np
@@ -416,6 +416,18 @@ def test_act_and_backward_vs_float64(cuda, act):
     lim = 1e-6 * xg.grad.abs() + 1e-6 * dy.double().abs()
     assert bool((err <= lim).all()), (act, float((err - lim).max()))
     assert _margins_intact(dxbuf, cols, left=4) and _margins_intact(dybuf, cols, left=2)
+
+    if act in ("relu", "leaky_relu"):
+        # where y <= 0, relu's gradient is torch's threshold_backward: exactly +0 for any dy, ±inf and NaN included;
+        # leaky_relu's is 0.01 · dy in float32
+        ys = torch.tensor([0.0, -0.0, -2.0], device=cuda).repeat_interleave(6).view(3, 6)
+        dys = torch.tensor([float("inf"), -float("inf"), float("nan"), -1.5, -1e-30, 2.0], device=cuda).repeat(3, 1)
+        dx = ops.act_bwd(dys, act, y=ys).cpu()
+        if act == "relu":
+            assert bool((dx.view(torch.int32) == 0).all()), dx
+        else:
+            ref = dys.cpu() * 0.01
+            assert torch.equal(dx.isnan(), ref.isnan()) and torch.equal(dx[~dx.isnan()], ref[~ref.isnan()]), (dx, ref)
 
 
 def test_scatter_rows_offset_permuted_strided(cuda):

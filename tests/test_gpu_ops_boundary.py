@@ -80,9 +80,6 @@ def _cases():
     def _(d): return (dict(param=r(10, dev=d), grad=r(10, dev=d), exp_avg=r(10, dev=d), exp_avg_sq=r(10, dev=d), step=1),
                       ["grad", "exp_avg", "exp_avg_sq"], ["param"])
 
-    @case("relu_bwd")
-    def _(d): return dict(grad=r(10, dev=d), y=r(10, dev=d), out=o(10, dev=d)), ["y", "out"], ["grad"]
-
     @case("reparam_fwd")
     def _(d): return (dict(mu=r(6, 8, dev=d), logvar=r(6, 8, dev=d), eps=r(6, 8, dev=d), out=o(6, 8, dev=d)),
                       ["logvar", "eps", "out"], ["mu"])

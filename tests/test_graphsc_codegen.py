@@ -3,7 +3,7 @@ import pytest
 
 from kernel_codegen import compiled, needs_nvcc
 
-KERNELS = ("block_degrees_kernel", "block_aggregate_kernel", "batch_decoder_kernel", "act_fwd_kernel", "act_bwd_kernel", "scatter_rows_kernel")
+KERNELS = ("block_degrees_kernel", "block_aggregate_kernel", "batch_decoder_kernel", "scatter_rows_kernel")
 
 
 @needs_nvcc

@@ -1,5 +1,6 @@
-"""Argument validation of the graph-sc entry points (no GPU needed): every case is rejected before any CUDA call, so it runs
-on a machine without a device and the stand-in pointers are never dereferenced."""
+"""Argument validation of the graph-sc entry points and of the activation pair b2_act_f32 / b2_act_bwd_f32 (no GPU needed):
+every case is rejected before any CUDA call, so it runs on a machine without a device and the stand-in pointers are never
+dereferenced."""
 import pytest
 
 INVALID = -1

@@ -32,8 +32,9 @@ KERNELS = {
     "gae_tc.cu": tuple(f"gae_{sweep}_tc_kernelILi{dp}E" for sweep in ("allpairs", "tri") for dp in (8, 16, 32)),
     "gemm_tc.cu": tuple(gemm_kernel(mode, bn) for mode, bn in GEMM),
     "gat.cu": ("gat_aggregate_fwd_kernelILb1E", "gat_bwd_target_kernelILb1E", "gat_bwd_source_kernelILb1E",
-               "gat_combine_fwd_kernelILb1E", "gat_combine_bwd_identity_kernel"),
+               "gat_combine_fwd_kernelILb1E", "gat_combine_bwd_kernel", "gat_combine_bwd_identity_kernel"),
     "dropout.cu": ("dropout_kernel",),
+    "optim.cu": ("act_fwd_kernel", "act_bwd_kernel"),
     "quantile.cu": ("radix_hist_kernelILi0", "radix_hist_kernelILi1", "radix_hist_kernelILi2", "radix_scan_kernelILi0",
                     "radix_scan_kernelILi1", "radix_scan_kernelILi2", "quantile_finish_kernel", "col_minmax_kernel",
                     "concat_kernelILb1", "concat_kernelILb0", "minmax_params_kernel"),

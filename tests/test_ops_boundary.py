@@ -101,7 +101,6 @@ CASES = {
     "gae_loss_grad": lambda: ops.gae_loss_grad(f32(6, 8), _fake_csr(vals=False), 1.0, 1.0),
     "gae_loss_grad_sym": lambda: ops.gae_loss_grad_sym(f32(6, 8), _fake_csr(vals=False), 1.0, 1.0, 0, 1),
     "adam_step": lambda: ops.adam_step(f32(4), f32(4), f32(4), f32(4), 1),
-    "relu_bwd": lambda: ops.relu_bwd(f32(4), f32(4)),
     "reparam_fwd": lambda: ops.reparam_fwd(f32(4, 8), f32(4, 8), f32(4, 8)),
     "reparam_bwd": lambda: ops.reparam_bwd(f32(4, 8), f32(4, 8), f32(4, 8), f32(4, 8), f32(4, 8)),
     "knn": lambda: ops.knn(f32(8, 4), 2),

@@ -34,8 +34,8 @@
 // fp16 A fragment (two columns packed per register), so its dZ_I takes G in the natural column order.  The full sweep's tf32
 // A fragment wants columns (t, t+4); the sum over j does not care about order, so the 8 columns of each block are fed to its
 // dZ MMA in the order (0, 2, 4, 6, 1, 3, 5, 7) and Z_Jᵀ is stored with its columns permuted the same way (zt_pos).  The
-// triangle's dZ_J reorders the sum over i likewise: rows r and r + 8 of a thread's fragment are put side by side in the K
-// order of Gᵀ and Z_Iᵀ (gt_pos), so that each thread writes its two Gᵀ values of a column with one 32-bit store per plane.
+// triangle's packed fp16 G is also the fragment stmatrix takes: each 8 x 8 block goes to the Gᵀ planes transposed
+// (stmatrix .trans, four blocks per instruction), so Gᵀ and Z_Iᵀ are K-major in the natural order of i.
 //
 // Work units: row blocks.  The row form covers [row_begin, row_begin + n_rows); the pair-sharded form (multi-GPU) takes
 // "super-blocks" s = {block s, block nb−1−s} (a lone middle block when nb is odd), so that super-block ranges split the work
@@ -93,8 +93,6 @@ struct Tiles {
 
 // position of column jj of a tile in the permuted order of the dZ MMA (see header)
 __host__ __device__ __forceinline__ int zt_pos(int jj) { const int q = jj & 7; return (jj & ~7) | ((q & 1) ? 4 + (q >> 1) : (q >> 1)); }
-// position of row i (0..63) of a warpgroup in the K order of the dZ_J MMA: rows r and r + 8 of a 16-row group become neighbours
-__host__ __device__ __forceinline__ int gt_pos(int i) { return (i & ~15) | ((i & 7) << 1) | ((i >> 3) & 1); }
 
 __device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 
@@ -216,38 +214,46 @@ __device__ __forceinline__ void mma_ss16(float (&d)[N / 2], uint64_t a, uint64_t
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t x) {
-  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(x) : "memory");
+// Four 8 x 8 b16 matrices in the mma fragment layout (register q of lane l: row l/4, columns 2·(l%4), +1 of matrix q) stored
+// transposed: lane l gives the address of row l % 8 of stored matrix l / 8, i.e. of column l % 8 of fragment matrix l / 8.
+__device__ __forceinline__ void stsm_x4_trans(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c),
+               "r"(d) : "memory");
 }
 
 // σ and softplus of one thread's logits S (the m64nJW accumulator), in place: S becomes the hi part of G = σ(S) and L its lo
 // part, ready to be the register A operand of the dZ product.  Returns the thread's share of Σ softplus.  MASKED zeroes G and
 // drops the loss of columns j ≥ n and of rows past the range (the last J tile, a partial I block); interior tiles skip the
 // per-logit mask and its selects.  F16 (the triangle): G·2^14 is split into fp16 hi / lo, packed two columns per register
-// (the f16 A fragment) into S[0 .. V/2) and L[0 .. V/2).
+// (the f16 A fragment) into S[0 .. V/2) and L[0 .. V/2).  The 2^14 rides in the reciprocal's argument, rcp(2^-14·(1+e)) =
+// 2^14 / (1+e) (power-of-two scaling is exact, so G·2^14 is what σ · 2^14 gave), and the product of the (1+e) is formed as
+// prod·e + prod in one FFMA; with the mask, a dropped logit multiplies by 1 + 0.  Both save an instruction per logit in the
+// consumers' serial σ / softplus phase; the MUFU count (ex2, rcp, one lg2 per 32) is the same.
 template <bool MASKED, int V, bool F16>
 __device__ __forceinline__ float sigmoid_softplus(float (&S)[V], float (&L)[V], int jbase, int n, bool live_a, bool live_b) {
-  constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f;
+  constexpr float LOG2E = 1.4426950408889634f, LN2 = 0.6931471805599453f, INV_G_SCALE = 1.f / 16384.f;
   float relu = 0.f, lg = 0.f, prod = 1.f;
 #pragma unroll
   for (int v = 0; v < V; ++v) {
     if ((v & 31) == 31) { lg += lg2_approx(prod); prod = 1.f; }
     const float x = S[v];
     const float e = ex2_approx(-fabsf(x) * LOG2E);
-    const float inv = rcp_approx(1.f + e);
+    const float inv = F16 ? rcp_approx(fmaf(e, INV_G_SCALE, INV_G_SCALE)) : rcp_approx(1.f + e);
     float sg = x >= 0.f ? inv : e * inv;
     if constexpr (MASKED) {
       const int j = jbase + 8 * (v >> 2) + (v & 1);
       const bool ok = j < n && (((v >> 1) & 1) ? live_b : live_a);
       relu += ok ? fmaxf(x, 0.f) : 0.f;
-      prod *= ok ? 1.f + e : 1.f;
+      if constexpr (F16) prod = fmaf(prod, ok ? e : 0.f, prod);
+      else prod *= ok ? 1.f + e : 1.f;
       sg = ok ? sg : 0.f;
     } else {
       relu += fmaxf(x, 0.f);
-      prod *= 1.f + e;
+      if constexpr (F16) prod = fmaf(prod, e, prod);
+      else prod *= 1.f + e;
     }
     if constexpr (F16) {
-      S[v] = sg * 16384.f;
+      S[v] = sg;
     } else {
       const float hi = tf32_trunc(sg);
       S[v] = hi;
@@ -341,15 +347,15 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
       // each warpgroup half of Z_I in its 64-row tile's scale; the half's sum is unscaled before the two are added
       const int e0 = p.exps[2 * blockIdx.x], e1 = p.exps[2 * blockIdx.x + 1];
       const float sc_i[2] = {unscale(e0), unscale(e1)};
-      // Z_Iᵀ (B of dZ_J) per consumer warpgroup: [DP hi rows | DP lo rows] x 64 i (fp16) in the gt_pos order, scaled by 2^e;
-      // rows past the range are zero
+      // Z_Iᵀ (B of dZ_J) per consumer warpgroup: [DP hi rows | DP lo rows] x 64 i (fp16), scaled by 2^e; rows past the range
+      // are zero
       for (int e = t; e < BT * DP; e += 128) {
         const int r = e / DP, k = e % DP;
         const int row = row0 + r;
         const float v = (row < row_end && k < p.d) ? p.z[(int64_t)row * p.ldz + k] : 0.f;
         const float x = ldexpf(v, (r >> 6) ? e1 : e0);
         const __half xh = __float2half_rn(x);
-        const uint32_t q = (uint32_t)gt_pos(r & 63);
+        const uint32_t q = (uint32_t)(r & 63);
         uint8_t* b = zit + (r >> 6) * T::ZIT;
         *reinterpret_cast<__half*>(b + sw128_offset16((uint32_t)k, q)) = xh;
         *reinterpret_cast<__half*>(b + sw128_offset16((uint32_t)(DP + k), q)) = __float2half_rn(x - __half2float(xh));
@@ -449,9 +455,12 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
   const bool live_a = ra < row_end, live_b = ra + 8 < row_end;
   const uint32_t ai_hi = smem_u32(zi_hi) + wg * 64 * 128, ai_lo = smem_u32(zi_lo) + wg * 64 * 128;
   const bool full_rows = row0 + BT <= row_end;                   // no dead rows in this block: only the last J tile is masked
-  // triangle: this warpgroup's Gᵀ planes (A of dZ_J)
-  uint8_t* gt_hi = zit + 2 * T::ZIT + wg * 2 * T::GT;
-  uint8_t* gt_lo = gt_hi + T::GT;
+  // triangle: this warpgroup's Gᵀ planes (A of dZ_J); the address this lane gives stmatrix in the hi plane is column
+  // 16·m + 8·(lane / 16) + lane % 8 of G (row j of Gᵀ, m = 0 .. 3 below), rows i from 16·warp + 8·((lane / 8) % 2) (the
+  // 16-byte chunk of 8 i in the 128-byte swizzle)
+  const uint32_t gt_hi = smem_u32(zit + 2 * T::ZIT + wg * 2 * T::GT) +
+                         sw128_offset16((uint32_t)(8 * (lane >> 4) + (lane & 7)), (uint32_t)(16 * warp + 8 * ((lane >> 3) & 1)));
+  const uint32_t gt_lo = gt_hi + T::GT;
   const float c2 = 2.f * p.coef;
 
   // The accumulation inside the tensor core truncates, and the hi·hi product carries almost all of dZ: over a whole J sweep one
@@ -566,20 +575,15 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
       if (i >= handed0) {
         loss += 2.0 * (double)l;   // a tile above the diagonal block stands for its mirror too
         mbar_wait(gt_empty + 8 * wg, (uint32_t)(((i - handed0) & 1) ^ 1));
-        // column jj of G is row jj of Gᵀ; the thread's rows r, r + 8 sit at K positions gt_pos(r), gt_pos(r) + 1
-        const uint32_t k = (uint32_t)gt_pos(warp * 16 + (lane >> 2));
-        // one 32-bit store per column and plane: (r, j) and (r + 8, j) from the two registers that hold column j
+        // column j of G is row j of Gᵀ.  The packed registers S[2c], S[2c + 1] (and L) are the fragments of the 8 x 8 blocks
+        // (rows r .. r + 7 and r + 8 .. r + 15 of the warp, columns 8c .. 8c + 7); stmatrix .trans writes four of them as rows
+        // of Gᵀ, K-major in the natural i order.
 #pragma unroll
-        for (int c = 0; c < JW / 8; ++c) {
-          const uint32_t h0 = __float_as_uint(S[2 * c]), h1 = __float_as_uint(S[2 * c + 1]);
-          const uint32_t l0 = __float_as_uint(L[2 * c]), l1 = __float_as_uint(L[2 * c + 1]);
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const uint32_t sel = e ? 0x7632u : 0x5410u;
-            const uint32_t o = sw128_offset16((uint32_t)(8 * c + 2 * (lane & 3) + e), k);
-            sts_u32(smem_u32(gt_hi) + o, __byte_perm(h0, h1, sel));
-            sts_u32(smem_u32(gt_lo) + o, __byte_perm(l0, l1, sel));
-          }
+        for (int m = 0; m < JW / 16; ++m) {
+          stsm_x4_trans(gt_hi + m * 16 * 128, __float_as_uint(S[4 * m]), __float_as_uint(S[4 * m + 1]),
+                        __float_as_uint(S[4 * m + 2]), __float_as_uint(S[4 * m + 3]));
+          stsm_x4_trans(gt_lo + m * 16 * 128, __float_as_uint(L[4 * m]), __float_as_uint(L[4 * m + 1]),
+                        __float_as_uint(L[4 * m + 2]), __float_as_uint(L[4 * m + 3]));
         }
         fence_proxy_async();
         __syncwarp();

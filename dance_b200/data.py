@@ -326,3 +326,10 @@ class Data:
 
     def get_y(self, split_name: Optional[str] = None, return_type: str = "numpy"):
         return self._get("label", split_name, return_type)
+
+    def get_data(self, split_name: Optional[str] = None, return_type: str = "numpy"):
+        """(features, labels) of a split (data/base.py get_data)."""
+        return self.get_x(split_name, return_type), self.get_y(split_name, return_type)
+
+    def get_train_data(self, return_type: str = "numpy"):
+        return self.get_data("train", return_type)

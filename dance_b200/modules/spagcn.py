@@ -22,6 +22,7 @@ import torch
 
 from .. import ops
 from ..engine import FlatParams
+from ..leiden import leiden, neighbor_graph
 
 
 def _dev(a, device, dtype=torch.float32) -> torch.Tensor:
@@ -199,20 +200,14 @@ class SimpleGCDEC:
     def _init_labels(self, features: torch.Tensor, X, init, n_clusters, n_neighbors, res, init_spa, init_labels):
         if init_labels is not None:
             return np.asarray(init_labels).astype(np.int64)
-        base = features.cpu().numpy() if init_spa else np.asarray(X, dtype=np.float32)
         if init == "kmeans":   # same third-party call as the reference (:471-480); initialisation only, not the hot path
+            base = features.cpu().numpy() if init_spa else np.asarray(X, dtype=np.float32)
             from sklearn.cluster import KMeans
             return KMeans(int(n_clusters), n_init=20).fit_predict(base).astype(np.int64)
-        if init == "louvain":
-            try:
-                import scanpy as sc
-            except ImportError as e:
-                raise NotImplementedError("init='louvain' needs scanpy (neighbors + leiden, spagcn.py:481-492); "
-                                          "pass init='kmeans' or init_labels=") from e
-            adata = sc.AnnData(base)
-            sc.pp.neighbors(adata, n_neighbors=n_neighbors, use_rep="X")
-            sc.tl.leiden(adata, resolution=res, key_added="louvain")
-            return adata.obs["louvain"].astype(int).to_numpy().astype(np.int64)
+        if init == "louvain":   # sc.pp.neighbors(n_neighbors, use_rep="X") + sc.tl.leiden(resolution=res) (:481-492), on the device
+            X0 = features if init_spa else _dev(X, self.device)
+            labels = leiden(neighbor_graph(X0.contiguous(), int(n_neighbors)), resolution=float(res)).labels
+            return labels.cpu().numpy().astype(np.int64)
         raise ValueError(f"unknown init {init!r}")
 
     def _centers(self, features: torch.Tensor, y: np.ndarray) -> torch.Tensor:
@@ -329,8 +324,8 @@ class SpaGCN:
         self.l = l
 
     def search_set_res(self, x, l, target_num, start=0.4, step=0.1, tol=5e-3, lr=0.05, epochs=10, max_run=10):
-        """Search the leiden resolution that yields ``target_num`` domains (spagcn.py:771-805; same control flow).  Needs the
-        ``init="louvain"`` initialisation, i.e. scanpy — raises NotImplementedError from ``fit`` where scanpy is absent."""
+        """Search the leiden resolution that yields ``target_num`` domains (spagcn.py:771-805; same control flow).  Each step fits
+        with ``init="louvain"``, i.e. the device neighbour graph and Leiden (:mod:`dance_b200.leiden`)."""
         res = start
         clf = SpaGCN(l, device=self.device, precision=self.precision, seed=self.seed)
         old_num = len(set(clf.fit_predict(x, init_spa=True, init="louvain", res=res, tol=tol, lr=lr, epochs=epochs)))
@@ -389,12 +384,16 @@ class SpaGCN:
         self.fit(x, y, **fit_kwargs)
         return self.predict(x)
 
+    @staticmethod
+    def default_score_func(y_true, y_pred) -> float:
+        """Adjusted Rand index (``BaseClusteringMethod._DEFAULT_METRIC = "ari"``, modules/base.py:46-47,168)."""
+        from sklearn.metrics import adjusted_rand_score
+        return float(adjusted_rand_score(np.asarray(y_true), np.asarray(y_pred)))
+
     def score(self, x, y, score_func=None) -> float:
-        """Adjusted Rand index by default (``BaseClusteringMethod._DEFAULT_METRIC = "ari"``, modules/base.py)."""
+        """Adjusted Rand index by default (``default_score_func``)."""
         pred = self.predict(x)
-        if score_func is None:
-            from sklearn.metrics import adjusted_rand_score as score_func
-        return float(score_func(np.asarray(y), pred))
+        return float((score_func or self.default_score_func)(np.asarray(y), pred))
 
     def fit_score(self, x, y, score_func=None, **fit_kwargs) -> float:
         self.fit(x, y, **fit_kwargs)

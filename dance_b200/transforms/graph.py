@@ -15,6 +15,7 @@ import torch
 
 from .. import ops
 from ..graph import GraphLite
+from ..leiden import neighbor_graph
 from .base import BaseTransform
 from .cell_feature import WeightedFeaturePCA
 
@@ -260,8 +261,7 @@ class NeighborGraph(BaseTransform):
         if self.n_pcs is not None:
             rep = rep[:, :self.n_pcs]
         X = torch.as_tensor(np.ascontiguousarray(rep, dtype=np.float32)).cuda()
-        idx, dist = ops.knn(X, int(self.n_neighbors), include_rank0=True)
-        Cn = ops.umap_connectivities(idx, dist.float())
+        Cn = neighbor_graph(X, int(self.n_neighbors))
         n = X.shape[0]
         adj = sp.csr_matrix((Cn.vals.cpu().numpy(), Cn.colidx.cpu().numpy(), Cn.rowptr.cpu().numpy()), shape=(n, n))
         data.data.obsp[self.out] = adj

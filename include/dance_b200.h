@@ -577,6 +577,25 @@ int b2_louvain_csr_host(const int64_t* rowptr, const int32_t* colidx, const doub
                         int32_t* n_comm_out, double* modularity_out, int max_levels, double min_gain);
 
 /* ------------------------------------------------------------------------
+ * Leiden community detection (csrc/leiden.cu): SpaGCN's init="louvain" (spagcn.py:481-492 → scanpy 1.10 tl.leiden →
+ * leidenalg.RBConfigurationVertexPartition with weights = the connectivities and resolution_parameter = resolution).
+ *   The graph is an n×n CSR on the device that must be SYMMETRIC with both directions stored (scanpy's connectivities always
+ *   are; a self-loop is stored once); vals NULL means unit weights, otherwise they must be finite and non-negative.  With
+ *   W = Σ vals, k_i = row sums and K_c = Σ_{i∈c} k_i, the optimised quality is Q = Σ_c (e_c − resolution·K_c²/W), e_c the
+ *   weight inside c; quality_out (host) receives Q / W, which is networkx's modularity(resolution=...) on the undirected graph.
+ *   max_iterations = -1 repeats Leiden iterations until one leaves the membership unchanged (at most 100), k > 0 runs at most k.
+ *   labels_out [n] (device) are 0..K-1 by decreasing community size, ties by the smallest member; *n_comm_out (host) = K.
+ *   info_out (host, nullable) [2]: iterations run, most aggregation levels in one iteration.
+ *   Run-to-run deterministic.  Refinement merges greedily (leidenalg samples with θ = 0.01), so labels are not leidenalg's.
+ *   Synchronises the stream: each phase needs its counts on the host.  The workspace bound depends on (n, nnz) only, since no
+ *   aggregated level is larger than the input; b2_leiden_workspace_bytes returns 0 for n <= 0 or nnz outside [0, 2^31).
+ * ---------------------------------------------------------------------- */
+size_t b2_leiden_workspace_bytes(int32_t n, int64_t nnz);
+int b2_leiden_f32(const int32_t* rowptr, const int32_t* colidx, const float* vals, int32_t n, int64_t nnz, double resolution,
+                  int max_iterations, int32_t* labels_out, int32_t* n_comm_out, double* quality_out, int32_t* info_out,
+                  void* workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------
  * scGNN's normalizer(X, base) (scgnn2.py:795-805) and the concatenations that use it: *_concat_prev_embed
  * (feature_AE_handler scgnn2.py:283-294, graph_AE_handler scgnn2.py:543-546) and clustering_embed = "both" (scgnn2.py:155-157).
  *   b2_quantiles_f32     : np.quantile(base, qs[j]) over ALL rows*cols elements of the row-padded matrix base (method "linear",

@@ -131,14 +131,6 @@ softmax_ce_kernel(const float* __restrict__ logits, int64_t ld, const int64_t* _
   if (lane == 0 && local != 0.f) atomicAdd(loss_out, local);
 }
 
-static unsigned warp_grid2(int64_t rows) {
-  int64_t b = ceil_div<int64_t>(rows, 8);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (unsigned)b;
-}
-
 }  // namespace b2
 
 using namespace b2;
@@ -174,9 +166,9 @@ extern "C" int b2_cellgene_graph_count(const float* X, int64_t ldx, int32_t n_ce
   void* d_temp = ws + cg_off(n_cells, n_genes, 6);
   size_t temp = workspace_bytes - cg_off(n_cells, n_genes, 6);
   B2_CHECK_CUDA(cudaMemsetAsync(col_cnt, 0, cg_off(n_cells, n_genes, 4) - cg_off(n_cells, n_genes, 2), st));
-  cg_count_kernel<<<warp_grid2(n_cells), 256, 0, st>>>(X, ldx, n_cells, n_genes, row_cnt, row_sum, col_cnt, col_sum);
+  cg_count_kernel<<<grid_blocks(n_cells, 8), 256, 0, st>>>(X, ldx, n_cells, n_genes, row_cnt, row_sum, col_cnt, col_sum);
   B2_CHECK_LAUNCH("cg_count_kernel");
-  cast_i32_i64_kernel<<<warp_grid2(n_cells / 32 + 1), 256, 0, st>>>(row_cnt, row_cnt64, n_cells);
+  cast_i32_i64_kernel<<<grid_blocks(n_cells / 32 + 1, 8), 256, 0, st>>>(row_cnt, row_cnt64, n_cells);
   B2_CHECK_LAUNCH("cast_i32_i64_kernel");
   B2_CHECK_CUDA(cudaMemsetAsync(row_cnt64 + n_cells, 0, sizeof(int64_t), st));
   // exclusive scan over n_cells+1 items → row_off[n_cells] = nnz
@@ -195,7 +187,7 @@ extern "C" int b2_cellgene_graph_fill(const float* X, int64_t ldx, int32_t n_cel
   B2_REQUIRE(workspace_bytes >= b2_cellgene_graph_workspace_bytes(n_cells, n_genes), "b2_cellgene_graph_fill: workspace too small");
   cudaStream_t st = as_stream(stream);
   char* ws = reinterpret_cast<char*>(workspace);
-  cg_fill_kernel<<<warp_grid2(n_cells), 256, 0, st>>>(
+  cg_fill_kernel<<<grid_blocks(n_cells, 8), 256, 0, st>>>(
       X, ldx, n_cells, n_genes, reinterpret_cast<int64_t*>(ws + cg_off(n_cells, n_genes, 5)),
       reinterpret_cast<int32_t*>(ws + cg_off(n_cells, n_genes, 0)), reinterpret_cast<float*>(ws + cg_off(n_cells, n_genes, 1)),
       reinterpret_cast<int32_t*>(ws + cg_off(n_cells, n_genes, 2)), reinterpret_cast<float*>(ws + cg_off(n_cells, n_genes, 3)),
@@ -208,7 +200,7 @@ extern "C" int b2_sage_edge_values_f32(const int32_t* rowptr, const int32_t* col
                                        int32_t n_nodes, int32_t n_genes, float* out, void* stream) {
   B2_REQUIRE(rowptr && colidx && w && alpha && out && n_nodes >= 0 && n_genes >= 0, "b2_sage_edge_values_f32: bad arguments");
   if (n_nodes == 0) return B2_OK;
-  sage_edge_values_kernel<<<warp_grid2(n_nodes), 256, 0, as_stream(stream)>>>(rowptr, colidx, w, alpha, n_nodes, n_genes, out);
+  sage_edge_values_kernel<<<grid_blocks(n_nodes, 8), 256, 0, as_stream(stream)>>>(rowptr, colidx, w, alpha, n_nodes, n_genes, out);
   B2_CHECK_LAUNCH("sage_edge_values_kernel");
   return B2_OK;
 }
@@ -217,7 +209,7 @@ extern "C" int b2_softmax_ce_sum_f32(const float* logits, int64_t ld, const int6
                                      float* dlogits, int64_t ldd, float* loss_out, void* stream) {
   B2_REQUIRE(logits && labels && loss_out && n >= 0 && c > 0 && ld >= c, "b2_softmax_ce_sum_f32: bad arguments");
   if (n == 0) return B2_OK;
-  softmax_ce_kernel<<<warp_grid2(n), 256, 0, as_stream(stream)>>>(logits, ld, labels, n, c, dlogits, ldd, loss_out);
+  softmax_ce_kernel<<<grid_blocks(n, 8), 256, 0, as_stream(stream)>>>(logits, ld, labels, n, c, dlogits, ldd, loss_out);
   B2_CHECK_LAUNCH("softmax_ce_kernel");
   return B2_OK;
 }

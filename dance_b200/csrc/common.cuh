@@ -46,6 +46,19 @@ __host__ __device__ constexpr T ceil_div(T a, T b) { return (a + b - 1) / b; }
 
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// Grid-stride launch size: ceil(work / per_block) blocks, clamped to [1, sm_count() · blocks_per_sm].
+static inline unsigned grid_blocks(int64_t work, int64_t per_block, int blocks_per_sm = 16) {
+  const int64_t b = ceil_div(work, per_block), cap = (int64_t)sm_count() * blocks_per_sm;
+  return (unsigned)(b < 1 ? 1 : b > cap ? cap : b);
+}
+
+// gridDim.y of a column-tiled reduction that splits its rows: ceil(sm_count() · waves / col_tiles), clamped to
+// [1, max(rows / min_rows, 1)].
+static inline int row_splits(int col_tiles, int64_t rows, int min_rows, int waves) {
+  const int64_t s = ceil_div(sm_count() * waves, col_tiles), most = rows / min_rows > 1 ? rows / min_rows : 1;
+  return (int)(s < 1 ? 1 : s > most ? most : s);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

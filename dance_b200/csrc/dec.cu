@@ -181,14 +181,6 @@ exp_adj_kernel(const float* __restrict__ D, float* __restrict__ out, int64_t tot
   }
 }
 
-static unsigned dec_grid(int64_t rows) {
-  int64_t b = ceil_div<int64_t>(rows, 8);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (unsigned)b;
-}
-
 }  // namespace b2
 
 using namespace b2;
@@ -197,7 +189,7 @@ extern "C" int b2_dec_q_f32(const float* z, int64_t ldz, const float* mu, int32_
                             float* q, int64_t ldq, void* stream) {
   B2_REQUIRE(z && mu && q && n >= 0 && K > 0 && K <= DEC_MAXK && h > 0 && ldz >= h && ldq >= K, "b2_dec_q_f32: bad arguments (K <= 64)");
   if (n == 0) return B2_OK;
-  dec_q_kernel<<<dec_grid(n), 256, 0, as_stream(stream)>>>(z, ldz, mu, n, K, h, alpha, q, ldq);
+  dec_q_kernel<<<grid_blocks(n, 8), 256, 0, as_stream(stream)>>>(z, ldz, mu, n, K, h, alpha, q, ldq);
   B2_CHECK_LAUNCH("dec_q_kernel");
   return B2_OK;
 }
@@ -206,7 +198,7 @@ extern "C" int b2_dec_target_f32(const float* q, int64_t ldq, const float* colsu
                                  int64_t ldp, void* stream) {
   B2_REQUIRE(q && colsum && p && n >= 0 && K > 0 && K <= DEC_MAXK && ldq >= K && ldp >= K, "b2_dec_target_f32: bad arguments");
   if (n == 0) return B2_OK;
-  dec_target_kernel<<<dec_grid(n), 256, 0, as_stream(stream)>>>(q, ldq, colsum, n, K, p, ldp);
+  dec_target_kernel<<<grid_blocks(n, 8), 256, 0, as_stream(stream)>>>(q, ldq, colsum, n, K, p, ldp);
   B2_CHECK_LAUNCH("dec_target_kernel");
   return B2_OK;
 }
@@ -220,8 +212,7 @@ extern "C" int b2_dec_kl_grad_f32(const float* z, int64_t ldz, const float* mu, 
   B2_CHECK_CUDA(cudaMemsetAsync(loss_out, 0, sizeof(float), st));
   const size_t smem = sizeof(float) * (size_t)K * h;
   const int use_smem = smem <= 48 * 1024;
-  unsigned grid = dec_grid(n);
-  if (use_smem && grid > (unsigned)sm_count() * 4) grid = (unsigned)sm_count() * 4;     // fewer, longer-lived blocks → fewer flushes
+  const unsigned grid = grid_blocks(n, 8, use_smem ? 4 : 16);   // fewer, longer-lived blocks → fewer flushes
   dec_kl_grad_kernel<<<grid, 256, use_smem ? smem : 0, st>>>(z, ldz, mu, p, ldp, n, K, h, alpha, q_out, ldq, dz, lddz, dmu, loss_out,
                                                               labels_out, use_smem);
   B2_CHECK_LAUNCH("dec_kl_grad_kernel");
@@ -232,11 +223,8 @@ extern "C" int b2_sgd_momentum_step_f32(float* param, const float* grad, float* 
                                         float momentum, float weight_decay, int32_t step, void* stream) {
   B2_REQUIRE(param && grad && momentum_buf && n >= 0 && step >= 1, "b2_sgd_momentum_step_f32: bad arguments");
   if (n == 0) return B2_OK;
-  int64_t blocks = ceil_div<int64_t>(n, 1024);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  sgd_momentum_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(param, grad, momentum_buf, n, lr, momentum, weight_decay,
-                                                                      step == 1);
+  sgd_momentum_kernel<<<grid_blocks(n, 1024), 256, 0, as_stream(stream)>>>(param, grad, momentum_buf, n, lr, momentum, weight_decay,
+                                                                           step == 1);
   B2_CHECK_LAUNCH("sgd_momentum_kernel");
   return B2_OK;
 }
@@ -246,17 +234,14 @@ extern "C" int b2_exp_adj_f32(const float* D, float* out, int64_t n_elem, double
   if (n_elem == 0) return B2_OK;
   cudaStream_t st = as_stream(stream);
   const float two_l2 = (float)(2.0 * (l * l));   // numpy: fp32 array / python float → the scalar is rounded to fp32
-  int64_t blocks = ceil_div<int64_t>(n_elem, 2048);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  const unsigned blocks = grid_blocks(n_elem, 2048);
   if (sum_out_dev) {
     B2_CHECK_CUDA(cudaMemsetAsync(sum_out_dev, 0, sizeof(double), st));
-    exp_adj_sum_kernel<<<(unsigned)blocks, 256, 0, st>>>(D, n_elem, two_l2, sum_out_dev);
+    exp_adj_sum_kernel<<<blocks, 256, 0, st>>>(D, n_elem, two_l2, sum_out_dev);
     B2_CHECK_LAUNCH("exp_adj_sum_kernel");
   }
   if (out) {
-    exp_adj_kernel<<<(unsigned)blocks, 256, 0, st>>>(D, out, n_elem, two_l2);
+    exp_adj_kernel<<<blocks, 256, 0, st>>>(D, out, n_elem, two_l2);
     B2_CHECK_LAUNCH("exp_adj_kernel");
   }
   return B2_OK;

@@ -29,11 +29,8 @@ extern "C" int b2_dropout_f32(const float* x, int64_t ldx, int64_t rows, int32_t
   B2_REQUIRE(p >= 0.f && p <= 1.f, "b2_dropout_f32: p must be in [0, 1]");
   if (rows == 0 || cols == 0) return B2_OK;
   B2_REQUIRE(x && y, "b2_dropout_f32: null pointer");
-  int64_t blocks = ceil_div<int64_t>(rows * cols, 256 * 4);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  dropout_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(x, ldx, rows, cols, p, p < 1.f ? 1.f / (1.f - p) : 0.f, seed, key,
-                                                                 y, ldy);
+  dropout_kernel<<<grid_blocks(rows * cols, 1024), 256, 0, as_stream(stream)>>>(x, ldx, rows, cols, p, p < 1.f ? 1.f / (1.f - p) : 0.f,
+                                                                                seed, key, y, ldy);
   B2_CHECK_LAUNCH("dropout_kernel");
   return B2_OK;
 }

@@ -179,13 +179,6 @@ l1_grad_kernel(const float* __restrict__ p, float* __restrict__ grad, int64_t n,
   if ((threadIdx.x & 31) == 0 && l1_out) atomicAdd(l1_out, (float)(a * coef));
 }
 
-int grid_for(int64_t work, int per_thread = 4) {
-  int64_t b = ceil_div<int64_t>(work, 256 * per_thread);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (b > cap) b = cap;
-  return (int)(b < 1 ? 1 : b);
-}
-
 }  // namespace
 }  // namespace b2
 
@@ -212,7 +205,7 @@ extern "C" int b2_kmeans_step_f32(const float* X, int64_t ldx, int32_t n, int32_
   const size_t smem = (size_t)k * d * sizeof(float);
   static bool attr = false;
   if (!attr) { B2_CHECK_CUDA(cudaFuncSetAttribute(kmeans_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)); attr = true; }
-  kmeans_assign_kernel<<<grid_for(n, 1), 256, smem, st>>>(X, ldx, n, d, C, k, labels, update ? sums : nullptr, counts, changed, stats);
+  kmeans_assign_kernel<<<grid_blocks(n, 256), 256, smem, st>>>(X, ldx, n, d, C, k, labels, update ? sums : nullptr, counts, changed, stats);
   B2_CHECK_LAUNCH("kmeans_assign_kernel");
   if (update) {
     kmeans_update_kernel<<<ceil_div(k * d, 128), 128, 0, st>>>(C, sums, counts, k, d, stats + 1);
@@ -230,9 +223,9 @@ extern "C" int b2_graph_regu_weights_f32(const int32_t* rowptr, const int32_t* c
   if (n <= 0) return B2_OK;
   cudaStream_t st = as_stream(stream);
   B2_CHECK_CUDA(cudaMemsetAsync(cluster_sums, 0, sizeof(double) * (size_t)n_clusters, st));
-  cluster_inv_degree_kernel<<<grid_for(n, 1), 256, 0, st>>>(rowptr, colidx, labels, n, n_clusters, cluster_sums);
+  cluster_inv_degree_kernel<<<grid_blocks(n, 256), 256, 0, st>>>(rowptr, colidx, labels, n, n_clusters, cluster_sums);
   B2_CHECK_LAUNCH("cluster_inv_degree_kernel");
-  graph_regu_weights_kernel<<<grid_for(n, 1), 256, 0, st>>>(rowptr, colidx, labels, n, n_clusters, cluster_sums, w);
+  graph_regu_weights_kernel<<<grid_blocks(n, 256), 256, 0, st>>>(rowptr, colidx, labels, n, n_clusters, cluster_sums, w);
   B2_CHECK_LAUNCH("graph_regu_weights_kernel");
   return B2_OK;
 }
@@ -246,9 +239,9 @@ extern "C" int b2_graph_regu_weights_weighted_f32(const int32_t* rowptr, const i
   double* colsum = scratch;
   double* sums = scratch + n;
   B2_CHECK_CUDA(cudaMemsetAsync(scratch, 0, sizeof(double) * ((size_t)n + n_clusters), st));
-  weighted_sums_kernel<<<grid_for(n, 1), 256, 0, st>>>(rowptr, colidx, vals, labels, n, n_clusters, colsum, sums);
+  weighted_sums_kernel<<<grid_blocks(n, 256), 256, 0, st>>>(rowptr, colidx, vals, labels, n, n_clusters, colsum, sums);
   B2_CHECK_LAUNCH("weighted_sums_kernel");
-  weighted_regu_weights_kernel<<<grid_for(n, 1), 256, 0, st>>>(labels, n, n_clusters, colsum, sums, w);
+  weighted_regu_weights_kernel<<<grid_blocks(n, 256), 256, 0, st>>>(labels, n, n_clusters, colsum, sums, w);
   B2_CHECK_LAUNCH("weighted_regu_weights_kernel");
   return B2_OK;
 }
@@ -262,7 +255,7 @@ extern "C" int b2_celltype_loss_grad_f32(const float* recon, const float* target
   if (rows == 0) return B2_OK;
   cudaStream_t st = as_stream(stream);
   B2_CHECK_CUDA(cudaMemsetAsync(scratch2, 0, 2 * sizeof(double), st));
-  const int g = grid_for(rows * cols);
+  const unsigned g = grid_blocks(rows * cols, 1024);
   celltype_reduce_kernel<<<g, 256, 0, st>>>(recon, target, x_dropout, row_weight, rows, cols, cols_orig, scratch2);
   B2_CHECK_LAUNCH("celltype_reduce_kernel");
   celltype_grad_kernel<<<g, 256, 0, st>>>(recon, target, x_dropout, row_weight, rows, cols, cols_orig, scratch2, relu_mask, grad, loss_out);
@@ -274,7 +267,7 @@ extern "C" int b2_l1_grad_add_f32(const float* param, float* grad, int64_t n, fl
   using namespace b2;
   B2_REQUIRE(param && grad, "b2_l1_grad_add_f32: null pointer");
   if (n <= 0) return B2_OK;
-  l1_grad_kernel<<<grid_for(n), 256, 0, as_stream(stream)>>>(param, grad, n, coef, l1_out);
+  l1_grad_kernel<<<grid_blocks(n, 1024), 256, 0, as_stream(stream)>>>(param, grad, n, coef, l1_out);
   B2_CHECK_LAUNCH("l1_grad_kernel");
   return B2_OK;
 }

@@ -173,10 +173,7 @@ extern "C" int b2_pearson_corr_f32(const float* X, int64_t ldx, int32_t n, int32
   B2_CHECK_CUDA(cudaMemsetAsync(sum, 0, sizeof(double) * g, st));
   {
     const int col_tiles = ceil_div(g, 32);
-    int splits = ceil_div(sm_count() * 4, col_tiles);
-    const int max_splits = n / 64 > 0 ? n / 64 : 1;
-    if (splits > max_splits) splits = max_splits;
-    dim3 grid(col_tiles, splits < 1 ? 1 : splits);
+    dim3 grid(col_tiles, row_splits(col_tiles, n, 64, 4));
     fg_colsum_kernel<<<grid, 256, 0, st>>>(X, ldx, n, g, sum);
     B2_CHECK_LAUNCH("fg_colsum_kernel");
     fg_mean_kernel<<<ceil_div(g, 256), 256, 0, st>>>(sum, g, n);
@@ -184,18 +181,12 @@ extern "C" int b2_pearson_corr_f32(const float* X, int64_t ldx, int32_t n, int32
   }
   const int tiles = ceil_div(g, FG_T);
   const int tri = tiles * (tiles + 1) / 2;
-  int splits = ceil_div(sm_count() * 2, tri);
-  const int max_splits = n / 256 > 0 ? n / 256 : 1;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
+  const int splits = row_splits(tri, n, 256, 2);
   if (splits > 1) B2_CHECK_CUDA(cudaMemsetAsync(Cm, 0, sizeof(double) * (size_t)g * g, st));
   dim3 grid(tiles, tiles, splits);
   fg_gram_kernel<<<grid, 256, 0, st>>>(X, ldx, n, g, sum, Cm);
   B2_CHECK_LAUNCH("fg_gram_kernel");
-  int64_t blocks = ceil_div<int64_t>((int64_t)g * g, 1024);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  fg_corr_kernel<<<(unsigned)blocks, 256, 0, st>>>(Cm, g, n, adj, lda);
+  fg_corr_kernel<<<grid_blocks((int64_t)g * g, 1024), 256, 0, st>>>(Cm, g, n, adj, lda);
   B2_CHECK_LAUNCH("fg_corr_kernel");
   return B2_OK;
 }
@@ -219,10 +210,7 @@ extern "C" int b2_threshold_graph_count(const float* adj, int64_t lda, int32_t g
   int32_t* row_cnt = reinterpret_cast<int32_t*>(base + align_up(temp, 256));
   int32_t* col_cnt = reinterpret_cast<int32_t*>(base + align_up(temp, 256) + cnt_bytes);
   B2_CHECK_CUDA(cudaMemsetAsync(row_cnt, 0, 2 * cnt_bytes, st));
-  int64_t blocks = ceil_div<int64_t>(g, 8);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  fg_count_kernel<<<(unsigned)blocks, 256, 0, st>>>(adj, lda, g, threshold, positive_only, row_cnt, col_cnt);
+  fg_count_kernel<<<grid_blocks(g, 8), 256, 0, st>>>(adj, lda, g, threshold, positive_only, row_cnt, col_cnt);
   B2_CHECK_LAUNCH("fg_count_kernel");
   B2_CHECK_CUDA(cub::DeviceScan::ExclusiveSum(base, temp, row_cnt, rowptr, g + 1, st));
   int32_t total = 0;
@@ -242,11 +230,8 @@ extern "C" int b2_threshold_graph_fill(const float* adj, int64_t lda, int32_t g,
   char* base = reinterpret_cast<char*>(workspace);
   const size_t cnt_bytes = align_up(sizeof(int32_t) * ((size_t)g + 1), 256);
   const int32_t* col_cnt = reinterpret_cast<const int32_t*>(base + align_up(temp, 256) + cnt_bytes);   // left there by `count`
-  int64_t blocks = ceil_div<int64_t>(g, 8);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  fg_fill_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(adj, lda, g, threshold, positive_only, rowptr, col_cnt,
-                                                                 normalize_edges, src, dst, w);
+  fg_fill_kernel<<<grid_blocks(g, 8), 256, 0, as_stream(stream)>>>(adj, lda, g, threshold, positive_only, rowptr, col_cnt,
+                                                                   normalize_edges, src, dst, w);
   B2_CHECK_LAUNCH("fg_fill_kernel");
   return B2_OK;
 }

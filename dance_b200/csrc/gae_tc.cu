@@ -746,10 +746,7 @@ static int launch_dp(Params p, int units, bool tri, void* ws, cudaStream_t st) {
     return launch_sweep<DP, true>(p, units, st);
   }
   uint8_t* zt_lo = zt_hi + (size_t)p.nb * zt_bytes<DP>();
-  int64_t blocks = ceil_div<int64_t>(npad * DP, 256);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  gae_split_kernel<DP><<<(unsigned)blocks, 256, 0, st>>>(p.z, p.ldz, p.n, p.d, npad, zs_hi, zs_lo, zt_hi, zt_lo);
+  gae_split_kernel<DP><<<grid_blocks(npad * DP, 256), 256, 0, st>>>(p.z, p.ldz, p.n, p.d, npad, zs_hi, zs_lo, zt_hi, zt_lo);
   B2_CHECK_LAUNCH("gae_split_kernel");
   if (units <= 0) return B2_OK;
   p.zs_hi = zs_hi; p.zs_lo = zs_lo; p.zt_hi = zt_hi; p.zt_lo = zt_lo;

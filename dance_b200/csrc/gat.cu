@@ -487,21 +487,6 @@ gat_combine_bwd_identity_kernel(const float* __restrict__ dout, int64_t lddo, co
   }
 }
 
-static unsigned warp_rows_grid(int64_t rows) {
-  int64_t b = ceil_div<int64_t>(rows, 8);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (unsigned)b;
-}
-static unsigned ew_blocks(int64_t n) {
-  int64_t b = ceil_div<int64_t>(n, 256 * 4);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (unsigned)b;
-}
-
 }  // namespace b2
 
 using namespace b2;
@@ -511,7 +496,7 @@ extern "C" int b2_gat_scores_f32(const float* H, int64_t ldh, const float* a_src
   B2_REQUIRE(n >= 0 && nheads > 0 && F > 0 && ldh >= (int64_t)nheads * F, "b2_gat_scores_f32: bad arguments");
   if (n == 0) return B2_OK;
   B2_REQUIRE(H && a_src && a_trg && s_src && s_trg, "b2_gat_scores_f32: null pointer");
-  gat_scores_kernel<<<warp_rows_grid(n), 256, 0, as_stream(stream)>>>(H, ldh, a_src, a_trg, n, nheads, F, s_src, s_trg);
+  gat_scores_kernel<<<grid_blocks(n, 8), 256, 0, as_stream(stream)>>>(H, ldh, a_src, a_trg, n, nheads, F, s_src, s_trg);
   B2_CHECK_LAUNCH("gat_scores_kernel");
   return B2_OK;
 }
@@ -525,7 +510,7 @@ extern "C" int b2_gat_edge_max_f32(const int32_t* rowptr, const int32_t* colidx,
   B2_CHECK_LAUNCH("set_neg_inf_kernel");
   if (n == 0) return B2_OK;
   B2_REQUIRE(rowptr && colidx && s_src && s_trg, "b2_gat_edge_max_f32: null pointer");
-  gat_edge_max_kernel<<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, s_src, s_trg, n, nheads, score_act, slope, gmax_dev);
+  gat_edge_max_kernel<<<grid_blocks(n, 8), 256, 0, st>>>(rowptr, colidx, s_src, s_trg, n, nheads, score_act, slope, gmax_dev);
   B2_CHECK_LAUNCH("gat_edge_max_kernel");
   return B2_OK;
 }
@@ -545,7 +530,7 @@ extern "C" int b2_gat_aggregate_fwd_f32(const int32_t* rowptr, const int32_t* co
   if (n == 0) return B2_OK;
   B2_REQUIRE(rowptr && colidx && H && s_src && s_trg && out, "b2_gat_aggregate_fwd_f32: null pointer");
   const auto kernel = drop_p > 0.f ? gat_aggregate_fwd_kernel<true> : gat_aggregate_fwd_kernel<false>;
-  kernel<<<warp_rows_grid(n), 256, 0, as_stream(stream)>>>(rowptr, colidx, H, ldh, s_src, s_trg, n, nheads, F, score_act, slope,
+  kernel<<<grid_blocks(n, 8), 256, 0, as_stream(stream)>>>(rowptr, colidx, H, ldh, s_src, s_trg, n, nheads, F, score_act, slope,
                                                            shift_mode, gmax_dev, out, ldo, alpha_out, make_drop(drop_p, seed, key));
   B2_CHECK_LAUNCH("gat_aggregate_fwd_kernel");
   return B2_OK;
@@ -576,23 +561,19 @@ extern "C" int b2_gat_aggregate_bwd_f32(const int32_t* rowptr, const int32_t* co
   if (gmax_dev) B2_CHECK_CUDA(cudaMemsetAsync(shift_ws, 0, sizeof(float) * 2, st));
   const AttnDrop drop = make_drop(drop_p, seed, key);
   const auto target_kernel = drop_p > 0.f ? gat_bwd_target_kernel<true> : gat_bwd_target_kernel<false>;
-  target_kernel<<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, H, ldh, s_src, s_trg, alpha, dOut, lddo, H2, ldh2, dOut2, lddo2, n,
+  target_kernel<<<grid_blocks(n, 8), 256, 0, st>>>(rowptr, colidx, H, ldh, s_src, s_trg, alpha, dOut, lddo, H2, ldh2, dOut2, lddo2, n,
                                                    nheads, F, score_act, slope, gmax_dev, dpre_edge_ws, ds_trg_ws, shift_ws, drop);
   B2_CHECK_LAUNCH("gat_bwd_target_kernel");
   if (gmax_dev) {
-    gat_bwd_shift_kernel<<<warp_rows_grid(n), 256, 0, st>>>(rowptr, colidx, s_src, s_trg, n, nheads, score_act, slope, gmax_dev,
+    gat_bwd_shift_kernel<<<grid_blocks(n, 8), 256, 0, st>>>(rowptr, colidx, s_src, s_trg, n, nheads, score_act, slope, gmax_dev,
                                                            shift_ws, dpre_edge_ws, ds_trg_ws);
     B2_CHECK_LAUNCH("gat_bwd_shift_kernel");
   }
   const auto source_kernel = drop_p > 0.f ? gat_bwd_source_kernel<true> : gat_bwd_source_kernel<false>;
-  source_kernel<<<warp_rows_grid(n), 256, 0, st>>>(t_rowptr, t_colidx, t_perm, alpha, dpre_edge_ws, dOut, lddo, dH2 ? dOut2 : nullptr,
+  source_kernel<<<grid_blocks(n, 8), 256, 0, st>>>(t_rowptr, t_colidx, t_perm, alpha, dpre_edge_ws, dOut, lddo, dH2 ? dOut2 : nullptr,
                                                    lddo2, n, nheads, F, dH, lddh, dH2, lddh2, ds_src_ws, drop);
   B2_CHECK_LAUNCH("gat_bwd_source_kernel");
-  int splits = ceil_div(sm_count() * 2, ceil_div(W, 32));
-  const int max_splits = n / 256 > 0 ? n / 256 : 1;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  dim3 grid(ceil_div(W, 32), splits);
+  dim3 grid(ceil_div(W, 32), row_splits(ceil_div(W, 32), n, 256, 2));
   gat_bwd_scores_kernel<<<grid, 256, 0, st>>>(H, ldh, a_src, a_trg, ds_src_ws, ds_trg_ws, n, nheads, F, dH, lddh, da_src, da_trg);
   B2_CHECK_LAUNCH("gat_bwd_scores_kernel");
   return B2_OK;
@@ -607,8 +588,8 @@ extern "C" int b2_gat_combine_fwd_f32(const float* agg, int64_t ldagg, const flo
   if (n == 0) return B2_OK;
   B2_REQUIRE(agg && out && (skip || !identity_skip), "b2_gat_combine_fwd_f32: null pointer");
   const auto kernel = identity_skip ? gat_combine_fwd_kernel<true> : gat_combine_fwd_kernel<false>;
-  kernel<<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(agg, ldagg, skip, ldskip, bias, n, nheads, F,
-                                                                                         concat, act, out, ldo);
+  kernel<<<grid_blocks((int64_t)n * (concat ? nheads * F : F), 1024), 256, 0, as_stream(stream)>>>(agg, ldagg, skip, ldskip, bias, n,
+                                                                                                   nheads, F, concat, act, out, ldo);
   B2_CHECK_LAUNCH("gat_combine_fwd_kernel");
   return B2_OK;
 }
@@ -622,11 +603,11 @@ extern "C" int b2_gat_combine_bwd_f32(const float* dout, int64_t lddo, const flo
   if (n == 0) return B2_OK;
   B2_REQUIRE(dout && out && dpre, "b2_gat_combine_bwd_f32: null pointer");
   if (dx_skip) {
-    gat_combine_bwd_identity_kernel<<<ew_blocks((int64_t)n * F), 256, 0, as_stream(stream)>>>(dout, lddo, out, ldo, n, nheads, F, concat,
-                                                                                             act, dpre, ldp, dact, ldact, dx_skip, ldx);
+    gat_combine_bwd_identity_kernel<<<grid_blocks((int64_t)n * F, 1024), 256, 0, as_stream(stream)>>>(
+        dout, lddo, out, ldo, n, nheads, F, concat, act, dpre, ldp, dact, ldact, dx_skip, ldx);
     B2_CHECK_LAUNCH("gat_combine_bwd_identity_kernel");
   } else {
-    gat_combine_bwd_kernel<<<ew_blocks((int64_t)n * (concat ? nheads * F : F)), 256, 0, as_stream(stream)>>>(
+    gat_combine_bwd_kernel<<<grid_blocks((int64_t)n * (concat ? nheads * F : F), 1024), 256, 0, as_stream(stream)>>>(
         dout, lddo, out, ldo, n, nheads, F, concat, act, dpre, ldp, dact, ldact);
     B2_CHECK_LAUNCH("gat_combine_bwd_kernel");
   }

@@ -162,15 +162,8 @@ __global__ void colsum_finish_kernel(const float* __restrict__ partial, int N, i
 
 }  // namespace b2
 
-static int colsum_splits(int M, int N) {
-  // enough blocks to fill the machine: (N/32 column blocks) x splits; each split covers >= 256 rows
-  const int col_blocks = b2::ceil_div(N, 32);
-  int splits = b2::ceil_div(b2::sm_count() * 4, col_blocks);
-  const int max_splits = M / 256 > 0 ? M / 256 : 1;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  return splits;
-}
+// enough blocks to fill the machine: (N/32 column blocks) x splits; each split covers >= 256 rows
+static int colsum_splits(int M, int N) { return b2::row_splits(b2::ceil_div(N, 32), M, 256, 4); }
 
 extern "C" size_t b2_colsum_workspace_bytes(int M, int N) {
   const int splits = colsum_splits(M, N);

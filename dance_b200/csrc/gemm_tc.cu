@@ -460,10 +460,8 @@ int gemm_tc(const float* A, int64_t lda, int transA, const float* B, int64_t ldb
                : (mode == MODE_BF16 ? launch_gemm_mode<MODE_BF16>(p, pl, st) : launch_gemm_mode<MODE_TF32>(p, pl, st));
   if (rc != B2_OK) return rc;
   if (pl.splits > 1) {
-    size_t total = (size_t)M * N;
-    int blocks = (int)((total + 255) / 256);
-    if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-    splitk_reduce_kernel<<<blocks, 256, 0, st>>>(p.partial, pl.splits, M, N, C, ldc, bias, act, mask, ldmask, beta);
+    splitk_reduce_kernel<<<grid_blocks((int64_t)M * N, 256, 8), 256, 0, st>>>(p.partial, pl.splits, M, N, C, ldc, bias, act, mask,
+                                                                              ldmask, beta);
     B2_CHECK_LAUNCH("splitk_reduce_kernel");
   }
   return B2_OK;

@@ -71,14 +71,6 @@ static int bits_for(int64_t n) {
   return b;
 }
 
-static unsigned grid_for(int64_t n, int threads = 256) {
-  int64_t b = ceil_div<int64_t>(n, threads);
-  const int64_t cap = (int64_t)sm_count() * 32;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (unsigned)b;
-}
-
 // ---- kNN graph ------------------------------------------------------------
 
 __global__ void knn_edge_keys_kernel(const int32_t* knn_idx, int32_t n, int32_t k, uint64_t* keys) {
@@ -230,14 +222,14 @@ extern "C" int b2_csr_transpose(const int32_t* rowptr, const int32_t* colidx, co
   cub::DeviceRadixSort::SortPairs(nullptr, temp, colidx, keys_out, iota, perm, (int)nnz);
   void* d_temp = ws.take<char>(temp);
   if (!ws.ok()) { set_error("b2_csr_transpose: workspace carve overflow"); return B2_ERR_WORKSPACE; }
-  iota_kernel<<<grid_for(nnz), 256, 0, st>>>(iota, nnz);
+  iota_kernel<<<grid_blocks(nnz, 256, 32), 256, 0, st>>>(iota, nnz);
   B2_CHECK_LAUNCH("iota_kernel");
   // stable LSD radix sort: equal columns keep source (row-major) order → deterministic transpose
   B2_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(d_temp, temp, colidx, keys_out, iota, perm, (int)nnz, 0,
                                                 bits_for((int64_t)n_cols + 1), st));
-  rowptr_from_sorted_i32<<<grid_for((int64_t)n_cols + 1), 256, 0, st>>>(keys_out, nnz, n_cols, t_rowptr);
+  rowptr_from_sorted_i32<<<grid_blocks((int64_t)n_cols + 1, 256, 32), 256, 0, st>>>(keys_out, nnz, n_cols, t_rowptr);
   B2_CHECK_LAUNCH("rowptr_from_sorted_i32");
-  transpose_fill_kernel<<<grid_for(nnz), 256, 0, st>>>(rowptr, vals, perm, n_rows, nnz, t_colidx, t_vals);
+  transpose_fill_kernel<<<grid_blocks(nnz, 256, 32), 256, 0, st>>>(rowptr, vals, perm, n_rows, nnz, t_colidx, t_vals);
   B2_CHECK_LAUNCH("transpose_fill_kernel");
   return B2_OK;
 }
@@ -272,7 +264,7 @@ extern "C" int b2_knn_graph_build(const int32_t* knn_idx, int32_t n, int32_t k, 
   void* d_temp = ws.take<char>(temp);
   if (!ws.ok()) { set_error("b2_knn_graph_build: workspace carve overflow"); return B2_ERR_WORKSPACE; }
 
-  knn_edge_keys_kernel<<<grid_for((int64_t)n * k + n), 256, 0, st>>>(knn_idx, n, k, keys);
+  knn_edge_keys_kernel<<<grid_blocks((int64_t)n * k + n, 256, 32), 256, 0, st>>>(knn_idx, n, k, keys);
   B2_CHECK_LAUNCH("knn_edge_keys_kernel");
   B2_CHECK_CUDA(cub::DeviceRadixSort::SortKeys(d_temp, temp, keys, keys2, (int)total, 0, 32 + bits_for(n), st));
   B2_CHECK_CUDA(cub::DeviceSelect::Unique(d_temp, temp, keys2, keys, d_num, (int)total, st));
@@ -284,9 +276,9 @@ extern "C" int b2_knn_graph_build(const int32_t* knn_idx, int32_t n, int32_t k, 
     set_error("b2_knn_graph_build: capacity %lld < nnz %d", (long long)capacity, h_num);
     return B2_ERR_WORKSPACE;
   }
-  knn_rowptr_kernel<<<grid_for((int64_t)n + 1), 256, 0, st>>>(keys, d_num, n, rowptr);
+  knn_rowptr_kernel<<<grid_blocks((int64_t)n + 1, 256, 32), 256, 0, st>>>(keys, d_num, n, rowptr);
   B2_CHECK_LAUNCH("knn_rowptr_kernel");
-  knn_fill_kernel<<<grid_for(n), 256, 0, st>>>(keys, rowptr, n, colidx, vals_norm);
+  knn_fill_kernel<<<grid_blocks(n, 256, 32), 256, 0, st>>>(keys, rowptr, n, colidx, vals_norm);
   B2_CHECK_LAUNCH("knn_fill_kernel");
   return B2_OK;
 }
@@ -334,21 +326,22 @@ extern "C" int b2_knn_graph_weighted_build(const int32_t* knn_idx, const double*
   for (int pass = 0; pass < 2; ++pass) {   // 0: L by source row, 1: Lᵀ by target row
     const bool by_target = pass == 1;
     int32_t* rp = by_target ? t_rowptr : rowptr;
-    knn_weighted_keys_kernel<<<grid_for(total), 256, 0, st>>>(knn_idx, n, k, by_target, keys, slots, flags);
+    knn_weighted_keys_kernel<<<grid_blocks(total, 256, 32), 256, 0, st>>>(knn_idx, n, k, by_target, keys, slots, flags);
     B2_CHECK_LAUNCH("knn_weighted_keys_kernel");
     // LSD radix sort is stable, but every kept key is distinct, so the order within a row is the column order alone
     B2_CHECK_CUDA(cub::DeviceRadixSort::SortPairs(d_temp, temp, keys, keys_sorted, slots, slots_sorted, (int)total, 0, key_bits, st));
-    knn_weighted_rowptr_kernel<<<grid_for((int64_t)n + 1), 256, 0, st>>>(keys_sorted, total, n, rp);
+    knn_weighted_rowptr_kernel<<<grid_blocks((int64_t)n + 1, 256, 32), 256, 0, st>>>(keys_sorted, total, n, rp);
     B2_CHECK_LAUNCH("knn_weighted_rowptr_kernel");
-    sorted_keys_duplicate_kernel<<<grid_for(total), 256, 0, st>>>(keys_sorted, rp, n, flags + 1);
+    sorted_keys_duplicate_kernel<<<grid_blocks(total, 256, 32), 256, 0, st>>>(keys_sorted, rp, n, flags + 1);
     B2_CHECK_LAUNCH("sorted_keys_duplicate_kernel");
     if (!by_target) {
-      knn_weighted_rowsum_kernel<<<grid_for(n), 256, 0, st>>>(rp, keys_sorted, slots_sorted, knn_dist, n, k, dm, w_row);
+      knn_weighted_rowsum_kernel<<<grid_blocks(n, 256, 32), 256, 0, st>>>(rp, keys_sorted, slots_sorted, knn_dist, n, k, dm, w_row);
       B2_CHECK_LAUNCH("knn_weighted_rowsum_kernel");
       B2_CHECK_CUDA(cub::DeviceReduce::Sum(d_temp, temp, w_row, sum_w, n, st));   // ΣW = adj_train.sum() (scgnn2.py:567)
     }
-    knn_weighted_fill_kernel<<<grid_for(n), 256, 0, st>>>(rp, keys_sorted, slots_sorted, knn_dist, dm, n, k, by_target,
-                                                          by_target ? t_colidx : colidx, by_target ? t_y : y, by_target ? norm : norm_t);
+    knn_weighted_fill_kernel<<<grid_blocks(n, 256, 32), 256, 0, st>>>(rp, keys_sorted, slots_sorted, knn_dist, dm, n, k, by_target,
+                                                                      by_target ? t_colidx : colidx, by_target ? t_y : y,
+                                                                      by_target ? norm : norm_t);
     B2_CHECK_LAUNCH("knn_weighted_fill_kernel");
   }
   int32_t h_flags[2] = {0, 0}, h_nnz[2] = {0, 0};

@@ -175,12 +175,6 @@ scatter_rows_kernel(const float* __restrict__ x, int64_t ldx, int32_t rows, int3
   }
 }
 
-static unsigned grid_for(int64_t total) {
-  int64_t blocks = ceil_div<int64_t>(total, 256);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  return (unsigned)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
-}
-
 }  // namespace b2
 
 using namespace b2;
@@ -255,7 +249,7 @@ extern "C" int b2_graphsc_scatter_rows_f32(const float* x, int64_t ldx, int32_t 
   B2_REQUIRE(rows >= 0 && cols >= 0 && ldx >= cols && ldo >= cols, "b2_graphsc_scatter_rows_f32: bad shape");
   if (rows == 0 || cols == 0) return B2_OK;
   B2_REQUIRE(x && idx && out, "b2_graphsc_scatter_rows_f32: null pointer");
-  scatter_rows_kernel<<<grid_for((int64_t)rows * cols), 256, 0, as_stream(stream)>>>(x, ldx, rows, cols, idx, offset, out, ldo);
+  scatter_rows_kernel<<<grid_blocks((int64_t)rows * cols, 256), 256, 0, as_stream(stream)>>>(x, ldx, rows, cols, idx, offset, out, ldo);
   B2_CHECK_LAUNCH("scatter_rows_kernel");
   return B2_OK;
 }

@@ -297,23 +297,6 @@ adj_sample_kernel(const float* __restrict__ Mu, const float* __restrict__ Ls, co
     Z[t] = Mu[t] + expf(Ls[t]) * Eps[t];       // torch.normal(mean, exp(log_std)) with the noise made explicit
 }
 
-static unsigned ew_grid(int64_t total) {
-  int64_t b = ceil_div<int64_t>(total, 1024);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (unsigned)b;
-}
-
-static dim3 col_grid(int32_t n, int32_t c) {
-  const int col_tiles = ceil_div(c, 32);
-  int splits = ceil_div(sm_count() * 4, col_tiles);
-  const int max_splits = n / 64 > 0 ? n / 64 : 1;
-  if (splits > max_splits) splits = max_splits;
-  if (splits < 1) splits = 1;
-  return dim3(col_tiles, splits);
-}
-
 }  // namespace b2
 
 using namespace b2;
@@ -333,7 +316,7 @@ extern "C" int b2_batchnorm_fwd_f32(const float* X, int64_t ldx, int32_t n, int3
   double* sq = sum + c;
   if (training) {
     B2_CHECK_CUDA(cudaMemsetAsync(sum, 0, sizeof(double) * 2 * c, st));
-    const dim3 grid = col_grid(n, c);
+    const dim3 grid(ceil_div(c, 32), row_splits(ceil_div(c, 32), n, 64, 4));
     bn_stats_kernel<<<grid, 256, 0, st>>>(X, ldx, n, c, 0, sum, sq);
     B2_CHECK_LAUNCH("bn_stats_kernel<sum>");
     bn_stats_kernel<<<grid, 256, 0, st>>>(X, ldx, n, c, 1, sum, sq);
@@ -342,7 +325,7 @@ extern "C" int b2_batchnorm_fwd_f32(const float* X, int64_t ldx, int32_t n, int3
   bn_finalize_kernel<<<ceil_div(c, 256), 256, 0, st>>>(sum, sq, n, c, training, momentum, eps, running_mean, running_var, save_mean,
                                                        save_invstd);
   B2_CHECK_LAUNCH("bn_finalize_kernel");
-  bn_apply_kernel<<<ew_grid((int64_t)n * c), 256, 0, st>>>(X, ldx, n, c, gamma, beta, save_mean, save_invstd, act, out, ldo);
+  bn_apply_kernel<<<grid_blocks((int64_t)n * c, 1024), 256, 0, st>>>(X, ldx, n, c, gamma, beta, save_mean, save_invstd, act, out, ldo);
   B2_CHECK_LAUNCH("bn_apply_kernel");
   return B2_OK;
 }
@@ -359,10 +342,11 @@ extern "C" int b2_batchnorm_bwd_f32(const float* dY, int64_t lddy, const float* 
   double* db = reinterpret_cast<double*>(workspace);
   double* dg = db + c;
   B2_CHECK_CUDA(cudaMemsetAsync(db, 0, sizeof(double) * 2 * c, st));
-  bn_bwd_reduce_kernel<<<col_grid(n, c), 256, 0, st>>>(dY, lddy, Y, ldy, X, ldx, n, c, save_mean, save_invstd, act, db, dg);
+  const dim3 grid(ceil_div(c, 32), row_splits(ceil_div(c, 32), n, 64, 4));
+  bn_bwd_reduce_kernel<<<grid, 256, 0, st>>>(dY, lddy, Y, ldy, X, ldx, n, c, save_mean, save_invstd, act, db, dg);
   B2_CHECK_LAUNCH("bn_bwd_reduce_kernel");
-  bn_bwd_apply_kernel<<<ew_grid((int64_t)n * c), 256, 0, st>>>(dY, lddy, Y, ldy, X, ldx, n, c, gamma, save_mean, save_invstd, act,
-                                                              training, db, dg, dX, lddx, dgamma, dbeta);
+  bn_bwd_apply_kernel<<<grid_blocks((int64_t)n * c, 1024), 256, 0, st>>>(dY, lddy, Y, ldy, X, ldx, n, c, gamma, save_mean, save_invstd,
+                                                                         act, training, db, dg, dX, lddx, dgamma, dbeta);
   B2_CHECK_LAUNCH("bn_bwd_apply_kernel");
   return B2_OK;
 }
@@ -376,7 +360,7 @@ extern "C" int b2_zinb_loss_grad_f32(const float* a_pi, const float* b_disp, con
   B2_REQUIRE((!mean_out && !disp_out && !pi_out) || (mean_out && disp_out && pi_out), "b2_zinb_loss_grad_f32: outputs are all-or-none");
   cudaStream_t st = as_stream(stream);
   B2_CHECK_CUDA(cudaMemsetAsync(acc3, 0, sizeof(double) * 3, st));
-  const unsigned grid = ew_grid((int64_t)n * g);
+  const unsigned grid = grid_blocks((int64_t)n * g, 1024);
   zinb_kernel<false><<<grid, 256, 0, st>>>(a_pi, b_disp, c_mean, ld, Y, ldy, size_factors, mask, ldm, n, g, le, ke, nullptr, nullptr,
                                           nullptr, nullptr, 0, mean_out, disp_out, pi_out, ldo, acc3);
   B2_CHECK_LAUNCH("zinb_kernel<loss>");
@@ -391,7 +375,7 @@ extern "C" int b2_zinb_loss_grad_f32(const float* a_pi, const float* b_disp, con
 extern "C" int b2_adj_sample_f32(const float* mu, const float* log_std, const float* eps, int64_t n_elem, float* z, void* stream) {
   B2_REQUIRE(mu && log_std && eps && z && n_elem >= 0, "b2_adj_sample_f32: bad arguments");
   if (n_elem == 0) return B2_OK;
-  adj_sample_kernel<<<ew_grid(n_elem), 256, 0, as_stream(stream)>>>(mu, log_std, eps, n_elem, z);
+  adj_sample_kernel<<<grid_blocks(n_elem, 1024), 256, 0, as_stream(stream)>>>(mu, log_std, eps, n_elem, z);
   B2_CHECK_LAUNCH("adj_sample_kernel");
   return B2_OK;
 }
@@ -410,7 +394,7 @@ extern "C" int b2_adj_reparam_bwd_f32(const float* dz, const float* mu, const fl
                                       float coef_kl, float* dmu, float* dlog_std, void* stream) {
   B2_REQUIRE(dz && mu && log_std && eps && dmu && dlog_std && n_elem >= 0, "b2_adj_reparam_bwd_f32: bad arguments");
   if (n_elem == 0) return B2_OK;
-  adj_reparam_bwd_kernel<<<ew_grid(n_elem), 256, 0, as_stream(stream)>>>(dz, mu, log_std, eps, n_elem, coef_kl, dmu, dlog_std);
+  adj_reparam_bwd_kernel<<<grid_blocks(n_elem, 1024), 256, 0, as_stream(stream)>>>(dz, mu, log_std, eps, n_elem, coef_kl, dmu, dlog_std);
   B2_CHECK_LAUNCH("adj_reparam_bwd_kernel");
   return B2_OK;
 }

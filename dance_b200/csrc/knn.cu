@@ -323,13 +323,8 @@ extern "C" int b2_knn_l2_f32(const float* X, int64_t ldx, int32_t n, int32_t d, 
   int32_t* fail_count = reinterpret_cast<int32_t*>(ws + off + 16);
   B2_CHECK_CUDA(cudaMemsetAsync(ws + off, 0, 64, st));
 
-  {
-    int64_t blocks = ceil_div<int64_t>(n, 8);
-    const int64_t cap = (int64_t)sm_count() * 16;
-    if (blocks > cap) blocks = cap;
-    row_sqnorm_kernel<<<(unsigned)blocks, 256, 0, st>>>(X, ldx, n, d, sqn, max_sqn);
-    B2_CHECK_LAUNCH("row_sqnorm_kernel");
-  }
+  row_sqnorm_kernel<<<grid_blocks(n, 8), 256, 0, st>>>(X, ldx, n, d, sqn, max_sqn);
+  B2_CHECK_LAUNCH("row_sqnorm_kernel");
   float err_rel = 1.1920928955078125e-07f * (float)(d + 8);      // fp32 SIMT filter
   bool tc_done = false;
   if (ktc::eligible(n, d, n_q, M)) {
@@ -348,18 +343,14 @@ extern "C" int b2_knn_l2_f32(const float* X, int64_t ldx, int32_t n, int32_t d, 
     knn_candidates_kernel<64><<<grid, KTHREADS, smem, st>>>(X, ldx, sqn, n, d, q_begin, n_q, cand, thr);
   }
   if (!tc_done) B2_CHECK_LAUNCH("knn_candidates_kernel");
-  {
-    int64_t blocks = ceil_div<int64_t>(n_q, 8);
-    const int64_t cap = (int64_t)sm_count() * 16;
-    if (blocks > cap) blocks = cap;
-    if (M == 32)
-      knn_refine_kernel<32><<<(unsigned)blocks, 256, 0, st>>>(X, ldx, sqn, max_sqn, n, d, k, q_begin, n_q, r0, cand, thr, err_rel,
-                                                               idx_out, dist_out, fail_list, fail_count);
-    else
-      knn_refine_kernel<64><<<(unsigned)blocks, 256, 0, st>>>(X, ldx, sqn, max_sqn, n, d, k, q_begin, n_q, r0, cand, thr, err_rel,
-                                                               idx_out, dist_out, fail_list, fail_count);
-    B2_CHECK_LAUNCH("knn_refine_kernel");
-  }
+  const unsigned refine_grid = grid_blocks(n_q, 8);
+  if (M == 32)
+    knn_refine_kernel<32><<<refine_grid, 256, 0, st>>>(X, ldx, sqn, max_sqn, n, d, k, q_begin, n_q, r0, cand, thr, err_rel, idx_out,
+                                                       dist_out, fail_list, fail_count);
+  else
+    knn_refine_kernel<64><<<refine_grid, 256, 0, st>>>(X, ldx, sqn, max_sqn, n, d, k, q_begin, n_q, r0, cand, thr, err_rel, idx_out,
+                                                       dist_out, fail_list, fail_count);
+  B2_CHECK_LAUNCH("knn_refine_kernel");
   knn_fallback_kernel<<<(unsigned)sm_count(), 256, 0, st>>>(X, ldx, n, d, k, q_begin, r0, fail_list, fail_count, idx_out,
                                                             dist_out);
   B2_CHECK_LAUNCH("knn_fallback_kernel");
@@ -370,10 +361,7 @@ extern "C" int b2_pairwise_l2_dense_f32(const float* X, int64_t ldx, int32_t n, 
                                         void* stream) {
   B2_REQUIRE(X && D && n >= 0 && d > 0 && ldx >= d && ldd >= n, "b2_pairwise_l2_dense_f32: bad arguments");
   if (n == 0) return B2_OK;
-  int64_t blocks = ceil_div<int64_t>((int64_t)n * n, 256);
-  const int64_t cap = (int64_t)sm_count() * 32;
-  if (blocks > cap) blocks = cap;
-  pairwise_dense_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(X, ldx, n, d, D, ldd);
+  pairwise_dense_kernel<<<grid_blocks((int64_t)n * n, 256, 32), 256, 0, as_stream(stream)>>>(X, ldx, n, d, D, ldd);
   B2_CHECK_LAUNCH("pairwise_dense_kernel");
   return B2_OK;
 }

@@ -260,18 +260,11 @@ int launch(const float* X, int64_t ldx, const float* sqn, int32_t n, int32_t d, 
   __half* xh = reinterpret_cast<__half*>(w + 256);
   __half* xl = reinterpret_cast<__half*>(w + 256 + align_up((size_t)n * dp * sizeof(__half), 256));
   B2_CHECK_CUDA(cudaMemsetAsync(maxbits, 0, 4, st));
-  int64_t blocks = ceil_div<int64_t>((int64_t)n * d, 256 * 8);
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  absmax_kernel<<<(unsigned)blocks, 256, 0, st>>>(X, ldx, n, d, maxbits);
+  absmax_kernel<<<grid_blocks((int64_t)n * d, 2048, 8), 256, 0, st>>>(X, ldx, n, d, maxbits);
   B2_CHECK_LAUNCH("knn absmax_kernel");
   scale_kernel<<<1, 1, 0, st>>>(maxbits, scale);
   B2_CHECK_LAUNCH("knn scale_kernel");
-  blocks = ceil_div<int64_t>((int64_t)n * dp, 256 * 4);
-  const int64_t cap2 = (int64_t)sm_count() * 16;
-  if (blocks > cap2) blocks = cap2;
-  split_kernel<<<(unsigned)blocks, 256, 0, st>>>(X, ldx, n, d, dp, scale, xh, xl);
+  split_kernel<<<grid_blocks((int64_t)n * dp, 1024), 256, 0, st>>>(X, ldx, n, d, dp, scale, xh, xl);
   B2_CHECK_LAUNCH("knn split_kernel");
 
   Params p;

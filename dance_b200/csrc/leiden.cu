@@ -859,7 +859,7 @@ extern "C" int b2_leiden_f32(const int32_t* rowptr, const int32_t* colidx, const
   // input checks, and the fixed-point scale from the largest weight
   B2_CHECK_CUDA(cudaMemsetAsync(w.maxw, 0, sizeof(unsigned), st));
   B2_CHECK_CUDA(cudaMemsetAsync(w.ints + 4, 0, sizeof(int32_t), st));
-  const unsigned cg = (unsigned)std::min<int64_t>(ceil_div<int64_t>(std::max<int64_t>(nnz, n + 1), LD_THREADS), (int64_t)sm_count() * 8);
+  const unsigned cg = grid_blocks(std::max<int64_t>(nnz, n + 1), LD_THREADS, 8);
   ld_check_kernel<<<cg, LD_THREADS, 0, st>>>(rowptr, colidx, vals, n, nnz, w.maxw, w.ints + 4);
   B2_CHECK_LAUNCH("ld_check_kernel");
   int32_t bad = 0;

@@ -311,13 +311,9 @@ struct Labels {
 template <int D>
 static int launch_gae_edges(const float* z, int64_t ldz, const Labels& lab, int32_t row_begin, int32_t n_rows, float coef, float pw,
                             int use_pw, float* dz, double* acc, cudaStream_t st) {
-  int64_t blocks = ceil_div<int64_t>(n_rows, 8);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
   const auto kernel = lab.vals ? gae_edges_weighted_kernel<D, true> : gae_edges_weighted_kernel<D, false>;
-  kernel<<<(unsigned)blocks, 256, 0, st>>>(z, ldz, lab.rowptr, lab.colidx, lab.vals, lab.t_rowptr, lab.t_colidx, lab.t_vals, row_begin,
-                                           n_rows, coef, pw, use_pw, dz, acc);
+  kernel<<<grid_blocks(n_rows, 8), 256, 0, st>>>(z, ldz, lab.rowptr, lab.colidx, lab.vals, lab.t_rowptr, lab.t_colidx, lab.t_vals,
+                                                 row_begin, n_rows, coef, pw, use_pw, dz, acc);
   B2_CHECK_LAUNCH("gae_edges_weighted_kernel");
   return B2_OK;
 }
@@ -371,11 +367,7 @@ static int gae_loss_grad(const char* fn, const AllPairs& ap, const float* z, int
   });
   if (rc != B2_OK) return rc;
   if (mu) {
-    int64_t blocks = ceil_div<int64_t>((int64_t)n_rows * d, 256);
-    if (blocks < 1) blocks = 1;
-    const int64_t cap = (int64_t)sm_count() * 16;
-    if (blocks > cap) blocks = cap;
-    gae_kld_kernel<<<(unsigned)blocks, 256, 0, st>>>(mu, logvar, ldm, n, n_rows, d, dmu, dlogvar, ldd, acc);
+    gae_kld_kernel<<<grid_blocks((int64_t)n_rows * d, 256), 256, 0, st>>>(mu, logvar, ldm, n, n_rows, d, dmu, dlogvar, ldd, acc);
     B2_CHECK_LAUNCH("gae_kld_kernel");
   }
   gae_finish_kernel<<<1, 1, 0, st>>>(acc, loss_out);
@@ -393,12 +385,8 @@ extern "C" int b2_mse_sum_loss_grad_f32(const float* recon, const float* target,
   B2_REQUIRE(recon && target && grad && loss_out && n_elem >= 0, "b2_mse_sum_loss_grad_f32: bad arguments");
   if (n_elem == 0) return B2_OK;
   cudaStream_t st = as_stream(stream);
-  int64_t blocks = ceil_div<int64_t>(n_elem, 256 * 8);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  mse_loss_grad_kernel<<<(unsigned)blocks, 256, 0, st>>>(recon, target, ltmg_regu, regu_strength, relu_mask, grad,
-                                                         loss_out, n_elem);
+  mse_loss_grad_kernel<<<grid_blocks(n_elem, 2048), 256, 0, st>>>(recon, target, ltmg_regu, regu_strength, relu_mask, grad,
+                                                                  loss_out, n_elem);
   B2_CHECK_LAUNCH("mse_loss_grad_kernel");
   return B2_OK;
 }

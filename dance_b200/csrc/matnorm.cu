@@ -152,16 +152,13 @@ extern "C" int b2_matrix_normalize_f32(const float* X, int64_t ldx, int32_t n, i
   float* mx = mn + nv;
   float* shift = mx + nv;
   float* denom = shift + nv;
-  const int small_grid = ceil_div(nv, 256) < sm_count() * 4 ? ceil_div(nv, 256) : sm_count() * 4;
+  const unsigned small_grid = grid_blocks(nv, 256, 4);
   mn_init_kernel<<<small_grid, 256, 0, st>>>(sum, sq, mn, mx, nv);
   B2_CHECK_LAUNCH("mn_init_kernel");
   const int passes = mode == MN_STANDARDIZE ? 2 : 1;
   for (int pass = 0; pass < passes; ++pass) {
     if (axis == 1) {
-      int64_t blocks = ceil_div<int64_t>(n, 8);
-      const int64_t cap = (int64_t)sm_count() * 16;
-      if (blocks > cap) blocks = cap;
-      mn_row_stats_kernel<<<(unsigned)blocks, 256, 0, st>>>(X, ldx, n, g, pass, sum, sq, mn, mx);
+      mn_row_stats_kernel<<<grid_blocks(n, 8), 256, 0, st>>>(X, ldx, n, g, pass, sum, sq, mn, mx);
       B2_CHECK_LAUNCH("mn_row_stats_kernel");
     } else {
       if (pass == 1) {
@@ -169,21 +166,14 @@ extern "C" int b2_matrix_normalize_f32(const float* X, int64_t ldx, int32_t n, i
         B2_CHECK_LAUNCH("mn_zero_sq_kernel");
       }
       const int col_tiles = ceil_div(g, 32);
-      int splits = ceil_div(sm_count() * 4, col_tiles);
-      const int max_splits = n / 64 > 0 ? n / 64 : 1;
-      if (splits > max_splits) splits = max_splits;
-      if (splits < 1) splits = 1;
-      dim3 grid(col_tiles, splits);
+      dim3 grid(col_tiles, row_splits(col_tiles, n, 64, 4));
       mn_col_stats_kernel<<<grid, 256, 0, st>>>(X, ldx, n, g, pass, sum, sq, mn, mx);
       B2_CHECK_LAUNCH("mn_col_stats_kernel");
     }
   }
   mn_finalize_kernel<<<small_grid, 256, 0, st>>>(sum, sq, mn, mx, nv, len, mode, eps, shift, denom);
   B2_CHECK_LAUNCH("mn_finalize_kernel");
-  int64_t blocks = ceil_div<int64_t>((int64_t)n * g, 1024);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  mn_apply_kernel<<<(unsigned)blocks, 256, 0, st>>>(X, ldx, n, g, axis, shift, denom, out, ldo);
+  mn_apply_kernel<<<grid_blocks((int64_t)n * g, 1024), 256, 0, st>>>(X, ldx, n, g, axis, shift, denom, out, ldo);
   B2_CHECK_LAUNCH("mn_apply_kernel");
   return B2_OK;
 }

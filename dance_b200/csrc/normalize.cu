@@ -110,14 +110,6 @@ norm_apply_kernel(float* __restrict__ X, int64_t ldx, int32_t n, int32_t g, cons
   }
 }
 
-static unsigned warp_grid(int64_t rows) {
-  int64_t b = ceil_div<int64_t>(rows, 8);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (unsigned)b;
-}
-
 }  // namespace b2
 
 using namespace b2;
@@ -138,8 +130,8 @@ extern "C" int b2_normalize_total_log1p_f32(float* X, int64_t ldx, int32_t n, in
   const bool exclude = do_normalize && max_fraction < 1.f;
   const bool median = do_normalize && !(target_sum > 0.f);
   if (!exclude && !median) {
-    norm_apply_kernel<<<warp_grid(n), 256, 0, st>>>(X, ldx, n, g, nullptr, nullptr, target_sum, do_normalize, do_log1p,
-                                                    log_base);
+    norm_apply_kernel<<<grid_blocks(n, 8), 256, 0, st>>>(X, ldx, n, g, nullptr, nullptr, target_sum, do_normalize, do_log1p,
+                                                         log_base);
     B2_CHECK_LAUNCH("norm_apply_kernel");
     return B2_OK;
   }
@@ -159,19 +151,19 @@ extern "C" int b2_normalize_total_log1p_f32(float* X, int64_t ldx, int32_t n, in
   B2_CHECK_CUDA(cudaMemsetAsync(n_pos, 0, 64, st));
   if (exclude) {
     B2_CHECK_CUDA(cudaMemsetAsync(excl, 0, sizeof(int32_t) * (size_t)g, st));
-    norm_flag_kernel<<<warp_grid(n), 256, 0, st>>>(X, ldx, n, g, max_fraction, excl);
+    norm_flag_kernel<<<grid_blocks(n, 8), 256, 0, st>>>(X, ldx, n, g, max_fraction, excl);
     B2_CHECK_LAUNCH("norm_flag_kernel");
   }
-  norm_counts_kernel<<<warp_grid(n), 256, 0, st>>>(X, ldx, n, g, exclude ? excl : nullptr, counts,
-                                                   median ? keys : nullptr, median ? n_pos : nullptr);
+  norm_counts_kernel<<<grid_blocks(n, 8), 256, 0, st>>>(X, ldx, n, g, exclude ? excl : nullptr, counts,
+                                                        median ? keys : nullptr, median ? n_pos : nullptr);
   B2_CHECK_LAUNCH("norm_counts_kernel");
   if (median) {
     B2_CHECK_CUDA(cub::DeviceRadixSort::SortKeys(d_temp, temp, keys, sorted, (int)n, 0, 32, st));
     norm_median_kernel<<<1, 1, 0, st>>>(sorted, n_pos, target_dev);
     B2_CHECK_LAUNCH("norm_median_kernel");
   }
-  norm_apply_kernel<<<warp_grid(n), 256, 0, st>>>(X, ldx, n, g, counts, median ? target_dev : nullptr, target_sum,
-                                                  do_normalize, do_log1p, log_base);
+  norm_apply_kernel<<<grid_blocks(n, 8), 256, 0, st>>>(X, ldx, n, g, counts, median ? target_dev : nullptr, target_sum,
+                                                       do_normalize, do_log1p, log_base);
   B2_CHECK_LAUNCH("norm_apply_kernel");
   return B2_OK;
 }

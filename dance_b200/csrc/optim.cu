@@ -3,14 +3,6 @@
 
 namespace b2 {
 
-static unsigned ew_grid(int64_t n, int per_thread = 4) {
-  int64_t b = ceil_div<int64_t>(n, 256 * per_thread);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (b > cap) b = cap;
-  if (b < 1) b = 1;
-  return (unsigned)b;
-}
-
 // torch.optim.Adam single-tensor semantics (reference uses optim.Adam: scgnn2.py:301,573,850):
 //   g += wd·p ; m = β1 m + (1-β1) g ; v = β2 v + (1-β2) g² ;
 //   denom = sqrt(v)/sqrt(1-β2^t) + eps ; p -= (lr/(1-β1^t)) · m/denom
@@ -119,13 +111,11 @@ extern "C" int b2_clip_grad_norm_f32(float* grad, int64_t n, float pre_scale, fl
   B2_REQUIRE(grad && sumsq_ws && n >= 0, "b2_clip_grad_norm_f32: bad arguments");
   if (n == 0) return B2_OK;
   cudaStream_t st = as_stream(stream);
-  int64_t blocks = ceil_div<int64_t>(n, 1024);
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
+  const unsigned blocks = grid_blocks(n, 1024, 8);
   B2_CHECK_CUDA(cudaMemsetAsync(sumsq_ws, 0, sizeof(double), st));
-  sumsq_kernel<<<(unsigned)blocks, 256, 0, st>>>(grad, n, sumsq_ws);
+  sumsq_kernel<<<blocks, 256, 0, st>>>(grad, n, sumsq_ws);
   B2_CHECK_LAUNCH("sumsq_kernel");
-  clip_scale_kernel<<<(unsigned)blocks, 256, 0, st>>>(grad, n, pre_scale, max_norm, sumsq_ws, norm_out);
+  clip_scale_kernel<<<blocks, 256, 0, st>>>(grad, n, pre_scale, max_norm, sumsq_ws, norm_out);
   B2_CHECK_LAUNCH("clip_scale_kernel");
   return B2_OK;
 }
@@ -139,8 +129,8 @@ extern "C" int b2_adam_step_f32(float* param, const float* grad, float* exp_avg,
   // bias corrections are evaluated in double on the host exactly like torch (python floats)
   const double bc1 = 1.0 - pow((double)beta1, (double)step);
   const double bc2 = 1.0 - pow((double)beta2, (double)step);
-  adam_kernel<<<ew_grid(n), 256, 0, as_stream(stream)>>>(param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps,
-                                                         weight_decay, (float)bc1, (float)sqrt(bc2));
+  adam_kernel<<<grid_blocks(n, 1024), 256, 0, as_stream(stream)>>>(param, grad, exp_avg, exp_avg_sq, n, lr, beta1, beta2, eps,
+                                                                   weight_decay, (float)bc1, (float)sqrt(bc2));
   B2_CHECK_LAUNCH("adam_kernel");
   return B2_OK;
 }
@@ -150,7 +140,7 @@ extern "C" int b2_act_f32(const float* x, int64_t ldx, int64_t rows, int32_t col
   B2_REQUIRE(act >= B2_ACT_NONE && act <= B2_ACT_GELU, "b2_act_f32: unknown activation %d", act);
   if (rows == 0 || cols == 0) return B2_OK;
   B2_REQUIRE(x && y, "b2_act_f32: null pointer");
-  act_fwd_kernel<<<ew_grid(rows * cols, 1), 256, 0, as_stream(stream)>>>(x, ldx, rows, cols, act, y, ldy);
+  act_fwd_kernel<<<grid_blocks(rows * cols, 256), 256, 0, as_stream(stream)>>>(x, ldx, rows, cols, act, y, ldy);
   B2_CHECK_LAUNCH("act_fwd_kernel");
   return B2_OK;
 }
@@ -163,7 +153,7 @@ extern "C" int b2_act_bwd_f32(const float* dy, int64_t lddy, const float* y, int
   B2_REQUIRE(dy && dx, "b2_act_bwd_f32: null pointer");
   if (act == B2_ACT_GELU) B2_REQUIRE(x && ldx >= cols, "b2_act_bwd_f32: gelu needs the pre-activation x");
   else if (act != B2_ACT_NONE) B2_REQUIRE(y && ldy >= cols, "b2_act_bwd_f32: activation %d needs the output y", act);
-  act_bwd_kernel<<<ew_grid(rows * cols, 1), 256, 0, as_stream(stream)>>>(dy, lddy, y, ldy, x, ldx, rows, cols, act, dx, lddx);
+  act_bwd_kernel<<<grid_blocks(rows * cols, 256), 256, 0, as_stream(stream)>>>(dy, lddy, y, ldy, x, ldx, rows, cols, act, dx, lddx);
   B2_CHECK_LAUNCH("act_bwd_kernel");
   return B2_OK;
 }
@@ -173,7 +163,7 @@ extern "C" int b2_reparam_fwd_f32(const float* mu, const float* logvar, int64_t 
   B2_REQUIRE(mu && logvar && eps && z && n >= 0 && d > 0 && ldm >= d && lde >= d && ldz >= d,
              "b2_reparam_fwd_f32: bad arguments");
   if (n == 0) return B2_OK;
-  reparam_fwd_kernel<<<ew_grid(n * d), 256, 0, as_stream(stream)>>>(mu, logvar, ldm, eps, lde, z, ldz, n, d);
+  reparam_fwd_kernel<<<grid_blocks(n * d, 1024), 256, 0, as_stream(stream)>>>(mu, logvar, ldm, eps, lde, z, ldz, n, d);
   B2_CHECK_LAUNCH("reparam_fwd_kernel");
   return B2_OK;
 }
@@ -184,8 +174,8 @@ extern "C" int b2_reparam_bwd_f32(const float* dz, int64_t lddz, const float* lo
   B2_REQUIRE(dz && logvar && eps && dmu && dlogvar && n >= 0 && d > 0 && lddz >= d && ldm >= d && lde >= d && ldd >= d,
              "b2_reparam_bwd_f32: bad arguments");
   if (n == 0) return B2_OK;
-  reparam_bwd_kernel<<<ew_grid(n * d), 256, 0, as_stream(stream)>>>(dz, lddz, logvar, ldm, eps, lde, dmu, dlogvar, ldd,
-                                                                    n, d);
+  reparam_bwd_kernel<<<grid_blocks(n * d, 1024), 256, 0, as_stream(stream)>>>(dz, lddz, logvar, ldm, eps, lde, dmu, dlogvar, ldd,
+                                                                              n, d);
   B2_CHECK_LAUNCH("reparam_bwd_kernel");
   return B2_OK;
 }

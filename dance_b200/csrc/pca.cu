@@ -133,12 +133,8 @@ extern "C" int b2_sym_eig_jacobi_f32(float* W, float* V, int32_t g, int32_t max_
   cudaStream_t st = as_stream(stream);
   float* off_max = reinterpret_cast<float*>(workspace);
   const int m = (g + 1) / 2 * 2;
-  {
-    size_t blocks = ((size_t)g * g + 255) / 256;
-    if (blocks > (size_t)sm_count() * 16) blocks = (size_t)sm_count() * 16;
-    eye_kernel<<<(unsigned)blocks, 256, 0, st>>>(V, g);
-    B2_CHECK_LAUNCH("eye_kernel");
-  }
+  eye_kernel<<<grid_blocks((int64_t)g * g, 256), 256, 0, st>>>(V, g);
+  B2_CHECK_LAUNCH("eye_kernel");
   // One sweep = memset + (m-1) tiny launches (a few µs of work each): at g = 2000 the solver is launch-bound, so the sweep
   // is captured once into a CUDA graph and replayed; the convergence flag is read back after every replay.
   cudaGraph_t graph = nullptr;
@@ -192,9 +188,7 @@ extern "C" int b2_sym_eig_jacobi_f32(float* W, float* V, int32_t g, int32_t max_
 
 extern "C" int b2_cov_rank1_sub_f32(float* Cm, const float* mean, int32_t g, float n, void* stream) {
   B2_REQUIRE(Cm && mean && g > 0, "b2_cov_rank1_sub_f32: bad arguments");
-  size_t blocks = ((size_t)g * g + 255) / 256;
-  if (blocks > (size_t)sm_count() * 16) blocks = (size_t)sm_count() * 16;
-  rank1_sub_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(Cm, mean, g, n);
+  rank1_sub_kernel<<<grid_blocks((int64_t)g * g, 256), 256, 0, as_stream(stream)>>>(Cm, mean, g, n);
   B2_CHECK_LAUNCH("rank1_sub_kernel");
   return B2_OK;
 }
@@ -202,10 +196,7 @@ extern "C" int b2_cov_rank1_sub_f32(float* Cm, const float* mean, int32_t g, flo
 extern "C" int b2_row_center_f32(const float* X, int64_t ldx, int32_t n, int32_t g, float* out, int64_t ldo, void* stream) {
   B2_REQUIRE(X && out && n >= 0 && g > 0 && ldx >= g && ldo >= g, "b2_row_center_f32: bad arguments");
   if (n == 0) return B2_OK;
-  int64_t blocks = ceil_div<int64_t>(n, 8);
-  const int64_t cap = (int64_t)sm_count() * 16;
-  if (blocks > cap) blocks = cap;
-  row_center_kernel<<<(unsigned)blocks, 256, 0, as_stream(stream)>>>(X, ldx, n, g, out, ldo);
+  row_center_kernel<<<grid_blocks(n, 8), 256, 0, as_stream(stream)>>>(X, ldx, n, g, out, ldo);
   B2_CHECK_LAUNCH("row_center_kernel");
   return B2_OK;
 }

@@ -139,13 +139,6 @@ cellwise_mask_kernel(const float* __restrict__ X, int64_t ldx, int32_t g, float 
   }
 }
 
-int grid_cap(int64_t work_items, int per_block, int mult = 16) {
-  int64_t b = ceil_div<int64_t>(work_items, per_block);
-  const int64_t cap = (int64_t)sm_count() * mult;
-  if (b > cap) b = cap;
-  return (int)(b < 1 ? 1 : b);
-}
-
 }  // namespace
 }  // namespace b2
 
@@ -173,7 +166,7 @@ extern "C" int b2_cell_stats_f32(const float* X, int64_t ldx, int64_t n, int32_t
   using namespace b2;
   B2_REQUIRE(X && sum && n >= 0 && g > 0 && ldx >= g, "b2_cell_stats_f32: bad arguments");
   if (n == 0) return B2_OK;
-  cell_stats_kernel<<<grid_cap(n, 8), 256, 0, as_stream(stream)>>>(X, ldx, n, g, sum, nnz);
+  cell_stats_kernel<<<grid_blocks(n, 8), 256, 0, as_stream(stream)>>>(X, ldx, n, g, sum, nnz);
   B2_CHECK_LAUNCH("cell_stats_kernel");
   return B2_OK;
 }
@@ -183,7 +176,7 @@ extern "C" int b2_subset_f32(const float* X, int64_t ldx, const int64_t* rows, c
   using namespace b2;
   B2_REQUIRE(X && out && n_out >= 0 && g_out >= 0 && ldo >= g_out, "b2_subset_f32: bad arguments");
   if (n_out == 0 || g_out == 0) return B2_OK;
-  subset_kernel<<<grid_cap(n_out * g_out, 256 * 4, 32), 256, 0, as_stream(stream)>>>(X, ldx, rows, cols, n_out, g_out, out, ldo);
+  subset_kernel<<<grid_blocks(n_out * g_out, 1024, 32), 256, 0, as_stream(stream)>>>(X, ldx, rows, cols, n_out, g_out, out, ldo);
   B2_CHECK_LAUNCH("subset_kernel");
   return B2_OK;
 }

@@ -316,13 +316,6 @@ concat_kernel(const float* __restrict__ left, int64_t ldl, int32_t a, const floa
   }
 }
 
-int grid_blocks(int64_t work, int per_block) {
-  int64_t b = ceil_div<int64_t>(work, per_block);
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (b > cap) b = cap;
-  return (int)(b < 1 ? 1 : b);
-}
-
 }  // namespace
 }  // namespace b2
 
@@ -366,7 +359,7 @@ extern "C" int b2_quantiles_f32(const float* base, int64_t ldb, int64_t rows, in
   sel_init_kernel<<<1, 1, 0, s>>>(st);
   B2_CHECK_LAUNCH("sel_init_kernel");
   const int64_t per_launch = (ldb == cols || rows == 1) ? n / 4 : rows * 32;
-  const int g = grid_blocks(per_launch, kHistThreads);
+  const unsigned g = grid_blocks(per_launch, kHistThreads, 8);
   radix_hist_kernel<0><<<g, kHistThreads, 0, s>>>(base, ldb, rows, cols, st, h0);
   B2_CHECK_LAUNCH("radix_hist_kernel<0>");
   radix_scan_kernel<0><<<1, kScanThreads, 0, s>>>(h0, st, plan);
@@ -430,7 +423,7 @@ extern "C" int b2_concat_scaled_f32(const float* left, int64_t ldl, int32_t a, c
   B2_REQUIRE(!scale || (workspace && workspace_bytes >= b2_concat_scaled_workspace_bytes(e)), "b2_concat_scaled_f32: workspace too small");
   if (rows == 0) return B2_OK;
   cudaStream_t s = as_stream(stream);
-  const int g = grid_blocks(rows, 1);
+  const unsigned g = grid_blocks(rows, 1, 8);
   if (scale) {
     float* sc = reinterpret_cast<float*>(workspace);
     float* sh = sc + e;

@@ -179,11 +179,7 @@ static int launch_spmm(const int32_t* rowptr, const int32_t* colidx, const float
   constexpr int RPW = 32 / G;
   const int threads = 256;
   const int64_t warps_needed = ceil_div<int64_t>(n_rows, RPW);
-  int64_t blocks = ceil_div<int64_t>(warps_needed, threads / 32);
-  const int64_t max_blocks = (int64_t)sm_count() * 64;  // grid-stride beyond this
-  if (blocks > max_blocks) blocks = max_blocks;
-  if (blocks < 1) blocks = 1;
-  spmm_csr_kernel<DT, G, VPL><<<(unsigned)blocks, threads, 0, st>>>(
+  spmm_csr_kernel<DT, G, VPL><<<grid_blocks(warps_needed, threads / 32, 64), threads, 0, st>>>(
       rowptr, colidx, vals, reinterpret_cast<const typename E::Vec*>(X), ldx / E::N, reinterpret_cast<float4*>(Y), ldy / 4, n_rows,
       F / E::N, reduce, act, bias, reinterpret_cast<uint4*>(Y16), ldy16 / 8);
   B2_CHECK_LAUNCH("spmm_csr_kernel");
@@ -277,14 +273,10 @@ extern "C" int b2_convert_f32_to_x16(const float* src, int64_t lds, void* dst, i
              (long long)ldd);
   B2_REQUIRE((reinterpret_cast<uintptr_t>(src) & 7) == 0 && (reinterpret_cast<uintptr_t>(dst) & 3) == 0, "b2_convert_f32_to_x16: alignment");
   if (rows <= 0) return B2_OK;
-  const int64_t total = rows * (cols / 2);
-  int64_t blocks = ceil_div<int64_t>(total, 256 * 4);
-  const int64_t cap = (int64_t)sm_count() * 32;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
+  const unsigned blocks = grid_blocks(rows * (cols / 2), 1024, 32);
   cudaStream_t st = as_stream(stream);
-  if (dtype == 0) convert_x16_kernel<0><<<(unsigned)blocks, 256, 0, st>>>(src, lds, reinterpret_cast<uint32_t*>(dst), ldd / 2, rows, cols / 2);
-  else convert_x16_kernel<1><<<(unsigned)blocks, 256, 0, st>>>(src, lds, reinterpret_cast<uint32_t*>(dst), ldd / 2, rows, cols / 2);
+  if (dtype == 0) convert_x16_kernel<0><<<blocks, 256, 0, st>>>(src, lds, reinterpret_cast<uint32_t*>(dst), ldd / 2, rows, cols / 2);
+  else convert_x16_kernel<1><<<blocks, 256, 0, st>>>(src, lds, reinterpret_cast<uint32_t*>(dst), ldd / 2, rows, cols / 2);
   B2_CHECK_LAUNCH("convert_x16_kernel");
   return B2_OK;
 }

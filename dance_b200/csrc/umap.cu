@@ -112,10 +112,7 @@ extern "C" int b2_umap_fuzzy_knn_f32(const int32_t* knn_idx, const float* knn_di
   if (n == 0) return B2_OK;
   cudaStream_t st = as_stream(stream);
   B2_CHECK_CUDA(cudaMemsetAsync(sum_ws, 0, sizeof(double), st));
-  int64_t blocks = ceil_div<int64_t>((int64_t)n * k, 2048);
-  const int64_t cap = (int64_t)sm_count() * 8;
-  if (blocks > cap) blocks = cap;
-  um_mean_kernel<<<(unsigned)blocks, 256, 0, st>>>(knn_dist, (int64_t)n * k, sum_ws);
+  um_mean_kernel<<<grid_blocks((int64_t)n * k, 2048, 8), 256, 0, st>>>(knn_dist, (int64_t)n * k, sum_ws);
   B2_CHECK_LAUNCH("um_mean_kernel");
   um_smooth_kernel<<<ceil_div(n, 128), 128, 0, st>>>(knn_idx, knn_dist, n, k, sum_ws, vals, sigmas, rhos);
   B2_CHECK_LAUNCH("um_smooth_kernel");

@@ -9,7 +9,10 @@ config 4, scGNN 1 M × 2 000 — is bench.py).  Device-event timed on synthetic 
             bfloat16 in the kernel, fp32 accumulate and fp32 tensors); `--precision3 tf32` gives the earlier single-pass TF32
             line, `tf32x3` the fp32-accurate one.  dtype is reported as what ran
   config 5  SpaGCN: the reference model multiplies a DENSE N × N adjacency (spagcn.py:357-363); 200 k spots would need a 160 GB
-            matrix, so the line is measured at --spots (default 20 000) on one GPU and says so
+            matrix, so the dense line (`--adjacency dense`, the default) is measured at --spots (default 20 000) on one GPU and says
+            so.  `--adjacency coords --spots 200000` runs the BASELINE size on one GPU from the spot coordinates (matrix.SpotDistance):
+            calculate_p, the AX build, a training epoch and refine, each timed; AX is checked on 64 sampled rows against an fp64
+            sum over all columns before timing; plus the dense and the coordinate AX build on the same 20 000-spot input
 
     python benchmarks/configs.py --only 1,3 [--cells3 500000] [--precision3 bf16|tf32|tf32x3]
 """
@@ -139,14 +142,100 @@ def config5(args):
             "dtype": "f32 (tf32x3 GEMMs)", "n_gpus": 1, "data": "synthetic"}
 
 
+def _spot_weights64(xy, rows, c0, c1, l):
+    from dance_b200 import ops
+    r = xy[rows]
+    D = ops.pairwise_l2_dense(torch.cat([r, xy[c0:c1]]))[:r.shape[0], r.shape[0]:].contiguous()
+    return ops.exp_adj(D, l)[0].double()
+
+
+def _check_ax_rows(xy, X, AX, l, n_check=64, chunk=8192):
+    """64 sampled rows of AX against an fp64 sum over all columns of the dense path's fp32 weights; raises on a mismatch."""
+    n = xy.shape[0]
+    rows = torch.randperm(n, generator=torch.Generator().manual_seed(1))[:n_check].to(xy.device)
+    ref = torch.zeros((n_check, X.shape[1]), dtype=torch.float64, device=xy.device)
+    scale = torch.zeros_like(ref)
+    for c0 in range(0, n, chunk):
+        W = _spot_weights64(xy, rows, c0, min(n, c0 + chunk), l)
+        ref += W @ X[c0:c0 + chunk].double()
+        scale += W @ X[c0:c0 + chunk].double().abs()
+    ratio = float(((AX[rows].double() - ref).abs() / (scale * 2.0**-21)).max())
+    if not ratio < 8.0:
+        raise RuntimeError(f"config 5 coords: AX differs from the fp64 sum by {ratio:.2f} x 2^-21 of W·|X|")
+    return ratio
+
+
+def _card():
+    import subprocess
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True)
+    return q.stdout.strip() or torch.cuda.get_device_name(0)
+
+
+def config5_coords(args):
+    from dance_b200 import ops, synth
+    from dance_b200.matrix import SpotDistance
+    from dance_b200.modules.spagcn import SimpleGCDEC, calculate_p, refine
+    n, G, l = args.spots, 5000, 150.0
+    dev = torch.device("cuda:0")
+    X = synth.expression_counts(n, G, seed=2, density=0.10, device=dev)
+    ops.normalize_total_log1p_(X, target_sum=1e4, max_fraction=1.0)
+    pcs = ops.pca(X, 50)["scores"].contiguous()
+    del X
+    xy = synth.spatial_coordinates(n, seed=2, device=dev).contiguous()
+    m = SpotDistance(xy.cpu().numpy())
+    adj = m.exp(l)
+    model = SimpleGCDEC(50, 50, device=dev)
+    model.bind(pcs, adj)
+    ax_ratio = _check_ax_rows(xy, pcs, model.AX, l)
+
+    def timed(fn, reps):
+        fn()
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            fn()
+        torch.cuda.synchronize()
+        return (time.perf_counter() - t0) / reps * 1e3
+
+    p_ms = timed(lambda: calculate_p(m, l), 3)
+    bind_ms = timed(lambda: (setattr(model, "_bound", None), model.bind(pcs, adj)), 3)
+    init = torch.randint(0, 7, (n, ), generator=torch.Generator().manual_seed(0)).numpy()
+    model.fit(pcs, adj, lr=0.005, epochs=5, opt="admin", init_labels=init, tol=0)
+    torch.cuda.synchronize()
+    s, e = _ev(), _ev()
+    epochs = 50
+    s.record()
+    model.fit(pcs, adj, lr=0.005, epochs=epochs, opt="admin", init_labels=init, tol=0)
+    e.record()
+    torch.cuda.synchronize()
+    epoch_ms = s.elapsed_time(e) / epochs
+    labels = model._labels.cpu().numpy()
+    ids = list(range(n))
+    refine_ms = timed(lambda: refine(ids, labels, m, shape="hexagon"), 1)
+    # same input at 20 000 spots: the dense bind (N×N adjacency, tensor-core GEMM) against the coordinate bind
+    k = min(n, 20_000)
+    mk = SpotDistance(m.rows[:k])
+    dense_adj = mk.exp(l).to_device()
+    small = SimpleGCDEC(50, 50, device=dev)
+    dense_bind_ms = timed(lambda: (setattr(small, "_bound", None), small.bind(pcs[:k], dense_adj)), 3)
+    coords_bind_ms = timed(lambda: (setattr(small, "_bound", None), small.bind(pcs[:k], mk.exp(l))), 3)
+    return {"config": 5, "workload": f"SpaGCN SimpleGCDEC {n} spots × {G} genes → 50 PCs, adjacency from the spot coordinates "
+                                     "(SpotDistance, no N×N matrix), one GPU",
+            "metric": "spots/sec per training epoch", "value": n / (epoch_ms / 1e3), "unit": "spots/s", "ms_per_epoch": epoch_ms,
+            "calculate_p_ms": p_ms, "adj_x_build_ms": bind_ms, "refine_ms": refine_ms, "ax_check_max_err_over_2^-21": ax_ratio,
+            f"bind_{k}_dense_ms": dense_bind_ms, f"bind_{k}_coords_ms": coords_bind_ms,
+            "dtype": "f32 (tf32x3 weighted product)", "n_gpus": 1, "data": "synthetic", "card": _card()}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--only", type=str, default="1,3,5")
     ap.add_argument("--cells3", type=int, default=500_000)
     ap.add_argument("--spots", type=int, default=20_000)
     ap.add_argument("--precision3", choices=sorted(DTYPE3), default="bf16", help="GEMM precision of config 3")
+    ap.add_argument("--adjacency", choices=("dense", "coords"), default="dense", help="config 5: dense N×N adjacency or spot coordinates")
     args = ap.parse_args()
-    fns = {"1": config1, "3": config3, "5": config5}
+    fns = {"1": config1, "3": config3, "5": config5 if args.adjacency == "dense" else config5_coords}
     for k in args.only.split(","):
         try:
             print(json.dumps(fns[k.strip()](args)), flush=True)

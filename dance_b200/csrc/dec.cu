@@ -6,6 +6,7 @@
 // One warp per spot; K ≤ 64 clusters, embedding width h ≤ 256.  The backward pass recomputes q (nothing N×K is kept
 // besides p) and produces dz per spot and dmu through per-block shared-memory partials + atomics.
 #include "common.cuh"
+#include "spatial_pair.cuh"
 
 namespace b2 {
 
@@ -166,8 +167,7 @@ __global__ void __launch_bounds__(256)
 exp_adj_sum_kernel(const float* __restrict__ D, int64_t total, float two_l2, double* __restrict__ acc) {
   double local = 0.0;
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-    const float d = D[t];
-    local += (double)expf(-(d * d) / two_l2);
+    local += (double)exp_adj_weight(D[t], two_l2);
   }
   local = warp_sum(local);
   if ((threadIdx.x & 31) == 0) atomicAdd(acc, local);
@@ -176,8 +176,7 @@ exp_adj_sum_kernel(const float* __restrict__ D, int64_t total, float two_l2, dou
 __global__ void __launch_bounds__(256)
 exp_adj_kernel(const float* __restrict__ D, float* __restrict__ out, int64_t total, float two_l2) {
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-    const float d = D[t];
-    out[t] = expf(-(d * d) / two_l2);   // np.exp(-1 * adj**2 / (2 * l**2)), spagcn.py:807-809
+    out[t] = exp_adj_weight(D[t], two_l2);
   }
 }
 
@@ -233,7 +232,7 @@ extern "C" int b2_exp_adj_f32(const float* D, float* out, int64_t n_elem, double
   B2_REQUIRE(D && n_elem >= 0 && l > 0.0 && (out || sum_out_dev), "b2_exp_adj_f32: bad arguments");
   if (n_elem == 0) return B2_OK;
   cudaStream_t st = as_stream(stream);
-  const float two_l2 = (float)(2.0 * (l * l));   // numpy: fp32 array / python float → the scalar is rounded to fp32
+  const float two_l2 = exp_adj_two_l2(l);
   const unsigned blocks = grid_blocks(n_elem, 2048);
   if (sum_out_dev) {
     B2_CHECK_CUDA(cudaMemsetAsync(sum_out_dev, 0, sizeof(double), st));

@@ -8,6 +8,7 @@
 // features, `argsort`, take sorted ranks 1..k.  Also the kNN inside NeighborGraph
 // (neighbor_graph.py:50-57) and StagateGraph (spatial_graph.py:147-149).
 #include "common.cuh"
+#include "spatial_pair.cuh"
 
 #include <math_constants.h>
 
@@ -256,20 +257,14 @@ knn_fallback_kernel(const float* __restrict__ X, int64_t ldx, int32_t n, int32_t
   }
 }
 
-// dense fp32 euclidean matrix, evaluated like the reference's numba kernel
-// (utils/matrix.py:100-105): (a-b)² in fp32, accumulated in fp64, sqrt, cast to fp32.
+// dense fp32 euclidean matrix, each entry pair_l2 (spatial_pair.cuh)
 __global__ void __launch_bounds__(256)
 pairwise_dense_kernel(const float* __restrict__ X, int64_t ldx, int32_t n, int32_t d, float* __restrict__ D,
                       int64_t ldd) {
   const int64_t total = (int64_t)n * n;
   for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t i = t / n, j = t % n;
-    double s = 0.0;
-    for (int c = 0; c < d; ++c) {
-      const float diff = __fsub_rn(X[i * ldx + c], X[j * ldx + c]);
-      s = __dadd_rn(s, (double)__fmul_rn(diff, diff));
-    }
-    D[i * ldd + j] = (float)sqrt(s);
+    D[i * ldd + j] = pair_l2(X + i * ldx, X + j * ldx, d);
   }
 }
 

@@ -10,6 +10,8 @@ import numpy as np
 import scipy.sparse as sp
 import torch
 
+from .matrix import SpotDistance
+
 
 class AnnDataLite:
     """Attribute bag with the AnnData field names (X, obs, var, obsm, varm, obsp, varp, layers, uns).
@@ -296,6 +298,13 @@ class Data:
             if split_name is not None:
                 raise ValueError("split_name is not supported when return_type='default'")
             return feature
+        if isinstance(feature, SpotDistance):   # handed through unmaterialised unless a torch / sparse matrix is asked for
+            if split_name is not None:
+                idx = self.get_split_idx(split_name, error_on_miss=True)
+                feature = feature[idx][:, idx] if channel_type == "obsp" else feature[idx]
+            if return_type == "numpy":
+                return feature
+            feature = feature.toarray()
         if return_type == "sparse":
             feature = sp.csr_matrix(feature)
         else:

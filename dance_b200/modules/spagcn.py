@@ -20,9 +20,10 @@ from typing import Optional, Tuple
 import numpy as np
 import torch
 
-from .. import ops
+from .. import ops, spatial_ops
 from ..engine import FlatParams
 from ..leiden import leiden, neighbor_graph
+from ..matrix import SpotDistance
 
 
 def _dev(a, device, dtype=torch.float32) -> torch.Tensor:
@@ -32,15 +33,19 @@ def _dev(a, device, dtype=torch.float32) -> torch.Tensor:
 
 
 def calculate_p(adj, l: float) -> float:
-    """``mean_i Σ_j exp(-adj_ij²/2l²) - 1`` (spagcn.py:249-251); one reduction kernel, the N×N exponentials are never stored."""
+    """``mean_i Σ_j exp(-adj_ij²/2l²) - 1`` (spagcn.py:249-251); one reduction kernel, the N×N exponentials are never stored
+    (nor, for a ``SpotDistance``, the distances)."""
     n = adj.shape[0]
-    _, acc = ops.exp_adj(adj, l, want_matrix=False, want_sum=True)
+    if isinstance(adj, SpotDistance):
+        acc = spatial_ops.spatial_exp_adj_sum(*adj.device_coords(), l)
+    else:
+        _, acc = ops.exp_adj(adj, l, want_matrix=False, want_sum=True)
     return float(acc.item()) / n - 1.0
 
 
 def search_l(p: float, adj, start: float = 0.01, end: float = 1000, tol: float = 0.01, max_run: int = 100, device="cuda"):
     """Bisection on ``l`` so that ``calculate_p(adj, l) ≈ p`` — same control flow and return values as spagcn.py:254-287."""
-    adj = _dev(adj, device)
+    adj = adj if isinstance(adj, SpotDistance) else _dev(adj, device)
     run = 0
     p_low = calculate_p(adj, start)
     p_high = calculate_p(adj, end)
@@ -72,7 +77,11 @@ def _refine_labels(pred: torch.Tensor, dis: torch.Tensor, num_nbs: int) -> torch
     relabel when the spot's own label holds fewer than num_nbs/2 of those votes and some label holds more than num_nbs/2
     (spagcn.py:322-333).  ``pred`` int64 labels in 0..K-1; ties in distance go to the lower index (the reference's quicksort
     leaves them unspecified)."""
-    idx = torch.sort(dis, dim=1, stable=True).indices[:, :num_nbs + 1]
+    return _refine_votes(pred, torch.sort(dis, dim=1, stable=True).indices[:, :num_nbs + 1], num_nbs)
+
+
+def _refine_votes(pred: torch.Tensor, idx: torch.Tensor, num_nbs: int) -> torch.Tensor:
+    """The vote of :func:`_refine_labels` given each spot's nearest spots ``idx`` [n, num_nbs + 1]."""
     votes = torch.nn.functional.one_hot(pred[idx], int(pred.max().item()) + 1).sum(1)
     self_cnt = votes.gather(1, pred.view(-1, 1)).squeeze(1)
     max_cnt, major = votes.max(1)
@@ -82,7 +91,8 @@ def _refine_labels(pred: torch.Tensor, dis: torch.Tensor, num_nbs: int) -> torch
 
 def refine(sample_id, pred, dis, shape: str = "hexagon"):
     """Optional post-processing of the domain labels (module-level ``refine`` of the reference, spagcn.py:290-334): returns the
-    refined labels as a list in ``sample_id`` order.  ``dis`` is the spot-to-spot distance matrix (numpy or tensor)."""
+    refined labels as a list in ``sample_id`` order.  ``dis`` is the spot-to-spot distance matrix (numpy, tensor or
+    ``SpotDistance``; the last ranks the same fp32 distances on the device without forming the matrix)."""
     if shape == "hexagon":
         num_nbs = 6
     elif shape == "square":
@@ -90,6 +100,10 @@ def refine(sample_id, pred, dis, shape: str = "hexagon"):
     else:
         raise ValueError("Shape not recognized, shape='hexagon' for Visium data, 'square' for ST data.")   # the reference logs and then fails on an unbound name
     labels, inv = np.unique(np.asarray(pred), return_inverse=True)
+    if isinstance(dis, SpotDistance):
+        idx = spatial_ops.spatial_nearest(*dis.device_coords(), num_nbs + 1).long()
+        out = _refine_votes(torch.as_tensor(inv, dtype=torch.int64, device=idx.device), idx, num_nbs)
+        return labels[out.cpu().numpy()].tolist()
     dis_t = (dis if isinstance(dis, torch.Tensor) else torch.as_tensor(np.ascontiguousarray(dis))).to("cuda")   # no CPU path
     out = _refine_labels(torch.as_tensor(inv, dtype=torch.int64, device=dis_t.device), dis_t, num_nbs)
     return labels[out.cpu().numpy()].tolist()
@@ -158,14 +172,25 @@ class SimpleGCDEC:
 
     # ---- graph binding ----------------------------------------------------------------------
     def bind(self, X, adj):
-        """Upload ``X`` [N, nfeat] and the dense ``adj`` [N, N] and form ``AX = adj · X`` once."""
-        key = (id(X), id(adj), _fingerprint(X), _fingerprint(adj))   # identity AND content: an in-place edit of X / adj re-binds
+        """Upload ``X`` [N, nfeat] and the dense ``adj`` [N, N] and form ``AX = adj · X`` once.  A ``SpotDistance`` ``adj`` (the
+        exponentiated form, ``l`` set) forms ``AX`` from the coordinates; its key is the coordinates' digest and ``l``."""
+        spots = isinstance(adj, SpotDistance)
+        if spots:   # identity AND content: an in-place edit of X / adj re-binds
+            key = (id(X), _fingerprint(X), adj.fingerprint())
+        else:
+            key = (id(X), id(adj), _fingerprint(X), _fingerprint(adj))
         if self._bound is not None and self._bound[0] == key:
             return
-        Xd, Ad = _dev(X, self.device), _dev(adj, self.device)
-        if Ad.shape != (Xd.shape[0], Xd.shape[0]) or Xd.shape[1] != self.nfeat:
+        Xd = _dev(X, self.device)
+        if spots and adj.l is None:
+            raise ValueError("bind: a SpotDistance adjacency must be the exponentiated form (SpaGCN.calc_adj_exp)")
+        Ad = adj if spots else _dev(adj, self.device)
+        if tuple(Ad.shape) != (Xd.shape[0], Xd.shape[0]) or Xd.shape[1] != self.nfeat:
             raise ValueError(f"bind: X {tuple(Xd.shape)} / adj {tuple(Ad.shape)} do not fit nfeat={self.nfeat}")
-        self.AX = ops.gemm(Ad, Xd, precision=self.precision)
+        if spots:
+            self.AX = spatial_ops.spatial_exp_adj_matmul(*adj.device_coords(self.device), adj.l, Xd)
+        else:
+            self.AX = ops.gemm(Ad, Xd, precision=self.precision)
         self.n = Xd.shape[0]
         self._bound = (key, X, adj)          # keeps the host objects alive so that id() stays unique
         n, h = self.n, self.nhid
@@ -298,15 +323,17 @@ class SpaGCN:
         self.model: Optional[SimpleGCDEC] = None
 
     @staticmethod
-    def preprocessing_pipeline(alpha: float = 1, beta: int = 49, dim: int = 50, log_level="INFO"):
+    def preprocessing_pipeline(alpha: float = 1, beta: int = 49, dim: int = 50, log_level="INFO", dense: bool = True):
+        """The reference's pipeline (spagcn.py:716-731); ``dense=False`` makes both graph transforms store the coordinate-backed
+        ``SpotDistance`` instead of the N×N matrices."""
         from ..transforms import AnnDataTransform, CellPCA, Compose, FilterGenesMatch, SetConfig
         from ..transforms.graph import SpaGCNGraph, SpaGCNGraph2D
         return Compose(
             FilterGenesMatch(prefixes=["ERCC", "MT-"]),
             AnnDataTransform("scanpy.pp.normalize_total", target_sum=1e4),
             AnnDataTransform("scanpy.pp.log1p"),
-            SpaGCNGraph(alpha=alpha, beta=beta),
-            SpaGCNGraph2D(),
+            SpaGCNGraph(alpha=alpha, beta=beta, dense=dense),
+            SpaGCNGraph2D(dense=dense),
             CellPCA(n_components=dim),
             SetConfig({
                 "feature_channel": ["CellPCA", "SpaGCNGraph", "SpaGCNGraph2D"],
@@ -350,7 +377,10 @@ class SpaGCN:
         return res
 
     def calc_adj_exp(self, adj) -> torch.Tensor:
-        """``exp(-adj²/(2 l²))`` on the device (spagcn.py:807-809); returns a CUDA tensor (the reference returns numpy)."""
+        """``exp(-adj²/(2 l²))`` on the device (spagcn.py:807-809); returns a CUDA tensor (the reference returns numpy), or for a
+        ``SpotDistance`` its exponentiated form, still unmaterialised."""
+        if isinstance(adj, SpotDistance):
+            return adj.exp(self.l)
         out, _ = ops.exp_adj(_dev(adj, self.device), self.l, want_matrix=True, want_sum=False)
         return out
 

@@ -4,7 +4,8 @@
 ordering (genes first), edge order, weights and node data names (reference
 dance/transforms/graph/cell_feature_graph.py:12-79, incl. the ``cell_id``/``feat_id`` naming quirk :56-59).
 ``SpaGCNGraph`` / ``SpaGCNGraph2D`` (dance/transforms/graph/spatial_graph.py:13-76) produce the dense spot-to-spot
-euclidean distance matrices with the pairwise-distance kernel (``utils/matrix.py:164-180`` in the reference)."""
+euclidean distance matrices with the pairwise-distance kernel (``utils/matrix.py:164-180`` in the reference), or with
+``dense=False`` the coordinate-backed ``matrix.SpotDistance`` that SpaGCN sweeps without forming the N×N matrix."""
 from __future__ import annotations
 
 from typing import Optional
@@ -16,6 +17,7 @@ import torch
 from .. import ops
 from ..graph import GraphLite
 from ..leiden import neighbor_graph
+from ..matrix import SpotDistance
 from .base import BaseTransform
 from .cell_feature import WeightedFeaturePCA
 
@@ -76,6 +78,14 @@ def _pairwise_distance_host(x: np.ndarray) -> np.ndarray:
     return ops.pairwise_l2_dense(X).cpu().numpy()
 
 
+def _set_dense(t: BaseTransform, dense: bool):
+    """``dense=False`` stores the coordinate-backed ``SpotDistance`` instead of the N×N matrix.  It enters the repr (the dataset
+    cache key) only when False, so the default transforms keep their keys."""
+    t.dense = bool(dense)
+    if not t.dense:
+        t._DISPLAY_ATTRS = type(t)._DISPLAY_ATTRS + ("dense", )
+
+
 class SpaGCNGraph(BaseTransform):
     """Distance over (x, y, z) where z is the histology colour summary of each spot's pixel window
     (spatial_graph.py:13-62 ≡ spagcn.py:81-116).  The window means are a few thousand small uint8 slices of a host
@@ -83,10 +93,12 @@ class SpaGCNGraph(BaseTransform):
 
     _DISPLAY_ATTRS = ("alpha", "beta")
 
-    def __init__(self, alpha, beta, *, channels=("spatial", "spatial_pixel", "image"), channel_types=("obsm", "obsm", "uns"), **kwargs):
+    def __init__(self, alpha, beta, *, channels=("spatial", "spatial_pixel", "image"), channel_types=("obsm", "obsm", "uns"),
+                 dense: bool = True, **kwargs):
         super().__init__(**kwargs)
         self.alpha, self.beta = alpha, beta
         self.channels, self.channel_types = channels, channel_types
+        _set_dense(self, dense)
 
     def __call__(self, data):
         xy = data.get_feature(return_type="numpy", channel=self.channels[0], channel_type=self.channel_types[0])
@@ -113,20 +125,21 @@ class SpaGCNGraph(BaseTransform):
         depth = (depth - depth.mean()) / depth.std() * (xy.std(axis=0).max() * self.alpha)
         xyz = np.column_stack([xy, depth]).astype(np.float32)
         self.logger.info(f"coordinate variances (x, y, z): {xyz.var(axis=0)}")
-        data.data.obsp[self.out] = _pairwise_distance_host(xyz)
+        data.data.obsp[self.out] = _pairwise_distance_host(xyz) if self.dense else SpotDistance(xyz)
         return data
 
 
 class SpaGCNGraph2D(BaseTransform):
     """Distance over the pixel coordinates only (spatial_graph.py:66-76)."""
 
-    def __init__(self, *, channel: str = "spatial_pixel", **kwargs):
+    def __init__(self, *, channel: str = "spatial_pixel", dense: bool = True, **kwargs):
         super().__init__(**kwargs)
         self.channel = channel
+        _set_dense(self, dense)
 
     def __call__(self, data):
-        x = data.get_feature(channel=self.channel, channel_type="obsm", return_type="numpy")
-        data.data.obsp[self.out] = _pairwise_distance_host(x.astype(np.float32))
+        x = data.get_feature(channel=self.channel, channel_type="obsm", return_type="numpy").astype(np.float32)
+        data.data.obsp[self.out] = _pairwise_distance_host(x) if self.dense else SpotDistance(x)
         return data
 
 

@@ -493,6 +493,26 @@ int b2_sgd_momentum_step_f32(float* param, const float* grad, float* momentum_bu
 int b2_exp_adj_f32(const float* D, float* out, int64_t n_elem, double l, double* sum_out_dev, void* stream);
 
 /* ------------------------------------------------------------------------
+ * SpaGCN's spot graph from the coordinates, never forming the N×N matrices.  rows [n_rows, d] and cols [n_cols, d] are
+ * contiguous fp32 coordinate sets (1 <= d <= 4); a pair's distance D_rc and weight W_rc = exp(-D_rc²/(2 l²)) are the bits
+ * b2_pairwise_l2_dense_f32 and b2_exp_adj_f32 give for the same pair.
+ *   b2_spatial_exp_adj_mm_f32  : AX [n_rows, F] = W · X, X [n_cols, F] (tf32x3 tensor cores, ~2^-21 of W·|X|).  Replaces
+ *       adj_exp · X of GraphConvolution on calc_adj_exp's matrix (spagcn.py:337-366, 807-809).  Workspace:
+ *       b2_spatial_exp_adj_mm_workspace_bytes(n_cols, F), 16-byte aligned.
+ *   b2_spatial_exp_adj_sum_f32 : Σ_rc W_rc in fp64 (overwritten) — calculate_p / search_l (spagcn.py:249-287).
+ *   b2_spatial_nearest_f32     : idx_out [n_rows, m], 1 <= m <= 8: per row the m columns of smallest fp32 distance, ties to
+ *       the lower column index (a stable sort of the row) — the neighbours of refine (spagcn.py:290-334).
+ * ---------------------------------------------------------------------- */
+size_t b2_spatial_exp_adj_mm_workspace_bytes(int32_t n_cols, int32_t F);
+int b2_spatial_exp_adj_mm_f32(const float* rows, int32_t n_rows, const float* cols, int32_t n_cols, int32_t d, double l,
+                              const float* X, int64_t ldx, int32_t F, float* AX, int64_t ldax, void* workspace,
+                              size_t workspace_bytes, void* stream);
+int b2_spatial_exp_adj_sum_f32(const float* rows, int32_t n_rows, const float* cols, int32_t n_cols, int32_t d, double l,
+                               double* sum_out_dev, void* stream);
+int b2_spatial_nearest_f32(const float* rows, int32_t n_rows, const float* cols, int32_t n_cols, int32_t d, int32_t m,
+                           int32_t* idx_out, void* stream);
+
+/* ------------------------------------------------------------------------
  * GraphSCI (modules/single_modality/imputation/graphsci.py)
  *   b2_batchnorm_fwd/bwd_f32 : nn.BatchNorm1d over the rows of X [n, c] inside buildNetwork (:37-45); training → batch
  *       statistics (biased variance to normalise, running stats updated with momentum and the unbiased variance),

@@ -39,6 +39,16 @@ extern long long g_launch_count;   // kernels launched by this library (process-
     }                                                         \
   } while (0)
 
+// Dynamic shared memory a CTA may have on sm_90 once its kernel has opted in (227 KB; without the opt-in, 48 KB).
+constexpr size_t kMaxDynamicSmem = 227 * 1024;
+
+// Lets `kernel` launch with `bytes` of dynamic shared memory on the current device.  It raises the kernel's maximum-dynamic-
+// shared-memory attribute when a (kernel, device) needs more than it has been allowed so far, and does nothing for requests of
+// at most 48 KB (none of the opting-in kernels declares static shared memory).  The attribute belongs to the kernel as loaded
+// on one device, so each device opts in separately.  It only permits a size; the carve-out, and so the occupancy, is
+// unchanged.  Safe to call from several host threads.  Returns B2_OK or B2_ERR_CUDA.
+int allow_dynamic_smem(const void* kernel, size_t bytes);
+
 static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
 template <typename T>

@@ -203,8 +203,8 @@ extern "C" int b2_kmeans_step_f32(const float* X, int64_t ldx, int32_t n, int32_
   B2_CHECK_CUDA(cudaMemsetAsync(workspace, 0, b2_kmeans_workspace_bytes(k, d), st));
   B2_CHECK_CUDA(cudaMemsetAsync(stats, 0, 3 * sizeof(double), st));
   const size_t smem = (size_t)k * d * sizeof(float);
-  static bool attr = false;
-  if (!attr) { B2_CHECK_CUDA(cudaFuncSetAttribute(kmeans_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)); attr = true; }
+  const int rc = allow_dynamic_smem((const void*)kmeans_assign_kernel, smem);
+  if (rc != B2_OK) return rc;
   kmeans_assign_kernel<<<grid_blocks(n, 256), 256, smem, st>>>(X, ldx, n, d, C, k, labels, update ? sums : nullptr, counts, changed, stats);
   B2_CHECK_LAUNCH("kmeans_assign_kernel");
   if (update) {

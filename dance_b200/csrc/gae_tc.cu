@@ -70,7 +70,6 @@ constexpr int STAGES = 3;
 constexpr int MAX_D = 32;
 constexpr uint32_t ZS_BYTES = BT * 128; // one plane of a tile for S (K-major, 128-byte rows)
 constexpr int ZS_PLANES = 2;            // hi, lo
-constexpr size_t MAX_SMEM = 227 * 1024; // dynamic shared memory a CTA may have on sm_90
 
 static int64_t padded_n(int32_t n) { return ((int64_t)n + BT - 1) / BT * BT; }
 template <int DP> constexpr uint32_t zt_bytes() { return (uint32_t)DP * 4 * 128; }   // one plane of Z_Jᵀ: 4 atoms of DP x 128 B
@@ -94,8 +93,6 @@ struct Tiles {
 // position of column jj of a tile in the permuted order of the dZ MMA (see header)
 __host__ __device__ __forceinline__ int zt_pos(int jj) { const int q = jj & 7; return (jj & ~7) | ((q & 1) ? 4 + (q >> 1) : (q >> 1)); }
 
-__device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
-
 // z → hi / lo planes, tile by tile: ZS [tile][128 rows x 32 tf32, swizzled], ZT [tile][4 atoms][DP rows x 32 tf32, swizzled]
 template <int DP>
 __global__ void __launch_bounds__(256)
@@ -106,7 +103,7 @@ gae_split_kernel(const float* __restrict__ z, int64_t ldz, int32_t n, int32_t d,
     const int64_t row = t / DP;
     const int k = (int)(t % DP);
     const float v = (row < n && k < d) ? z[row * ldz + k] : 0.f;
-    const float h = tf32_trunc(v);
+    const float h = tf32_hi(v);
     const float l = v - h;
     const int64_t tile = row / BT;
     const int r = (int)(row % BT);
@@ -153,7 +150,7 @@ gae_split_f16_kernel(const float* __restrict__ z, int64_t ldz, int32_t n, int32_
     const int r = e / DP, k = e % DP;
     const int64_t row = row0 + r;
     const float v = load(e);
-    const float h = tf32_trunc(v);
+    const float h = tf32_hi(v);
     const size_t so = (size_t)(row / BT) * ZS_BYTES + sw128_offset32((uint32_t)(row % BT), (uint32_t)k);
     *reinterpret_cast<float*>(zs_hi + so) = h;
     *reinterpret_cast<float*>(zs_lo + so) = v - h;
@@ -180,36 +177,6 @@ struct Params {
   int n_jt;                    // J tiles
   const int* exps;             // triangle: scale exponent of each 64-row tile (zt_hi holds the fp16 blocks)
 };
-
-// tf32: the full sweep's dZ (N = DP) and S (N = JW)
-template <int N>
-__device__ __forceinline__ void mma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
-  if constexpr (N == 8) wgmma_tf32_rs_n8(d, a, b, scale_d);
-  else if constexpr (N == 16) wgmma_tf32_rs_n16(d, a, b, scale_d);
-  else wgmma_tf32_rs_n32(d, a, b, scale_d);
-}
-template <int N>
-__device__ __forceinline__ void mma_ss(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
-  if constexpr (N == 64) wgmma_tf32_ss_n64(d, a, b, scale_d);
-  else wgmma_tf32_ss_n128(d, a, b, scale_d);
-}
-
-// fp16: the triangle's dZ_I and dZ_J (N = DP and 2·DP)
-
-template <int N>
-__device__ __forceinline__ void mma_rs16(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
-  if constexpr (N == 8) wgmma_f16_rs_n8(d, a, b, scale_d);
-  else if constexpr (N == 16) wgmma_f16_rs_n16(d, a, b, scale_d);
-  else if constexpr (N == 32) wgmma_f16_rs_n32(d, a, b, scale_d);
-  else wgmma_f16_rs_n64(d, a, b, scale_d);
-}
-template <int N>
-__device__ __forceinline__ void mma_ss16(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
-  if constexpr (N == 8) wgmma_f16_ss_n8(d, a, b, scale_d);
-  else if constexpr (N == 16) wgmma_f16_ss_n16(d, a, b, scale_d);
-  else if constexpr (N == 32) wgmma_f16_ss_n32(d, a, b, scale_d);
-  else wgmma_f16_ss_n64(d, a, b, scale_d);
-}
 
 __device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
@@ -255,7 +222,7 @@ __device__ __forceinline__ float sigmoid_softplus(float (&S)[V], float (&L)[V], 
     if constexpr (F16) {
       S[v] = sg;
     } else {
-      const float hi = tf32_trunc(sg);
+      const float hi = tf32_hi(sg);
       S[v] = hi;
       L[v] = sg - hi;
     }
@@ -376,8 +343,8 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
 #pragma unroll
           for (int kk = 0; kk < 64 / 16; ++kk) {
             const uint32_t o = (uint32_t)kk * 32;
-            mma_ss16<DP>(djs, wgmma_desc_sw128(ag_lo + o), wgmma_desc_sw128(bi + o), kk > 0);
-            mma_ss16<2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + o), wgmma_desc_sw128(bi + o), kk >= NBM);
+            mma_ss<F16, DP>(djs, wgmma_desc_sw128(ag_lo + o), wgmma_desc_sw128(bi + o), kk > 0);
+            mma_ss<F16, 2 * DP>(djm[kk % NBM], wgmma_desc_sw128(ag_hi + o), wgmma_desc_sw128(bi + o), kk >= NBM);
           }
           wgmma_commit();
           wgmma_wait<0>();
@@ -439,7 +406,7 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
     const int r = e / DP, k = e % DP;
     const int row = row0 + r;
     const float v = (row < row_end && k < p.d) ? p.z[(int64_t)row * p.ldz + k] : 0.f;
-    const float h = tf32_trunc(v);
+    const float h = tf32_hi(v);
     const uint32_t o = sw128_offset32((uint32_t)r, (uint32_t)k);
     *reinterpret_cast<float*>(zi_hi + o) = h;
     *reinterpret_cast<float*>(zi_lo + o) = v - h;
@@ -501,9 +468,9 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
 #pragma unroll
     for (int kk = 0; kk < DP / 8; ++kk) {
       const uint32_t o = kk * 32;
-      mma_ss<JW>(S, wgmma_desc_sw128(ai_lo + o), wgmma_desc_sw128(bs_hi + o), kk > 0);
-      mma_ss<JW>(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_lo + o), 1);
-      mma_ss<JW>(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_hi + o), 1);
+      mma_ss<TF32, JW>(S, wgmma_desc_sw128(ai_lo + o), wgmma_desc_sw128(bs_hi + o), kk > 0);
+      mma_ss<TF32, JW>(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_lo + o), 1);
+      mma_ss<TF32, JW>(S, wgmma_desc_sw128(ai_hi + o), wgmma_desc_sw128(bs_hi + o), 1);
     }
     wgmma_commit();
   };
@@ -520,8 +487,8 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
                                  __float_as_uint(S[4 * kb + 3])};
         const uint32_t alo[4] = {__float_as_uint(L[4 * kb]), __float_as_uint(L[4 * kb + 1]), __float_as_uint(L[4 * kb + 2]),
                                  __float_as_uint(L[4 * kb + 3])};
-        mma_rs16<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + kb * 32), kb > 0);
-        mma_rs16<2 * DP>(dzm[kb % NBM], ahi, wgmma_desc_sw128(bt_hi + kb * 32), kb >= NBM);
+        mma_rs<F16, DP>(dzs, alo, wgmma_desc_sw128(bt_hi + kb * 32), kb > 0);
+        mma_rs<F16, 2 * DP>(dzm[kb % NBM], ahi, wgmma_desc_sw128(bt_hi + kb * 32), kb >= NBM);
       }
     } else {
 #pragma unroll
@@ -532,9 +499,9 @@ __device__ __forceinline__ void decoder_sweep(const Params& p) {
         const uint32_t alo[4] = {__float_as_uint(L[4 * kb]), __float_as_uint(L[4 * kb + 2]), __float_as_uint(L[4 * kb + 1]),
                                  __float_as_uint(L[4 * kb + 3])};
         const uint32_t o = (uint32_t)(kb >> 2) * ATOM + (uint32_t)(kb & 3) * 32;
-        mma_rs<DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
-        mma_rs<DP>(dzs, ahi, wgmma_desc_sw128(bt_lo + o), 1);
-        mma_rs<DP>(dzb[kb % NB], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NB);
+        mma_rs<TF32, DP>(dzs, alo, wgmma_desc_sw128(bt_hi + o), kb > 0);
+        mma_rs<TF32, DP>(dzs, ahi, wgmma_desc_sw128(bt_lo + o), 1);
+        mma_rs<TF32, DP>(dzb[kb % NB], ahi, wgmma_desc_sw128(bt_hi + o), kb >= NB);
       }
     }
     wgmma_commit();
@@ -715,12 +682,9 @@ static int launch_sweep(const Params& p, int units, cudaStream_t st) {
   if (splits < 1) splits = 1;
   auto kernel = TRI ? gae_tri_tc_kernel<DP> : gae_allpairs_tc_kernel<DP>;
   constexpr size_t smem = Tiles<DP, TRI>::SMEM;
-  static_assert(smem <= MAX_SMEM, "decoder shared memory");
-  static bool attr_set = false;
-  if (!attr_set) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  static_assert(smem <= kMaxDynamicSmem, "decoder shared memory");
+  const int rc = allow_dynamic_smem((const void*)kernel, smem);
+  if (rc != B2_OK) return rc;
   kernel<<<dim3((unsigned)units, (unsigned)splits), TRI ? TRI_THREADS : THREADS, smem, st>>>(p);
   B2_CHECK_LAUNCH(TRI ? "gae_tri_tc_kernel" : "gae_allpairs_tc_kernel");
   return B2_OK;

@@ -39,7 +39,6 @@ constexpr int THREADS = CONSUMERS + REWRITERS;
 // the CTA is launched with.
 constexpr int REWRITE_REGS = 80, CONSUMER_REGS = 208;
 constexpr int MAX_STAGES = 4;      // raw stages and plane stages, each
-constexpr int SMEM_LIMIT = 227 * 1024;
 
 enum Mode { MODE_TF32 = 0, MODE_TF32X3 = 1, MODE_BF16 = 2 };
 __host__ __device__ constexpr int plane_row_bytes(int mode) { return mode == MODE_BF16 ? BK * 2 : BK * 4; }
@@ -109,27 +108,13 @@ __device__ __forceinline__ void convert_tile(const uint8_t* raw, uint8_t* hi, ui
     const uint32_t off = sw128_offset32(r, kc * 4);
     if constexpr (MODE == MODE_TF32X3) {
       const float4 x = v[j];
-      const float4 h = make_float4(__uint_as_float(__float_as_uint(x.x) & 0xFFFFE000u), __uint_as_float(__float_as_uint(x.y) & 0xFFFFE000u),
-                                   __uint_as_float(__float_as_uint(x.z) & 0xFFFFE000u), __uint_as_float(__float_as_uint(x.w) & 0xFFFFE000u));
+      const float4 h = make_float4(tf32_hi(x.x), tf32_hi(x.y), tf32_hi(x.z), tf32_hi(x.w));
       *reinterpret_cast<float4*>(hi + off) = h;
       *reinterpret_cast<float4*>(lo + off) = make_float4(x.x - h.x, x.y - h.y, x.z - h.z, x.w - h.w);
     } else {
       *reinterpret_cast<float4*>(hi + off) = v[j];
     }
   }
-}
-
-template <int BN>
-__device__ __forceinline__ void mma_ss(float (&d)[BN / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
-  if constexpr (BN == 32) wgmma_tf32_ss_n32(d, a, b, scale_d);
-  else if constexpr (BN == 64) wgmma_tf32_ss_n64(d, a, b, scale_d);
-  else wgmma_tf32_ss_n128(d, a, b, scale_d);
-}
-template <int BN>
-__device__ __forceinline__ void mma_bf16_ss(float (&d)[BN / 2], uint64_t a, uint64_t b, uint32_t scale_d) {
-  if constexpr (BN == 32) wgmma_bf16_ss_n32(d, a, b, scale_d);
-  else if constexpr (BN == 64) wgmma_bf16_ss_n64(d, a, b, scale_d);
-  else wgmma_bf16_ss_n128(d, a, b, scale_d);
 }
 
 template <int BN, int MODE>
@@ -235,17 +220,17 @@ gemm_tc_kernel(const __grid_constant__ Params p) {
 #pragma unroll
       for (int k = 0; k < BK / 16; ++k) {
         const uint32_t ko = k * 16 * 2;
-        mma_bf16_ss<BN>(acc, wgmma_desc_sw64(ah + ko), wgmma_desc_sw64(bh + ko), (i | k) != 0);
+        mma_ss<BF16, BN>(acc, wgmma_desc_sw64(ah + ko), wgmma_desc_sw64(bh + ko), (i | k) != 0);
       }
     } else {
 #pragma unroll
       for (int k = 0; k < BK / 8; ++k) {
         const uint32_t ko = k * 8 * 4;
         if constexpr (MODE == MODE_TF32X3) {
-          mma_ss<BN>(acc_s, wgmma_desc_sw128(al + ko), wgmma_desc_sw128(bh + ko), (i | k) != 0);
-          mma_ss<BN>(acc_s, wgmma_desc_sw128(ah + ko), wgmma_desc_sw128(bl + ko), 1);
+          mma_ss<TF32, BN>(acc_s, wgmma_desc_sw128(al + ko), wgmma_desc_sw128(bh + ko), (i | k) != 0);
+          mma_ss<TF32, BN>(acc_s, wgmma_desc_sw128(ah + ko), wgmma_desc_sw128(bl + ko), 1);
         }
-        mma_ss<BN>(acc, wgmma_desc_sw128(ah + ko), wgmma_desc_sw128(bh + ko), (i | k) != 0);
+        mma_ss<TF32, BN>(acc, wgmma_desc_sw128(ah + ko), wgmma_desc_sw128(bh + ko), (i | k) != 0);
       }
     }
     wgmma_commit();
@@ -366,7 +351,7 @@ static Plan make_plan(int M, int N, int K, int mode) {
   pl.BN = N <= 32 ? 32 : (N <= 64 ? 64 : 128);
   // Two plane stages, then as many raw stages as fit (up to MAX_STAGES), then plane stages with what is left: at BN = 128
   // 2 x 64 KB planes + 3 x 32 KB raw in TF32X3, 3 x 32 KB + 4 x 32 KB in TF32, 4 x 16 KB + 4 x 32 KB in BF16.
-  const size_t budget = SMEM_LIMIT - 1024 /*align slack*/;
+  const size_t budget = kMaxDynamicSmem - 1024 /*align slack*/;
   const SmemLayout L0 = smem_layout(pl.BN, mode, 0, 2);
   pl.planes = 2;
   const size_t fit = (budget - L0.total) / L0.raw_stage;                            // ≥ 3 for every BN and mode
@@ -392,11 +377,8 @@ static Plan make_plan(int M, int N, int K, int mode) {
 
 template <int BN, int MODE>
 static int launch_gemm(const Params& p, const Plan& pl, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
-    attr_set = true;
-  }
+  const int rc = allow_dynamic_smem((const void*)gemm_tc_kernel<BN, MODE>, pl.smem);
+  if (rc != B2_OK) return rc;
   gemm_tc_kernel<BN, MODE><<<pl.tiles_m * pl.tiles_n * pl.splits, THREADS, pl.smem, st>>>(p);
   B2_CHECK_LAUNCH("gemm_tc_kernel");
   return B2_OK;

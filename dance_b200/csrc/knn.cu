@@ -328,16 +328,14 @@ extern "C" int b2_knn_l2_f32(const float* X, int64_t ldx, int32_t n, int32_t d, 
     else if (rc != B2_ERR_UNSUPPORTED) return rc;
   }
   const unsigned grid = (unsigned)ceil_div(n_q, KQ);
-  const size_t smem = cand_smem_bytes(M);
-  if (tc_done) {
-  } else if (M == 32) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(knn_candidates_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    knn_candidates_kernel<32><<<grid, KTHREADS, smem, st>>>(X, ldx, sqn, n, d, q_begin, n_q, cand, thr);
-  } else {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(knn_candidates_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    knn_candidates_kernel<64><<<grid, KTHREADS, smem, st>>>(X, ldx, sqn, n, d, q_begin, n_q, cand, thr);
+  if (!tc_done) {
+    auto kernel = M == 32 ? knn_candidates_kernel<32> : knn_candidates_kernel<64>;
+    const size_t smem = cand_smem_bytes(M);
+    const int rc = allow_dynamic_smem((const void*)kernel, smem);
+    if (rc != B2_OK) return rc;
+    kernel<<<grid, KTHREADS, smem, st>>>(X, ldx, sqn, n, d, q_begin, n_q, cand, thr);
+    B2_CHECK_LAUNCH("knn_candidates_kernel");
   }
-  if (!tc_done) B2_CHECK_LAUNCH("knn_candidates_kernel");
   const unsigned refine_grid = grid_blocks(n_q, 8);
   if (M == 32)
     knn_refine_kernel<32><<<refine_grid, 256, 0, st>>>(X, ldx, sqn, max_sqn, n, d, k, q_begin, n_q, r0, cand, thr, err_rel, idx_out,

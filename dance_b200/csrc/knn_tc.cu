@@ -164,9 +164,9 @@ knn_candidates_tc_kernel(const __grid_constant__ Params p) {
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {             // 64 halves per atom = 4 k-steps of 16
         const uint32_t off = (uint32_t)(a * ATOM_BYTES + kk * 32);
-        wgmma_f16_ss_n64(acc, wgmma_desc_sw128(s_q_lo + off), wgmma_desc_sw128(st + off), (a | kk) != 0);
-        wgmma_f16_ss_n64(acc, wgmma_desc_sw128(s_q_hi + off), wgmma_desc_sw128(st + op_bytes + off), 1);
-        wgmma_f16_ss_n64(acc, wgmma_desc_sw128(s_q_hi + off), wgmma_desc_sw128(st + off), 1);
+        mma_ss<F16, BR>(acc, wgmma_desc_sw128(s_q_lo + off), wgmma_desc_sw128(st + off), (a | kk) != 0);
+        mma_ss<F16, BR>(acc, wgmma_desc_sw128(s_q_hi + off), wgmma_desc_sw128(st + op_bytes + off), 1);
+        mma_ss<F16, BR>(acc, wgmma_desc_sw128(s_q_hi + off), wgmma_desc_sw128(st + off), 1);
       }
     }
     wgmma_commit();
@@ -277,11 +277,8 @@ int launch(const float* X, int64_t ldx, const float* sqn, int32_t n, int32_t d, 
   p.n = n; p.n_q = n_q; p.q_begin = q_begin; p.atoms = dp / 64;
   const int op_bytes = p.atoms * ATOM_BYTES;
   const size_t smem = (size_t)(2 + 2 * STAGES) * op_bytes + (size_t)BQ * S_PITCH * 4 + 8 * (1 + STAGES) + 1024;
-  static size_t attr_smem = 0;
-  if (smem > attr_smem) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(knn_candidates_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_smem = smem;
-  }
+  const int rc = allow_dynamic_smem((const void*)knn_candidates_tc_kernel, smem);
+  if (rc != B2_OK) return rc;
   knn_candidates_tc_kernel<<<ceil_div(n_q, BQ), THREADS, smem, st>>>(p);
   B2_CHECK_LAUNCH("knn_candidates_tc_kernel");
   return B2_OK;

@@ -42,11 +42,6 @@ __device__ __forceinline__ void load_point(const float* __restrict__ p, int64_t 
   for (int c = 0; c < MAXD; ++c) x[c] = c < d ? __ldg(p + i * d + c) : 0.f;
 }
 
-__device__ __forceinline__ void split_tf32(float w, uint32_t& hi, uint32_t& lo) {
-  hi = __float_as_uint(w) & 0xFFFFE000u;
-  lo = __float_as_uint(w - __uint_as_float(hi));
-}
-
 // X[:, 0:fc] → tile t of the planes holds columns j = 32t … 32t+31 as N feature rows of 32 tf32 (K-major in j), hi then lo;
 // features f ≥ fc and columns j ≥ n_cols are zero.
 __global__ void __launch_bounds__(256)
@@ -57,21 +52,12 @@ spatial_planes_kernel(const float* __restrict__ X, int64_t ldx, int32_t n_cols, 
     const int f = (int)(e % N);
     const int64_t j = e / N;
     const float x = (j < n_cols && f < fc) ? X[j * ldx + f] : 0.f;
-    uint32_t hi, lo;
-    split_tf32(x, hi, lo);
+    const float hi = tc::tf32_hi(x);
     uint8_t* tile = planes + (j / BJ) * tile_bytes(N);
     const uint32_t off = tc::sw128_offset32((uint32_t)f, (uint32_t)(j % BJ));
-    *reinterpret_cast<uint32_t*>(tile + off) = hi;
-    *reinterpret_cast<uint32_t*>(tile + N * 128 + off) = lo;
+    *reinterpret_cast<float*>(tile + off) = hi;
+    *reinterpret_cast<float*>(tile + N * 128 + off) = x - hi;
   }
-}
-
-template <int N>
-__device__ __forceinline__ void mma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
-  if constexpr (N == 8) tc::wgmma_tf32_rs_n8(d, a, b, scale_d);
-  else if constexpr (N == 16) tc::wgmma_tf32_rs_n16(d, a, b, scale_d);
-  else if constexpr (N == 32) tc::wgmma_tf32_rs_n32(d, a, b, scale_d);
-  else tc::wgmma_tf32_rs_n64(d, a, b, scale_d);
 }
 
 template <int N>
@@ -131,8 +117,11 @@ spatial_exp_adj_mm_kernel(const float* __restrict__ rows, int32_t n_rows, const 
           w0 = exp_adj_weight(pair_l2(p0, q, MAXD), two_l2);
           w1 = exp_adj_weight(pair_l2(p1, q, MAXD), two_l2);
         }
-        split_tf32(w0, hi[ks][2 * h], lo[ks][2 * h]);
-        split_tf32(w1, hi[ks][2 * h + 1], lo[ks][2 * h + 1]);
+        const float h0 = tf32_hi(w0), h1 = tf32_hi(w1);
+        hi[ks][2 * h] = __float_as_uint(h0);
+        lo[ks][2 * h] = __float_as_uint(w0 - h0);
+        hi[ks][2 * h + 1] = __float_as_uint(h1);
+        lo[ks][2 * h + 1] = __float_as_uint(w1 - h1);
       }
   };
   // hi·hi into acc, the cross terms into acc_x; the first product of a tile overwrites (scale-d = 0), so no ordinary
@@ -147,9 +136,9 @@ spatial_exp_adj_mm_kernel(const float* __restrict__ rows, int32_t n_rows, const 
     const uint32_t bh = smem_u32(smem + s * TB), bl = bh + N * 128;
 #pragma unroll
     for (int ks = 0; ks < 4; ++ks) {
-      mma_rs<N>(acc, hi[ks], wgmma_desc_sw128(bh + ks * 32), ks != 0);
-      mma_rs<N>(acc_x, hi[ks], wgmma_desc_sw128(bl + ks * 32), ks != 0);
-      mma_rs<N>(acc_x, lo[ks], wgmma_desc_sw128(bh + ks * 32), 1);
+      mma_rs<TF32, N>(acc, hi[ks], wgmma_desc_sw128(bh + ks * 32), ks != 0);
+      mma_rs<TF32, N>(acc_x, hi[ks], wgmma_desc_sw128(bl + ks * 32), ks != 0);
+      mma_rs<TF32, N>(acc_x, lo[ks], wgmma_desc_sw128(bh + ks * 32), 1);
     }
     wgmma_commit();
   };
@@ -268,11 +257,8 @@ template <int N>
 static int launch_mm(const float* rows, int32_t n_rows, const float* cols, int32_t n_cols, int32_t d, float two_l2,
                      const uint8_t* planes, int32_t tiles, int32_t fc, float* AX, int64_t ldax, cudaStream_t st) {
   const size_t smem = STAGES * tile_bytes(N) + 16 * STAGES + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(spatial_exp_adj_mm_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
+  const int rc = allow_dynamic_smem((const void*)spatial_exp_adj_mm_kernel<N>, smem);
+  if (rc != B2_OK) return rc;
   spatial_exp_adj_mm_kernel<N><<<(unsigned)ceil_div(n_rows, BM), THREADS, smem, st>>>(rows, n_rows, cols, n_cols, d, two_l2, planes,
                                                                                        tiles, fc, AX, ldax);
   B2_CHECK_LAUNCH("spatial_exp_adj_mm_kernel");

@@ -290,12 +290,9 @@ template <int DT, int RB, int CB, bool EPI>
 int launch_stream_epi(const StreamArgs& a, cudaStream_t st) {
   const size_t smem = (size_t)SS_WARPS * SS_NG * SS_BLK * RB + (size_t)SS_WARPS * 2 * SS_NG * SS_BLK * 8 + 128;
   auto kern = spmm_stream_kernel<DT, RB, CB, EPI>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    attr_set = true;
-  }
-  int per_sm = (int)((227 * 1024) / (smem + 1024));
+  const int rc = allow_dynamic_smem((const void*)kern, smem);
+  if (rc != B2_OK) return rc;
+  int per_sm = (int)(kMaxDynamicSmem / (smem + 1024));
   if (per_sm > 2048 / (SS_WARPS * 32)) per_sm = 2048 / (SS_WARPS * 32);
   if (per_sm < 1) per_sm = 1;
   int64_t blocks = (int64_t)sm_count() * per_sm;

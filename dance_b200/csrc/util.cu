@@ -3,6 +3,10 @@
 
 #include <string.h>
 
+#include <atomic>
+#include <mutex>
+#include <unordered_map>
+
 namespace b2 {
 
 static thread_local char g_err[512] = "";
@@ -20,17 +24,39 @@ int cuda_fail(cudaError_t e, const char* what) {
   return B2_ERR_CUDA;
 }
 
+// Per-device caches (sm_count, allow_dynamic_smem) hold devices 0 .. CACHED_DEVICES - 1; a device past them is queried, or
+// opted in, on every call.
+constexpr int CACHED_DEVICES = 16;
+static bool cached_device(int dev) { return dev >= 0 && dev < CACHED_DEVICES; }
+
 int sm_count() {
-  static int cached[16] = {0};
+  static std::atomic<int> cached[CACHED_DEVICES];
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-  if (dev < 0 || dev >= 16) dev = 0;
-  if (cached[dev] == 0) {
-    int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
-    cached[dev] = n;
+  if (cached_device(dev)) {
+    const int n = cached[dev].load(std::memory_order_relaxed);
+    if (n > 0) return n;
   }
-  return cached[dev];
+  int n = 0;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+  if (cached_device(dev)) cached[dev].store(n, std::memory_order_relaxed);
+  return n;
+}
+
+int allow_dynamic_smem(const void* kernel, size_t bytes) {
+  if (bytes <= 48 * 1024) return B2_OK;
+  int dev = 0;
+  B2_CHECK_CUDA(cudaGetDevice(&dev));
+  static std::mutex mu;
+  static std::unordered_map<const void*, size_t> allowed[CACHED_DEVICES];   // per device: kernel → largest size opted into
+  std::lock_guard<std::mutex> lock(mu);
+  if (cached_device(dev)) {
+    const auto it = allowed[dev].find(kernel);
+    if (it != allowed[dev].end() && it->second >= bytes) return B2_OK;
+  }
+  B2_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  if (cached_device(dev)) allowed[dev][kernel] = bytes;
+  return B2_OK;
 }
 
 const char* last_error() { return g_err; }

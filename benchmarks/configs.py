@@ -5,7 +5,8 @@ config 4, scGNN 1 M × 2 000 — is bench.py).  Device-event timed on synthetic 
             per-epoch train / validation evaluation the reference performs)
   config 2  scGNN 100 k × 2 k, k = 15: `python bench.py --cells 100000` (same step as the headline)
   config 3  GraphSCI, N cells × 3 000 genes (default N = 500 000): one training epoch of GraphSCI.train (AE + gene-graph GNN, ZINB
-            loss).  The GEMMs run in the precision BASELINE names, bf16 (`--precision3 bf16`, the default: operands rounded to
+            loss), with the training schedule GraphSCI chose for the size and the peak of torch.cuda.max_memory_allocated()
+            over the whole run (inputs included).  The GEMMs run in the precision BASELINE names, bf16 (`--precision3 bf16`, the default: operands rounded to
             bfloat16 in the kernel, fp32 accumulate and fp32 tensors); `--precision3 tf32` gives the earlier single-pass TF32
             line, `tf32x3` the fp32-accurate one.  dtype is reported as what ran
   config 5  SpaGCN: the reference model multiplies a DENSE N × N adjacency (spagcn.py:357-363); 200 k spots would need a 160 GB
@@ -64,12 +65,11 @@ def config1(args):
             "preprocessing_s": prep_s, "edges": int(g.num_edges()), "dtype": "f32 (tf32x3 GEMMs)", "n_gpus": 1, "data": "synthetic"}
 
 
-def config3(args):
+def config3_data(N, G=3000):
+    """Configuration 3's inputs at N cells: (X log1p counts, Xraw counts, the gene graph with Xᵀ as its node features)."""
     from dance_b200 import ops, synth
-    from dance_b200.modules.graphsci import GraphSCI
     from dance_b200.transforms import FeatureFeatureGraph
     from dance_b200.data import AnnDataLite, Data
-    N, G = args.cells3, 3000
     dev = torch.device("cuda:0")
     Xraw = synth.expression_counts(N, G, seed=1, density=0.10, device=dev)
     X = Xraw.clone()
@@ -79,12 +79,25 @@ def config3(args):
     FeatureFeatureGraph(threshold=0.05, normalize_edges=True)(sample)
     graph = sample.data.uns["FeatureFeatureGraph"]
     graph.ndata["feat"] = X.t().contiguous()       # node features of the gene graph = (log-)expression of ALL cells ([G, N], graphsci.py:126)
-    del sample
-    model = GraphSCI(num_cells=N, num_genes=G, dataset="synthetic", dropout=0.1, gpu=0, seed=0, precision=args.precision3)
+    return X, Xraw, graph
+
+
+def config3_model(N, G, X, Xraw, graph, precision):
+    from dance_b200.modules.graphsci import GraphSCI
+    model = GraphSCI(num_cells=N, num_genes=G, dataset="synthetic", dropout=0.1, gpu=0, seed=0, precision=precision)
     model._bind_graph(graph)
     n_counts = Xraw.sum(1)
     model.size_factors = (n_counts / torch.median(n_counts)).contiguous()      # what fit() sets up (graphsci.py:270-276)
     model.lr, model.weight_decay = 1e-3, 1e-5
+    return model
+
+
+def config3(args):
+    N, G = args.cells3, 3000
+    dev = torch.device("cuda:0")
+    torch.cuda.reset_peak_memory_stats()
+    X, Xraw, graph = config3_data(N, G)
+    model = config3_model(N, G, X, Xraw, graph, args.precision3)
     tm = torch.ones(N, G, dtype=torch.uint8, device=dev)
     for _ in range(2):
         model.train(X, Xraw, graph, tm, tm, le=1, la=1e-9, ke=1e2, ka=1)
@@ -99,8 +112,9 @@ def config3(args):
     ms = s.elapsed_time(e) / epochs
     return {"config": 3, "workload": f"GraphSCI {N} cells × {G} genes: one training epoch (AE + gene-graph GNN, ZINB + adjacency losses)",
             "metric": "cells/sec per training epoch", "value": N / (ms / 1e3), "unit": "cells/s", "ms_per_epoch": ms,
-            "dtype": DTYPE3[args.precision3], "n_gpus": 1,
-            "data": "synthetic", "gene_graph_edges": int(graph.num_edges())}
+            "dtype": DTYPE3[args.precision3], "n_gpus": 1, "schedule": model.schedule(),
+            "peak_memory_gib": torch.cuda.max_memory_allocated() / 2**30,
+            "data": "synthetic", "gene_graph_edges": int(graph.num_edges()), "card": _card()}
 
 
 DTYPE3 = {

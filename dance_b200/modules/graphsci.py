@@ -14,6 +14,12 @@ Model (one full-batch step = train forward → loss → eval forward for the val
 
 Randomness (dropout masks, ε) comes from a device ``torch.Generator`` seeded with ``seed``; tests inject ε explicitly and use
 dropout = 0, which is how the fixtures were produced.
+
+Two training schedules compute the same step.  The materialising one keeps every activation, keep-mask and loss gradient
+(about 25 [cells, genes] fp32 matrices); the lean one keeps five (a scratch matrix, the multiply layer's output and the
+three heads' pre-BatchNorm outputs, which the fused heads kernel overwrites with their gradients), draws its dropout masks
+from a counter-based hash so the backward regenerates them instead of storing them, and evaluates in row chunks.
+:func:`choose_schedule` picks one from the problem size and the device's memory (DESIGN §8); :data:`SCHEDULE` forces one.
 """
 from __future__ import annotations
 
@@ -24,10 +30,39 @@ import numpy as np
 import scipy.sparse as sp
 import torch
 
-from .. import ops
+from .. import graphsci_ops, ops
 from ..engine import FlatParams
 
 H1 = H2 = 256
+HEADS = ("dec_pi", "dec_disp", "dec_mean")
+# dropout sites in the order the reference draws them: GNN (graphsci.py:118-121), then AE (:81, buildNetwork :40)
+DROP_SITES = ("feat", "h1", "h2_mean", "h2_log_std", "X", "enc.1", "enc.5", "dec_pi", "dec_disp", "dec_mean")
+
+# Training schedule: "auto" (choose_schedule), or "materialise" / "lean" to force one (tests and benchmarks; user code never
+# needs it).
+SCHEDULE = "auto"
+# Rows per chunk of the lean schedule's evaluation forward (four [chunk, genes] fp32 buffers).
+EVAL_CHUNK_ROWS = 32768
+
+# Device memory of one train() step, in fp32 floats per cell (DESIGN §8): each schedule's own [cells, genes] matrices, those the
+# caller holds (X, Xraw, the GNN features Xᵀ, and a byte mask as a quarter), and per cell the [cells, 256] conv1 weight, its
+# gradient and two Adam moments plus about ten [cells, 256] encoder activations and gradients.
+OWN_MATRICES = {"materialise": 25, "lean": 5}
+CALLER_MATRICES = 3.25
+ROW_FLOATS = 14 * H1
+# share of the device's memory the materialising schedule may plan to use: the estimate leaves out allocator slack and the
+# [genes, genes] matrices (at 200 000 × 3 000 it is 65.8 GiB, the measured peak 69.8 GiB; DESIGN §8)
+HEADROOM = 0.85
+
+
+def schedule_bytes(schedule: str, n_cells: int, n_genes: int) -> int:
+    """Estimated device bytes of one train() step under ``schedule`` ("materialise" | "lean")."""
+    return int(4 * n_cells * ((OWN_MATRICES[schedule] + CALLER_MATRICES) * n_genes + ROW_FLOATS))
+
+
+def choose_schedule(n_cells: int, n_genes: int, device_bytes: int) -> str:
+    """"materialise" while its estimate fits in HEADROOM of ``device_bytes``, else "lean"."""
+    return "materialise" if schedule_bytes("materialise", n_cells, n_genes) <= HEADROOM * device_bytes else "lean"
 
 
 def _t(x, device, dtype=torch.float32):
@@ -68,6 +103,8 @@ class GraphSCI:
         self.unused: Dict[str, torch.Tensor] = {}
         self._init_params()
         self.gen = torch.Generator(device=self.device).manual_seed(int(seed))
+        self.drop_seed = int(seed) & 0xFFFFFFFF         # the lean schedule's dropout draws: keep(drop_seed, drop_key(site), r, c)
+        self.drop_step = 0                               # lean training steps taken: part of every dropout key
         self.best_state = None
         self.train_loss = self.valid_loss = self.loss_adj = self.loss_exp = self.kl = None
 
@@ -156,6 +193,21 @@ class GraphSCI:
         self.norm_adj = G * G / float((G * G - float(dense.sum().item())) * 2)         # (:456-457)
         self._graph_key = id(graph)
         self._graph = graph
+
+    # ---- schedule ---------------------------------------------------------------------------
+    def schedule(self) -> str:
+        """The training schedule train() / evaluate() run: :data:`SCHEDULE` unless "auto", else :func:`choose_schedule`."""
+        if SCHEDULE != "auto":
+            if SCHEDULE not in OWN_MATRICES:
+                raise ValueError(f"graphsci.SCHEDULE must be 'auto', 'materialise' or 'lean', got {SCHEDULE!r}")
+            return SCHEDULE
+        return choose_schedule(self.N, self.G, torch.cuda.get_device_properties(self.device).total_memory)
+
+    def drop_key(self, site: str, step: Optional[int] = None) -> int:
+        """Key of the lean schedule's dropout draw at ``site`` (one of :data:`DROP_SITES`) in training step ``step`` (default:
+        the step train() runs next).  ``ops.dropout(ones, p, model.drop_seed, key)`` reproduces the mask."""
+        s = self.drop_step if step is None else step
+        return s * len(DROP_SITES) + DROP_SITES.index(site)
 
     # ---- forward pieces ---------------------------------------------------------------------
     def _drop(self, x, training):
@@ -251,6 +303,7 @@ class GraphSCI:
         if mask is not None:
             mask = np.asarray(mask.cpu() if isinstance(mask, torch.Tensor) else mask).astype(bool)
             X_masked = self.maskdata(X, mask)
+            X = None          # drop this reference to the unmasked copy; a tensor the caller passed stays alive through theirs
             train_mask = np.copy(mask)
             test_idx = np.setdiff1d(np.arange(n), np.asarray(list(train_idx)))
             train_mask[test_idx] = False
@@ -260,9 +313,9 @@ class GraphSCI:
             X_masked = X
             perm = rng.permutation(np.asarray(list(train_idx)))
             tr, va = perm[:int(len(perm) * 0.9)], perm[int(len(perm) * 0.9):]
-            train_mask = np.zeros(tuple(X.shape), dtype=bool)
+            train_mask = np.zeros(tuple(X_masked.shape), dtype=bool)
             train_mask[tr] = True
-            valid_mask = np.zeros(tuple(X.shape), dtype=bool)
+            valid_mask = np.zeros(tuple(X_masked.shape), dtype=bool)
             valid_mask[va] = True
         self.train_data_masked = X_masked
         self._feat = X_masked.t().contiguous()                                         # graph.ndata["feat"] = masked.T (:270)
@@ -294,6 +347,8 @@ class GraphSCI:
         return self
 
     def train(self, train_data, train_data_raw, graph, train_mask, valid_mask, le=1, la=1, ke=1, ka=1, eps_train=None, eps_eval=None):
+        if self.schedule() == "lean":
+            return self._train_lean(train_data, train_data_raw, graph, train_mask, valid_mask, le, la, ke, ka, eps_train, eps_eval)
         self._bind_graph(graph)
         X, Xraw = train_data, train_data_raw
         G, N = self.G, self.N
@@ -377,6 +432,8 @@ class GraphSCI:
         if mask is not None and not isinstance(mask, torch.Tensor):
             mask = torch.from_numpy(np.asarray(mask).astype(bool)).to(self.device).view(torch.uint8)
         feat = self._graph_feat(graph)
+        if self.schedule() == "lean":
+            return self._evaluate_lean(X, Xraw, feat, mask, le, la, ke, ka, eps)
         z, ls, mu, _ = self._gnn_forward(feat, False, eps)
         a_pi, b_disp, c_mean, _ = self._ae_forward(X, z, False)
         acc3, _, (mean, _, _) = ops.zinb_loss_grad(a_pi, b_disp, c_mean, Xraw, self.size_factors, mask, float(le), float(ke), want_grad=False,
@@ -384,6 +441,171 @@ class GraphSCI:
         acc2, _ = ops.adj_loss_grad(z, mu, ls, self.adj, self.pos_weight, want_grad=False)
         *_, loss = self._losses(acc3, acc2, le, la, ke, ka)
         z_exp = mean * self.size_factors.view(-1, 1)
+        return loss, z, z_exp
+
+    # ---- the lean schedule --------------------------------------------------------------------
+    def _train_lean(self, X, Xraw, graph, train_mask, valid_mask, le, la, ke, ka, eps_train, eps_eval):
+        """One train() step keeping five [cells, genes] matrices: ``scratch`` (f_d [G, N] in the GNN forward, then X_d [N, G]
+        up to the dzf product, then f_d again, regenerated, for the conv1 weight gradient), ``h_d`` (the multiply layer's ReLU
+        output with the enc.1 input dropout applied in place) and the heads' ``pre`` (overwritten by their gradients; the first
+        then holds the multiply layer's gradient).  Dropout masks are hash draws (see :meth:`drop_key`), applied to the
+        gradients by drawing them again."""
+        self._bind_graph(graph)
+        G, N = self.G, self.N
+        P, Gd = self.params.p, self.params.g
+        pr, p = self.precision, self.dropout
+        drop = p > 0.0
+        keys = {site: self.drop_key(site) for site in DROP_SITES}
+
+        def dr(x, site, out=None):
+            return ops.dropout(x, p, self.drop_seed, keys[site], out=out) if drop else x
+
+        feat = self._graph_feat(graph)
+        scratch = torch.empty(N * G, dtype=torch.float32, device=self.device) if drop else None
+
+        # ---- GNN forward ----
+        f_d = dr(feat, "feat", out=scratch.view(G, N) if drop else None)
+        h1 = ops.spmm(self.An, ops.gemm(f_d, P["gnnmodel.conv1.weight"], precision=pr), act="tanh", bias=P["gnnmodel.conv1.bias"])
+        del f_d
+        S1 = ops.spmm(self.An, dr(h1, "h1"))
+        h2 = ops.gemm(S1, P["gnnmodel.conv2.weight"], bias=P["gnnmodel.conv2.bias"], act="relu", precision=pr)
+        Wm, bm = P["gnnmodel.dec_mean.weight"], P["gnnmodel.dec_mean.bias"]
+        S2a = ops.spmm(self.An, dr(h2, "h2_mean"))
+        mu = ops.gemm(S2a, Wm, bias=bm, precision=pr)
+        if drop:
+            S2b = ops.spmm(self.An, dr(h2, "h2_log_std"))
+            ls = ops.gemm(S2b, Wm, bias=bm, precision=pr)                           # dec_mean again (:129)
+        else:
+            S2b, ls = S2a, mu
+        eps = torch.randn(mu.shape, device=self.device, generator=self.gen) if eps_train is None else _t(eps_train, self.device)
+        z = ops.adj_sample(mu, ls, eps)
+
+        # ---- AE forward ----
+        zf = ops.gemm(z, P["aemodel.mul_layer.fc_layer.weight"], transB=True, precision=pr)
+        X_d = dr(X, "X", out=scratch.view(N, G) if drop else None)
+        h_d = ops.gemm(X_d, zf, bias=P["aemodel.mul_layer.bias"], act="relu", precision=pr)
+        if drop:
+            dr(h_d, "enc.1", out=h_d)
+        pre1 = ops.gemm(h_d, P["aemodel.enc.1.weight"], transB=True, bias=P["aemodel.enc.1.bias"], precision=pr)
+        out1, sm1, si1 = self._bn_fwd("enc.2", pre1, True, act="relu")
+        in2 = dr(out1, "enc.5")
+        pre2 = ops.gemm(in2, P["aemodel.enc.5.weight"], transB=True, bias=P["aemodel.enc.5.bias"], precision=pr)
+        out2, sm2, si2 = self._bn_fwd("enc.6", pre2, True, act="relu")
+        pre = [ops.gemm(dr(out2, h), P[f"aemodel.{h}.1.weight"], transB=True, bias=P[f"aemodel.{h}.1.bias"], precision=pr) for h in HEADS]
+        mean3 = torch.empty((3, G), dtype=torch.float32, device=self.device)
+        invstd3 = torch.empty_like(mean3)
+        for k, h in enumerate(HEADS):
+            b = self.bn[f"{h}.2"]
+            graphsci_ops.batchnorm_stats(pre[k], b.running_mean, b.running_var, True, 0.1, 1e-5, save_mean=mean3[k], save_invstd=invstd3[k])
+            b.num_batches_tracked += 1
+        gamma3, beta3 = self._head_affine()
+        # loss, and each pre overwritten by its gradient through the BatchNorm
+        acc3, dgamma3, dbeta3 = graphsci_ops.heads_train(pre, gamma3, beta3, mean3, invstd3, Xraw, self.size_factors, train_mask,
+                                                         float(le), float(ke))
+        for k, h in enumerate(HEADS):
+            Gd[f"aemodel.{h}.2.weight"].copy_(dgamma3[k])
+            Gd[f"aemodel.{h}.2.bias"].copy_(dbeta3[k])
+        acc2, dz_ce = ops.adj_loss_grad(z, mu, ls, self.adj, self.pos_weight, coef_ce=float(la) * self.norm_adj / G)
+        self.loss_adj, self.loss_exp, self.log_lik, self.kl, self.train_loss = self._losses(acc3, acc2, le, la, ke, ka)
+        self.valid_loss = self._evaluate_lean(X, Xraw, feat, valid_mask, le, la, ke, ka, eps_eval, want_z_exp=False)[0]
+
+        # ---- backward: AE ----
+        de2 = None
+        for k, h in enumerate(HEADS):
+            dpre = pre[k]
+            ops.gemm(dpre, dr(out2, h), transA=True, out=Gd[f"aemodel.{h}.1.weight"], precision=pr)
+            ops.colsum(dpre, out=Gd[f"aemodel.{h}.1.bias"])
+            dinp = ops.gemm(dpre, P[f"aemodel.{h}.1.weight"], precision=pr)
+            dr(dinp, h, out=dinp)
+            de2 = dinp if de2 is None else de2.add_(dinp)
+        buf = pre[0]
+        del pre, dpre
+        dpre, Gd["aemodel.enc.6.weight"], Gd["aemodel.enc.6.bias"] = self._bn_bwd(de2, out2, dict(pre=pre2, sm=sm2, si=si2), "enc.6", "relu")
+        ops.gemm(dpre, in2, transA=True, out=Gd["aemodel.enc.5.weight"], precision=pr)
+        ops.colsum(dpre, out=Gd["aemodel.enc.5.bias"])
+        dh = ops.gemm(dpre, P["aemodel.enc.5.weight"], precision=pr)
+        dr(dh, "enc.5", out=dh)
+        dpre, Gd["aemodel.enc.2.weight"], Gd["aemodel.enc.2.bias"] = self._bn_bwd(dh, out1, dict(pre=pre1, sm=sm1, si=si1), "enc.2", "relu")
+        ops.gemm(dpre, h_d, transA=True, out=Gd["aemodel.enc.1.weight"], precision=pr)
+        ops.colsum(dpre, out=Gd["aemodel.enc.1.bias"])
+        dpre0 = ops.gemm(dpre, P["aemodel.enc.1.weight"], out=buf, precision=pr)       # [N, G] in a freed head buffer
+        dr(dpre0, "enc.1", out=dpre0)
+        ops.act_bwd(dpre0, "relu", y=h_d, out=dpre0)      # h_d > 0 exactly where h0 > 0 and the element was kept
+        del h_d
+        ops.colsum(dpre0, out=Gd["aemodel.mul_layer.bias"])
+        dzf = ops.gemm(X_d, dpre0, transA=True, precision=pr)                            # [G, G]
+        del X_d, dpre0, buf
+        ops.gemm(dzf, z, transA=True, out=Gd["aemodel.mul_layer.fc_layer.weight"], precision=pr)
+        dz = ops.gemm(dzf, P["aemodel.mul_layer.fc_layer.weight"], precision=pr)
+        dz.add_(dz_ce)
+
+        # ---- backward: GNN ----
+        dmu, dls = ops.adj_reparam_bwd(dz, mu, ls, eps, coef_kl=-float(ka) * 0.5 / (N * G))
+        if not drop:
+            dmu.add_(dls)
+            ops.gemm(S2a, dmu, transA=True, out=Gd["gnnmodel.dec_mean.weight"], precision=pr)
+            ops.colsum(dmu, out=Gd["gnnmodel.dec_mean.bias"])
+            dh2 = ops.spmm(self.AnT, ops.gemm(dmu, Wm, transB=True, precision=pr))
+        else:
+            ops.gemm(S2a, dmu, transA=True, out=Gd["gnnmodel.dec_mean.weight"], precision=pr)
+            ops.gemm(S2b, dls, transA=True, out=Gd["gnnmodel.dec_mean.weight"], accumulate=True, precision=pr)
+            ops.colsum(dmu, out=Gd["gnnmodel.dec_mean.bias"])
+            ops.colsum(dls, out=Gd["gnnmodel.dec_mean.bias"], accumulate=True)
+            dh2 = ops.spmm(self.AnT, ops.gemm(dmu, Wm, transB=True, precision=pr))
+            dr(dh2, "h2_mean", out=dh2)
+            dh2.add_(dr(ops.spmm(self.AnT, ops.gemm(dls, Wm, transB=True, precision=pr)), "h2_log_std"))
+        dpre2 = ops.act_bwd(dh2, "relu", y=h2)
+        ops.gemm(S1, dpre2, transA=True, out=Gd["gnnmodel.conv2.weight"], precision=pr)
+        ops.colsum(dpre2, out=Gd["gnnmodel.conv2.bias"])
+        dh1 = ops.spmm(self.AnT, ops.gemm(dpre2, P["gnnmodel.conv2.weight"], transB=True, precision=pr))
+        dr(dh1, "h1", out=dh1)
+        dpre1 = ops.act_bwd(dh1, "tanh", y=h1)
+        ops.colsum(dpre1, out=Gd["gnnmodel.conv1.bias"])
+        dP = ops.spmm(self.AnT, dpre1)
+        f_d = dr(feat, "feat", out=scratch.view(G, N) if drop else None)                 # regenerated with the same key
+        ops.gemm(f_d, dP, transA=True, out=Gd["gnnmodel.conv1.weight"], precision=pr)
+        del f_d, scratch
+        self.drop_step += 1
+        self.params.adam_step(self.lr, weight_decay=self.weight_decay)
+        return self.train_loss
+
+    def _head_affine(self):
+        """The heads' BatchNorm γ and β packed [3, G] (order of :data:`HEADS`), as the fused heads kernels take them."""
+        P = self.params.p
+        return (torch.stack([P[f"aemodel.{h}.2.weight"] for h in HEADS]), torch.stack([P[f"aemodel.{h}.2.bias"] for h in HEADS]))
+
+    def _evaluate_lean(self, X, Xraw, feat, mask, le, la, ke, ka, eps, want_z_exp=True):
+        """Eval-mode forward + loss in row chunks of :data:`EVAL_CHUNK_ROWS` (running-statistics BatchNorm, no dropout, so rows
+        are independent).  Only z_exp (already times the size factors) is [cells, genes]; returns (loss, z_adj, z_exp | None)."""
+        P, pr, G = self.params.p, self.precision, self.G
+        z, ls, mu, _ = self._gnn_forward(feat, False, eps)
+        zf = ops.gemm(z, P["aemodel.mul_layer.fc_layer.weight"], transB=True, precision=pr)
+        mean3 = torch.empty((3, G), dtype=torch.float32, device=self.device)
+        invstd3 = torch.empty_like(mean3)
+        for k, h in enumerate(HEADS):
+            b = self.bn[f"{h}.2"]
+            graphsci_ops.batchnorm_stats(None, b.running_mean, b.running_var, False, 0.1, 1e-5, save_mean=mean3[k], save_invstd=invstd3[k])
+        gamma3, beta3 = self._head_affine()
+        n = X.shape[0]
+        rows = max(1, min(int(EVAL_CHUNK_ROWS), n))
+        z_exp = torch.empty((n, G), dtype=torch.float32, device=self.device) if want_z_exp else None
+        h0 = torch.empty((rows, G), dtype=torch.float32, device=self.device)
+        pre = [torch.empty_like(h0) for _ in HEADS]
+        acc3 = None
+        for r0 in range(0, n, rows):
+            r1 = min(n, r0 + rows)
+            m = r1 - r0
+            h = ops.gemm(X[r0:r1], zf, bias=P["aemodel.mul_layer.bias"], act="relu", out=h0[:m], precision=pr)
+            for lin, bn in (("enc.1", "enc.2"), ("enc.5", "enc.6")):
+                hp = ops.gemm(h, P[f"aemodel.{lin}.weight"], transB=True, bias=P[f"aemodel.{lin}.bias"], precision=pr)
+                h, _, _ = self._bn_fwd(bn, hp, False, act="relu")
+            for k, hd in enumerate(HEADS):
+                ops.gemm(h, P[f"aemodel.{hd}.1.weight"], transB=True, bias=P[f"aemodel.{hd}.1.bias"], out=pre[k][:m], precision=pr)
+            acc3 = graphsci_ops.heads_eval([t[:m] for t in pre], gamma3, beta3, mean3, invstd3, Xraw[r0:r1], self.size_factors[r0:r1],
+                                           None if mask is None else mask[r0:r1], acc=acc3,
+                                           z_exp=None if z_exp is None else z_exp[r0:r1])
+        acc2, _ = ops.adj_loss_grad(z, mu, ls, self.adj, self.pos_weight, want_grad=False)
+        *_, loss = self._losses(acc3, acc2, le, la, ke, ka)
         return loss, z, z_exp
 
     def _graph_feat(self, graph):

@@ -522,6 +522,17 @@ int b2_spatial_nearest_f32(const float* rows, int32_t n_rows, const float* cols,
  *       :57-63) + ZINB negative log-likelihood + reconstruction MSE over the masked entries (get_loss :463-483):
  *       acc3 = {Σ nll, Σ (mean·sf − y)², #masked}; with d_a/d_b/d_c the gradients of
  *       le·nll_mean + ke·(0.5/g)·mse_mean w.r.t. the three pre-activations.  mask: bytes [n, g] or NULL (all).
+ *   b2_batchnorm_stats_f32   : the statistics half of b2_batchnorm_fwd_f32 without the apply: save_mean / save_invstd
+ *       (training: from the batch, running stats updated; eval: from the running stats, X may be NULL).
+ *   b2_graphsci_heads_train_f32 : the three decoder heads (Linear, BatchNorm) of AEModel :101-104 fused with get_loss's ZINB /
+ *       MSE terms (:463-483), for the low-memory training schedule.  pre_pi / pre_disp / pre_mean [n, g] (common ldp) are the
+ *       heads' GEMM outputs; gamma, beta, mean, invstd, dgamma, dbeta are packed [3, g] (pi, disp, mean), mean / invstd from
+ *       b2_batchnorm_stats_f32.  BatchNorm, activations and loss stay in registers: acc3 as b2_zinb_loss_grad_f32, and each
+ *       pre_h is overwritten IN PLACE by ∂(le·nll_mean + ke·(0.5/g)·mse_mean)/∂pre_h through the BatchNorm (batch statistics);
+ *       dgamma / dbeta its affine gradients.  Two passes over the rows.  Workspace: b2_graphsci_heads_workspace_bytes(g).
+ *   b2_graphsci_heads_eval_f32 : the same heads in eval mode (running statistics, mean / invstd from b2_batchnorm_stats_f32
+ *       with training = 0) over n rows: acc3 (+)= {Σ nll, Σ mse, #masked} (accumulate = 1 adds to it, for row chunks) and,
+ *       when z_exp is given, z_exp = mean·sf (GraphSCI.evaluate :377-381).  Read-only on pre.
  *   b2_adj_sample_f32        : z = μ + exp(log_std)·ε  (torch.normal(mean, exp(log_std)) :130 with explicit noise)
  *   b2_adj_loss_grad_f32     : acc2 = {Σ_i −Σ_c w_c t_ic log_softmax(z_i)_c, Σ (1 + 2ls − μ² − e^{2ls})} (F.cross_entropy with
  *       probability targets and class weights :461, kl_adj :479-480); dz = coef_ce·∂CE_sum/∂z (optional).
@@ -540,6 +551,19 @@ int b2_zinb_loss_grad_f32(const float* a_pi, const float* b_disp, const float* c
                           const float* Y, int64_t ldy, const float* size_factors, const uint8_t* mask, int64_t ldm,
                           int32_t n, int32_t g, float le, float ke, float* d_a, float* d_b, float* d_c, int64_t ldd,
                           float* mean_out, float* disp_out, float* pi_out, int64_t ldo, double* acc3, void* stream);
+int b2_batchnorm_stats_f32(const float* X, int64_t ldx, int32_t n, int32_t c, float* running_mean, float* running_var,
+                           int training, float momentum, float eps, float* save_mean, float* save_invstd,
+                           void* workspace, size_t workspace_bytes, void* stream);
+size_t b2_graphsci_heads_workspace_bytes(int32_t g);
+int b2_graphsci_heads_train_f32(float* pre_pi, float* pre_disp, float* pre_mean, int64_t ldp, const float* gamma,
+                                const float* beta, const float* mean, const float* invstd, const float* Y, int64_t ldy,
+                                const float* size_factors, const uint8_t* mask, int64_t ldm, int32_t n, int32_t g, float le,
+                                float ke, float* dgamma, float* dbeta, double* acc3, void* workspace, size_t workspace_bytes,
+                                void* stream);
+int b2_graphsci_heads_eval_f32(const float* pre_pi, const float* pre_disp, const float* pre_mean, int64_t ldp,
+                               const float* gamma, const float* beta, const float* mean, const float* invstd, const float* Y,
+                               int64_t ldy, const float* size_factors, const uint8_t* mask, int64_t ldm, int32_t n, int32_t g,
+                               int accumulate, double* acc3, float* z_exp, int64_t ldz, void* stream);
 int b2_adj_sample_f32(const float* mu, const float* log_std, const float* eps, int64_t n_elem, float* z, void* stream);
 int b2_adj_loss_grad_f32(const float* z, const float* mu, const float* log_std, const float* target,
                          const float* class_weight, int32_t g, float coef_ce, float* dz, double* acc2, void* stream);

@@ -5,8 +5,9 @@
 //                            Σ_{j>=1} exp(-max(d_j - rho, 0)/sigma) = log2(k); floors at 1e-3 × mean distance
 //   membership strengths   : v_ij = 0 (self) | 1 (d <= rho or sigma = 0) | exp(-(d - rho)/sigma)
 //   fuzzy union            : C = A + Aᵀ - A∘Aᵀ, explicit zeros dropped, CSR with ascending columns
-// One thread per cell for the bisection (k <= 64 distances, fp64 bisection state like the numba code); the union is a
-// sorted two-list merge per row over A and Aᵀ (b2_csr_transpose provides both with ascending columns).
+// One thread per cell for the bisection when k <= 64 (fp64 bisection state like the numba code), one warp per cell above that
+// (the lanes hold the cell's distances and each bisection step's fp64 sum is a warp reduction); the union is a sorted two-list
+// merge per row over A and Aᵀ (b2_csr_transpose provides both with ascending columns).
 #include "common.cuh"
 
 #include <cub/device/device_scan.cuh>
@@ -73,6 +74,74 @@ um_smooth_kernel(const int32_t* __restrict__ knn_idx, const float* __restrict__ 
   }
 }
 
+// um_smooth_kernel for k > UM_MAXK, one warp per cell.  rho, the σ floors and the memberships are um_smooth_kernel's
+// arithmetic; only the order of each bisection step's fp64 sum differs (lanes, then a warp reduction).
+constexpr int UM_WSLOTS = 16;   // distances a lane keeps in registers (k <= 512); longer rows are read again through L1
+
+__global__ void __launch_bounds__(256)
+um_smooth_warp_kernel(const int32_t* __restrict__ knn_idx, const float* __restrict__ knn_dist, int32_t n, int32_t k,
+                      const double* __restrict__ dist_sum, float* __restrict__ vals, float* __restrict__ sigmas,
+                      float* __restrict__ rhos) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += nwarps) {
+    const float* drow = knn_dist + i * k;
+    // in row order, the same in every lane (uniform loads): the fp32 sum, the first positive distance and the largest one
+    float rho = 0.f, dmax = 0.f, dsum = 0.f;
+    float first_pos = -1.f;
+    int npos = 0;
+    for (int j = 0; j < k; ++j) {
+      const float dj = drow[j];
+      dsum += dj;
+      if (dj > 0.f) { if (npos == 0) first_pos = dj; ++npos; dmax = fmaxf(dmax, dj); }
+    }
+    if (npos >= 1) rho = first_pos;
+    else if (npos > 0) rho = dmax;
+    float dl[UM_WSLOTS];
+#pragma unroll
+    for (int u = 0; u < UM_WSLOTS; ++u) {
+      const int j = lane + 32 * u;
+      dl[u] = j < k ? drow[j] : 0.f;
+    }
+    const double target = log2((double)k);
+    double lo = 0.0, hi = CUDART_INF, mid = 1.0;
+    for (int it = 0; it < 64; ++it) {
+      double psum = 0.0;
+#pragma unroll
+      for (int u = 0; u < UM_WSLOTS; ++u) {
+        const int j = lane + 32 * u;
+        const float dd = dl[u] - rho;
+        if (j >= 1 && j < k) psum += dd > 0.f ? exp(-((double)dd / mid)) : 1.0;
+      }
+      for (int j = lane + 32 * UM_WSLOTS; j < k; j += 32) {
+        const float dd = drow[j] - rho;
+        psum += dd > 0.f ? exp(-((double)dd / mid)) : 1.0;
+      }
+      psum = warp_sum(psum);                       // xor butterfly: every lane holds the same bits
+      if (fabs(psum - target) < 1e-5) break;
+      if (psum > target) { hi = mid; mid = (lo + hi) / 2.0; }
+      else { lo = mid; if (hi == CUDART_INF) mid *= 2.0; else mid = (lo + hi) / 2.0; }
+    }
+    float sigma = (float)mid;
+    if (rho > 0.f) {
+      const float mean_i = dsum / (float)k;
+      if (sigma < 1e-3f * mean_i) sigma = 1e-3f * mean_i;
+    } else {
+      const float mean_all = (float)(dist_sum[0] / ((double)n * k));
+      if (sigma < 1e-3f * mean_all) sigma = 1e-3f * mean_all;
+    }
+    if (lane == 0) { sigmas[i] = sigma; rhos[i] = rho; }
+    for (int j = lane; j < k; j += 32) {
+      const float dj = drow[j];
+      float v;
+      if (knn_idx[i * k + j] == (int32_t)i) v = 0.f;
+      else if (dj - rho <= 0.f || sigma == 0.f) v = 1.f;
+      else v = expf(-((dj - rho) / sigma));
+      vals[i * k + j] = v;
+    }
+  }
+}
+
 // merge of row i of A and of Aᵀ (both ascending): value a + b - a·b, zeros dropped
 template <bool FILL>
 __global__ void __launch_bounds__(256)
@@ -107,15 +176,20 @@ using namespace b2;
 
 extern "C" int b2_umap_fuzzy_knn_f32(const int32_t* knn_idx, const float* knn_dist, int32_t n, int32_t k, float* vals,
                                      float* sigmas, float* rhos, double* sum_ws, void* stream) {
-  B2_REQUIRE(knn_idx && knn_dist && vals && sigmas && rhos && sum_ws && n >= 0 && k >= 2 && k <= UM_MAXK,
-             "b2_umap_fuzzy_knn_f32: bad arguments (2 <= k <= 64)");
+  B2_REQUIRE(knn_idx && knn_dist && vals && sigmas && rhos && sum_ws && n >= 0 && k >= 2,
+             "b2_umap_fuzzy_knn_f32: bad arguments (k >= 2)");
   if (n == 0) return B2_OK;
   cudaStream_t st = as_stream(stream);
   B2_CHECK_CUDA(cudaMemsetAsync(sum_ws, 0, sizeof(double), st));
   um_mean_kernel<<<grid_blocks((int64_t)n * k, 2048, 8), 256, 0, st>>>(knn_dist, (int64_t)n * k, sum_ws);
   B2_CHECK_LAUNCH("um_mean_kernel");
-  um_smooth_kernel<<<ceil_div(n, 128), 128, 0, st>>>(knn_idx, knn_dist, n, k, sum_ws, vals, sigmas, rhos);
-  B2_CHECK_LAUNCH("um_smooth_kernel");
+  if (k <= UM_MAXK) {
+    um_smooth_kernel<<<ceil_div(n, 128), 128, 0, st>>>(knn_idx, knn_dist, n, k, sum_ws, vals, sigmas, rhos);
+    B2_CHECK_LAUNCH("um_smooth_kernel");
+  } else {
+    um_smooth_warp_kernel<<<grid_blocks((int64_t)n * 32, 256), 256, 0, st>>>(knn_idx, knn_dist, n, k, sum_ws, vals, sigmas, rhos);
+    B2_CHECK_LAUNCH("um_smooth_warp_kernel");
+  }
   return B2_OK;
 }
 

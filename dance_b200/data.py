@@ -298,6 +298,10 @@ class Data:
             if split_name is not None:
                 raise ValueError("split_name is not supported when return_type='default'")
             return feature
+        if channel_type == "uns" and not (sp.issparse(feature) or isinstance(feature, (np.ndarray, torch.Tensor))):
+            # an object kept in uns (graph-sc's CellFeatureGraph) is handed over as it is: the reference indexes no uns entry by
+            # split and leaves a non-array one unconverted (data/base.py:454-467)
+            return feature
         if isinstance(feature, SpotDistance):   # handed through unmaterialised unless a torch / sparse matrix is asked for
             if split_name is not None:
                 idx = self.get_split_idx(split_name, error_on_miss=True)

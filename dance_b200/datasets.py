@@ -136,7 +136,7 @@ class ClusteringDataset(BaseDataset):
     def load_raw_data(self):
         X, types, var = _counts(synth_config())
         return AnnDataLite(X, obs={"names": np.array([str(i) for i in range(len(X))])}, var=var,
-                           obsm={"Group": pd.DataFrame({"Group": types}, index=[str(i) for i in range(len(X))])})
+                           obsm={"Group": np.asarray(types)})     # a 1-D label vector, as the reference's h5 "Y" (:428-439)
 
     def _raw_to_dance(self, adata):
         data = Data(adata, train_size="all")

@@ -47,8 +47,8 @@ class GraphSC:
     @staticmethod
     def preprocessing_pipeline(n_top_genes: int = 3000, normalize_weights: str = "log_per_cell", n_components: int = 50,
                                normalize_edges: bool = False, log_level="INFO"):
-        """graphsc.py:109-153.  The scanpy steps run through AnnDataTransform (highly_variable_genes(flavor="cell_ranger") needs
-        scanpy itself); the cell–gene graph is PCACellFeatureGraph on the device."""
+        """graphsc.py:109-153.  The scanpy steps run through AnnDataTransform, each dispatched to its device counterpart in
+        :mod:`dance_b200.transforms.pp`; the cell–gene graph is PCACellFeatureGraph on the device."""
         from ..transforms import AnnDataTransform, Compose, SetConfig
         from ..transforms.graph import PCACellFeatureGraph
         transforms = [
@@ -96,11 +96,12 @@ class GraphSC:
         return self
 
     def predict(self, x: Optional[Any] = None):
-        """KMeans(n_clusters, init="k-means++", random_state=5, n_init=10) on the device (graphsc.py:259-260), or leiden."""
+        """KMeans(n_clusters, init="k-means++", random_state=5, n_init=10) on the device (graphsc.py:259-260), or Leiden on the
+        embedding's 300-NN graph (:func:`run_leiden`)."""
         if self.cluster_method == "kmeans":
             return kmeans_fit_predict(self.z, self.n_clusters, self.device, seed=5, n_init=10).cpu().numpy().astype(np.int64)
         if self.cluster_method == "leiden":
-            return run_leiden(self.z)
+            return run_leiden(self.z, self.device)
         raise ValueError(f"Unknown clustering {self.cluster_method}, available options are: 'kmeans', 'leiden'")
 
     def get_latent(self):
@@ -122,14 +123,14 @@ class GraphSC:
         return self.score(x, y, score_func)
 
 
-def run_leiden(data):
-    """graphsc.py:273-293: scanpy neighbours (300, on X) then leiden."""
-    try:
-        import scanpy as sc
-    except ImportError as e:
-        raise NotImplementedError("cluster_method='leiden' needs scanpy and leidenalg (neighbors + leiden, graphsc.py:273-293); "
-                                  "use cluster_method='kmeans'") from e
-    adata = sc.AnnData(data)
-    sc.pp.neighbors(adata, use_rep="X", n_neighbors=300, n_pcs=0)
-    sc.tl.leiden(adata)
-    return [int(x) for x in adata.obs["leiden"].to_list()]
+def run_leiden(data, device=None):
+    """graphsc.py:568-587, ``sc.pp.neighbors(AnnData(z), use_rep="X", n_neighbors=300, n_pcs=0); sc.tl.leiden(adata)``, on the
+    device: the UMAP connectivities of the exact 300-NN graph of the rows of ``data`` (scanpy 1.10.1 ``compute_neighbors`` takes
+    ``1 + int(0.5 · n_obs)`` neighbours when 300 > n_obs), then Leiden at ``tl.leiden``'s resolution = 1 until nothing moves.
+    Returns the labels as a list of Python ints.  Label parity with leidenalg is unpinned (see :mod:`dance_b200.leiden`)."""
+    from ..leiden import leiden, neighbor_graph
+    X = torch.as_tensor(np.ascontiguousarray(data, dtype=np.float32), device=device or "cuda")
+    n_obs = X.shape[0]
+    n_neighbors = 300 if 300 <= n_obs else 1 + int(0.5 * n_obs)
+    res = leiden(neighbor_graph(X, n_neighbors), resolution=1.0, max_iterations=-1)
+    return [int(x) for x in res.labels.cpu().tolist()]

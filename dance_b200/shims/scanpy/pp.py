@@ -15,3 +15,7 @@ def filter_genes(data, *args, **kwargs):
 
 def filter_cells(data, *args, **kwargs):
     return _pp.filter_cells(data, *args, **kwargs)
+
+
+def highly_variable_genes(adata, *args, **kwargs):
+    return _pp.highly_variable_genes(adata, *args, **kwargs)

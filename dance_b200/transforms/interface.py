@@ -1,7 +1,7 @@
 """``AnnDataTransform(func, **kwargs)`` (reference dance/transforms/interface.py:9-68).  ``func`` may be a
-callable or a dotted name; the two scanpy functions on the hot path — ``scanpy.pp.normalize_total`` and
-``scanpy.pp.log1p`` — are dispatched to the GPU implementations in :mod:`dance_b200.transforms.pp`, by name,
-whether or not scanpy itself is installed."""
+callable or a dotted name; the scanpy functions the pipelines call (``scanpy.pp.normalize_total``, ``log1p``,
+``filter_genes``, ``filter_cells`` and ``highly_variable_genes``) are dispatched to the GPU implementations in
+:mod:`dance_b200.transforms.pp`, by name, whether or not scanpy itself is installed."""
 from __future__ import annotations
 
 import importlib
@@ -14,7 +14,9 @@ _GPU_DISPATCH = {"scanpy.pp.normalize_total": pp.normalize_total, "scanpy.pp.log
                  "scanpy.preprocessing._normalization.normalize_total": pp.normalize_total,
                  "scanpy.preprocessing._simple.log1p": pp.log1p,
                  "scanpy.pp.filter_genes": pp.filter_genes, "scanpy.pp.filter_cells": pp.filter_cells,
-                 "scanpy.preprocessing._simple.filter_genes": pp.filter_genes, "scanpy.preprocessing._simple.filter_cells": pp.filter_cells}
+                 "scanpy.preprocessing._simple.filter_genes": pp.filter_genes, "scanpy.preprocessing._simple.filter_cells": pp.filter_cells,
+                 "scanpy.pp.highly_variable_genes": pp.highly_variable_genes,
+                 "scanpy.preprocessing._highly_variable_genes.highly_variable_genes": pp.highly_variable_genes}
 
 
 class AnnDataTransform(BaseTransform):

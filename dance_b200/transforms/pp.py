@@ -1,6 +1,6 @@
-"""GPU counterparts of the two ``scanpy.pp`` functions the hot-path pipelines call through
-``AnnDataTransform`` (reference examples/single_modality/imputation/scgnn2.py:190,
-examples/spatial/spatial_domain/spagcn.py pipeline; transforms/normalize.py:563,618-620).
+"""GPU counterparts of the ``scanpy.pp`` functions the pipelines call through ``AnnDataTransform`` (reference
+examples/single_modality/imputation/scgnn2.py:190, examples/spatial/spatial_domain/spagcn.py pipeline,
+transforms/normalize.py:563,618-620, graph-sc's preprocessing_pipeline graphsc.py:109-153).
 Same call signature for the arguments the reference uses; they mutate ``adata.X`` in place.
 
 The matrix makes one round trip host → HBM → host per call (the AnnData contract keeps X on the host);
@@ -102,3 +102,69 @@ def _filter(data, target, min_counts, min_other, max_counts, max_other, inplace,
     else:
         data.obs[label] = number_np
         data._inplace_subset_obs(subset_np)
+
+
+_MAD_SCALE = 0.6744897501960817     # Φ⁻¹(3/4): statsmodels.robust.mad's normalising constant
+
+
+def highly_variable_genes(adata, layer=None, n_top_genes: Optional[int] = None, min_disp: float = 0.5, max_disp: float = np.inf,
+                          min_mean: float = 0.0125, max_mean: float = 3, span: float = 0.3, n_bins: int = 20, flavor: str = "seurat",
+                          subset: bool = False, inplace: bool = True, batch_key=None, check_values: bool = True):
+    """``scanpy.pp.highly_variable_genes(flavor="cell_ranger", n_top_genes=…)``, restated from scanpy 1.10.1.
+
+    One device pass (:func:`ops.gene_stats`) gives each gene's fp64 Σx and Σx² over ``adata.X``; the rest is over G values on the
+    host in float64.  Writes ``var`` columns ``highly_variable``, ``means``, ``dispersions`` and ``dispersions_norm`` (float32,
+    as scanpy casts it) and ``uns["hvg"]``; ``subset=True`` keeps the selected genes (on the device when X is resident there).
+    As in scanpy, ``n_top_genes`` makes the mean / dispersion cut-offs irrelevant.  Other flavours, ``batch_key``,
+    ``n_top_genes=None``, ``layer`` and ``inplace=False`` raise NotImplementedError."""
+    if flavor != "cell_ranger" or batch_key is not None or n_top_genes is None or layer is not None or not inplace:
+        raise NotImplementedError("only highly_variable_genes(flavor='cell_ranger', n_top_genes=…) in place on adata.X is built")
+    Xd = _to_device(adata)
+    n = Xd.shape[0]
+    s, q, _ = ops.gene_stats(Xd, want_nnz=False)
+    df = cell_ranger_hvg(s.cpu().numpy(), q.cpu().numpy(), n, n_top_genes)
+    adata.uns["hvg"] = {"flavor": flavor}
+    for key in ("highly_variable", "means", "dispersions"):
+        adata.var[key] = df[key]
+    adata.var["dispersions_norm"] = df["dispersions_norm"].astype(np.float32)
+    if subset:
+        adata._inplace_subset_var(df["highly_variable"])
+
+
+def cell_ranger_hvg(gene_sum: np.ndarray, gene_sumsq: np.ndarray, n_obs: int, n_top_genes: int) -> dict:
+    """The cell_ranger selection (float64 columns) from each gene's Σx and Σx² over ``n_obs`` cells (scanpy 1.10.1
+    ``_highly_variable_genes_single_batch`` / ``_subset_genes``):
+
+    1. ``mean``; ``var`` with ddof = 1 as ``(mean(x²) − mean²)·n/(n − 1)``; ``mean[mean == 0] = 1e-12``; ``disp = var / mean``.
+    2. Bins with edges ``[-inf, percentile(mean, 10, 15, …, 100), inf]``, right-closed like ``pd.cut``; duplicate edges raise
+       ValueError as ``pd.cut`` does.
+    3. Per bin ``median(disp)`` and ``MAD = median(|disp − median| / 0.6744897501960817)``; ``disp_norm = (disp − median) / MAD``.
+       Choice of this restatement: a bin holding one gene has MAD = 0 and its gene gets NaN (0 / 0), as NumPy gives it; a bin whose
+       genes share one dispersion likewise gets NaN.  NaN genes are never selected.
+    4. ``n = min(n_top_genes, G)``, lowered to the number of non-NaN ``disp_norm`` if that is smaller; the cut is the n-th largest
+       non-NaN ``disp_norm``, and a gene is selected when ``nan_to_num(disp_norm, nan=-inf) >= cut``."""
+    gene_sum = np.asarray(gene_sum, np.float64)
+    mean = gene_sum / n_obs
+    var = (np.asarray(gene_sumsq, np.float64) / n_obs - mean**2) * (n_obs / (n_obs - 1))
+    mean[mean == 0] = 1e-12
+    disp = var / mean
+    edges = np.r_[-np.inf, np.percentile(mean, np.arange(10, 105, 5)), np.inf]
+    if np.any(np.diff(edges) == 0):
+        raise ValueError(f"Bin edges must be unique: {edges!r}.")
+    bins = np.searchsorted(edges, mean, side="left") - 1          # (edges[b], edges[b + 1]]
+    avg = np.full(len(edges) - 1, np.nan)
+    dev = np.full(len(edges) - 1, np.nan)
+    for b in np.unique(bins):
+        d = disp[bins == b]
+        avg[b] = np.median(d)
+        dev[b] = np.median(np.abs(d - avg[b]) / _MAD_SCALE)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        disp_norm = (disp - avg[bins]) / dev[bins]
+    finite = disp_norm[~np.isnan(disp_norm)]
+    n = min(int(n_top_genes), disp_norm.size, finite.size)
+    if n == 0:
+        hv = np.zeros(disp_norm.size, bool)
+    else:
+        cut = np.sort(finite)[::-1][n - 1]
+        hv = np.nan_to_num(disp_norm, nan=-np.inf) >= cut
+    return {"highly_variable": hv, "means": mean, "dispersions": disp, "dispersions_norm": disp_norm}

@@ -238,6 +238,11 @@ int b2_reparam_bwd_f32(const float* dz, int64_t lddz, const float* logvar, int64
  *   return ranks 1..k; 1: return ranks 0..k-1.
  *   Distances are ranked in fp64 exactly like the reference; ties broken by
  *   the smaller index.
+ *   Limits: 1 <= k, k + r0 <= n (r0 = 0 with include_rank0, else 1), any d.
+ *   k + r0 + 8 <= 64 keeps per-query candidate lists; larger k runs a batched
+ *   path (tf32x3 GEMM estimate in [bq, n] blocks of at most 2 GiB, radix
+ *   select, fp64 refine) that synchronises the stream once per batch.
+ *   b2_knn_workspace_bytes gives what either path needs.
  * ---------------------------------------------------------------------- */
 size_t b2_knn_workspace_bytes(int32_t n, int32_t d, int32_t k, int32_t n_queries);
 int b2_knn_l2_f32(const float* X, int64_t ldx, int32_t n, int32_t d, int32_t k,
@@ -376,7 +381,8 @@ int b2_dropout_f32(const float* x, int64_t ldx, int64_t rows, int32_t cols, floa
 /* ------------------------------------------------------------------------
  * NeighborGraph connectivities (transforms/graph/neighbor_graph.py:50-57 → scanpy.pp.neighbors(method="umap") →
  * umap fuzzy_simplicial_set; third-party algorithm restated, see csrc/umap.cu)
- *   b2_umap_fuzzy_knn_f32 : knn_idx/knn_dist [n,k] (column 0 = the cell itself, ascending distances, 2 <= k <= 64)
+ *   b2_umap_fuzzy_knn_f32 : knn_idx/knn_dist [n,k] (column 0 = the cell itself, ascending distances, k >= 2; a thread per
+ *                           cell for k <= 64, a warp per cell above)
  *                           → membership strengths vals [n,k], sigmas [n], rhos [n]; sum_ws = one device double.
  *   b2_fuzzy_union_*      : C = A + Aᵀ - A∘Aᵀ from A and Aᵀ in CSR with ascending columns (b2_csr_transpose gives both),
  *                           zeros dropped; `count` writes rowptr_out and returns nnz (synchronises), `fill` the rest.

@@ -205,7 +205,8 @@ extern "C" int b2_dec_target_f32(const float* q, int64_t ldq, const float* colsu
 extern "C" int b2_dec_kl_grad_f32(const float* z, int64_t ldz, const float* mu, const float* p, int64_t ldp, int32_t n,
                                   int32_t K, int32_t h, float alpha, float* q_out, int64_t ldq, float* dz, int64_t lddz,
                                   float* dmu, float* loss_out, int32_t* labels_out, void* stream) {
-  B2_REQUIRE(z && mu && p && dz && dmu && loss_out && n > 0 && K > 0 && K <= DEC_MAXK && h > 0, "b2_dec_kl_grad_f32: bad arguments");
+  B2_REQUIRE(z && mu && p && dz && dmu && loss_out && n > 0 && K > 0 && K <= DEC_MAXK && h > 0 && ldz >= h && ldp >= K && lddz >= h &&
+             (!q_out || ldq >= K), "b2_dec_kl_grad_f32: bad arguments (K <= 64)");
   cudaStream_t st = as_stream(stream);
   B2_CHECK_CUDA(cudaMemsetAsync(dmu, 0, sizeof(float) * (size_t)K * h, st));
   B2_CHECK_CUDA(cudaMemsetAsync(loss_out, 0, sizeof(float), st));
